@@ -103,9 +103,9 @@ class CsrMatrix:
             _lib.check(_lib.load().pcgb_csr_set_boundary_rows(self._h, _lib.ptr(rows), rows.numel(), _lib.stream_ptr()),
                        "pcgb_csr_set_boundary_rows")
 
-    def spmv_split(self, x: torch.Tensor, with_dot: bool = False):
+    def spmv_split(self, x: torch.Tensor, with_dot: bool = False, out: torch.Tensor | None = None):
         """y = A x as two launches (interface tiles first); returns y or (y, x.y)."""
-        y = torch.empty(self.shape[0], dtype=torch.float64, device=self.device)
+        y = out if out is not None else torch.empty(self.shape[0], dtype=torch.float64, device=self.device)
         d = torch.zeros(1, dtype=torch.float64, device=self.device) if with_dot else None
         with torch.cuda.device(self.device):
             _lib.check(_lib.load().pcgb_spmv_split(self._h, _lib.ptr(x), _lib.ptr(y), _lib.ptr(d), _lib.stream_ptr()), "pcgb_spmv_split")
