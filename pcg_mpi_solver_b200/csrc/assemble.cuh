@@ -10,8 +10,12 @@
 //   2. symbolic pass, one warp per row: the columns of all incident elements are gathered into shared memory, sorted
 //      (bitonic) and compacted to the distinct ascending columns -> row lengths -> row offsets (exclusive scan);
 //   3. numeric pass, one warp per row: same column list, then for every incident element IN LIST ORDER the nd values
-//      ((s_i s_j) Ke[i][j]) Ck_e are added into the row's shared-memory accumulator at the binary-searched position
-//      (the columns of one element are distinct, so the lanes never collide) -> col / val written once, ascending.
+//      ((s_i s_j) Ke[i][j]) Ck_e are added into the row's shared-memory accumulator at the binary-searched position,
+//      in ascending j.  An element may list the same free dof twice (the host COO assembly and the EBE operator sum
+//      such repeats too); lanes of one pass that share a position are then added by the lowest of them in lane order
+//      -> col / val written once, ascending.
+// Both scans are checked against totals counted independently (atomics on the counts), so a wrong offset is reported
+// instead of being used to size or index an allocation.
 #pragma once
 #include <vector>
 
@@ -105,11 +109,13 @@ inline int exclusive_scan_i64(const int64_t *in, int64_t n, int64_t *out, cudaSt
 }
 
 // ---- incidence lists
-__global__ void k_asm_count(AsmGroup g, int64_t *__restrict__ cnt) {
+// cnt[d] += incidences of dof d; cnt[n] += all of them (the total the scan of cnt[0..n) must reach)
+__global__ void k_asm_count(AsmGroup g, int64_t n, int64_t *__restrict__ cnt) {
   const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
-  if (t >= g.ne * g.nd) return;
-  const int d = g.idx[t];
+  const int d = t < g.ne * g.nd ? g.idx[t] : -1;
   if (d >= 0) atomicAdd(reinterpret_cast<unsigned long long *>(cnt + d), 1ull);
+  const int c = __syncthreads_count(d >= 0);
+  if (threadIdx.x == 0 && c > 0) atomicAdd(reinterpret_cast<unsigned long long *>(cnt + n), (unsigned long long)c);
 }
 __global__ void k_asm_fill(AsmGroup g, int gi, const int64_t *__restrict__ inc_ptr, int64_t *__restrict__ cursor,
                            unsigned long long *__restrict__ inc) {
@@ -183,16 +189,19 @@ __device__ __forceinline__ int asm_row_columns(const AsmGroup *__restrict__ grou
 
 __global__ void __launch_bounds__(kAsmWarps * 32)
 k_asm_row_count(const AsmGroup *__restrict__ groups, const int64_t *__restrict__ inc_ptr, const unsigned long long *__restrict__ inc,
-                int64_t n, int64_t *__restrict__ rowcount, int *__restrict__ fail) {
+                int64_t n, int64_t *__restrict__ rowcount, int *__restrict__ fail) {   // rowcount[n] += sum of the row lengths
   extern __shared__ int asm_smem[];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   int *sc = asm_smem + warp * kAsmMaxCand;
+  unsigned long long sum = 0;
   for (int64_t row = blockIdx.x * (int64_t)kAsmWarps + warp; row < n; row += (int64_t)gridDim.x * kAsmWarps) {
     const int nu = asm_row_columns(groups, inc_ptr, inc, row, sc, lane);
     if (nu < 0) { if (lane == 0) *fail = 1; continue; }
     if (lane == 0) rowcount[row] = nu;
+    sum += (unsigned)nu;
     __syncwarp();
   }
+  if (lane == 0 && sum > 0) atomicAdd(reinterpret_cast<unsigned long long *>(rowcount + n), sum);
 }
 
 __global__ void __launch_bounds__(kAsmWarps * 32)
@@ -215,21 +224,36 @@ k_asm_row_fill(const AsmGroup *__restrict__ groups, const int64_t *__restrict__ 
       const int i = (int)(key & 0xffull);
       const double ck = g.ck[e];
       const bool si = g.sign != nullptr && g.sign[(int64_t)i * g.ne + e] != 0;
-      for (int j = lane; j < g.nd; j += 32) {
-        const int c = g.idx[(int64_t)j * g.ne + e];
-        if (c < 0) continue;
-        const bool sj = g.sign != nullptr && g.sign[(int64_t)j * g.ne + e] != 0;
-        double v = g.ke[i * g.nd + j];
-        if (si != sj) v = -v;            // (s_i s_j) Ke[i][j]   (pcg_solver.py:278,280)
-        v *= ck;                          // . Ck_e               (:279)
-        int lo = 0, hi = nu - 1;          // position of column c in the distinct ascending list
-        while (lo < hi) {
-          const int mid = (lo + hi) >> 1;
-          if (sc[mid] < c) lo = mid + 1; else hi = mid;
+      for (int j0 = 0; j0 < g.nd; j0 += 32) {
+        const int j = j0 + lane;
+        const int c = j < g.nd ? g.idx[(int64_t)j * g.ne + e] : -1;
+        double v = 0.0;
+        int lo = -1;                      // position of column c in the distinct ascending list, -1 = nothing to add
+        if (c >= 0) {
+          const bool sj = g.sign != nullptr && g.sign[(int64_t)j * g.ne + e] != 0;
+          v = g.ke[i * g.nd + j];
+          if (si != sj) v = -v;          // (s_i s_j) Ke[i][j]   (pcg_solver.py:278,280), times Ck_e (:279) in the fma below
+          int hi = nu - 1;
+          lo = 0;
+          while (lo < hi) {
+            const int mid = (lo + hi) >> 1;
+            if (sc[mid] < c) lo = mid + 1; else hi = mid;
+          }
         }
-        sv[lo] += v;                      // the columns of ONE element are distinct: no two lanes share `lo`
+        const unsigned peers = __match_any_sync(0xffffffffu, lo);
+        // every term enters with one rounding, sv = fma(v, Ck_e, sv), in ascending j
+        if (!__any_sync(0xffffffffu, lo >= 0 && peers != (1u << lane))) {
+          if (lo >= 0) sv[lo] = fma(v, ck, sv[lo]);   // the columns of this pass are distinct
+        } else {                          // a repeated column: its lowest lane adds the peers' terms in lane order
+          double s = lo >= 0 ? sv[lo] : 0.0;
+          for (int src = 0; src < 32; ++src) {
+            const double w = __shfl_sync(0xffffffffu, v, src);
+            if (((peers >> src) & 1u) && lo >= 0) s = fma(w, ck, s);
+          }
+          if (lo >= 0 && lane == __ffs(peers) - 1) sv[lo] = s;
+        }
+        __syncwarp();                     // a column repeated in the next pass reads this pass's sum
       }
-      __syncwarp();
     }
     const int64_t o = rowptr[row];
     for (int u = lane; u < nu; u += 32) { col[o + u] = sc[u]; val[o + u] = sv[u]; }
@@ -263,13 +287,17 @@ inline int asm_symbolic(AsmPlan &P, int64_t *d_rowptr, cudaStream_t st) {
   if (!P.groups.empty()) PCGB_AS(cudaMemcpyAsync(P.d_groups, P.groups.data(), P.groups.size() * sizeof(AsmGroup), cudaMemcpyHostToDevice, st));
   for (const AsmGroup &g : P.groups) {
     const int64_t tot = g.ne * g.nd;
-    if (tot > 0) k_asm_count<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(g, cnt);
+    if (tot > 0) k_asm_count<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(g, n, cnt);
   }
   PCGB_AS(cudaGetLastError());
   rc = exclusive_scan_i64(cnt, n, P.d_inc_ptr, st);
   if (rc != PCGB_OK) return done(rc);
+  int64_t counted = 0;
   PCGB_AS(cudaMemcpyAsync(&P.ninc, P.d_inc_ptr + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  PCGB_AS(cudaMemcpyAsync(&counted, cnt + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
   PCGB_AS(cudaStreamSynchronize(st));
+  if (P.ninc != counted)
+    return done(fail(PCGB_ERR_CUDA, "pcgb_assemble: incidence offsets end at %lld, but %lld incidences were counted", (long long)P.ninc, (long long)counted));
   PCGB_AS(cudaMalloc(&P.d_inc, std::max<size_t>((size_t)P.ninc, 1) * sizeof(unsigned long long)));
   for (size_t gi = 0; gi < P.groups.size(); ++gi) {
     const AsmGroup &g = P.groups[gi];
@@ -278,7 +306,8 @@ inline int asm_symbolic(AsmPlan &P, int64_t *d_rowptr, cudaStream_t st) {
   }
   if (n > 0) k_asm_sort_inc<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(n, P.d_inc_ptr, P.d_inc);
   PCGB_AS(cudaGetLastError());
-  // row lengths (reuses cnt), then the row offsets
+  // row lengths (reuses cnt; cnt[n] collects their sum), then the row offsets
+  PCGB_AS(cudaMemsetAsync(cnt + n, 0, sizeof(int64_t), st));
   const int smem = kAsmWarps * kAsmMaxCand * (int)sizeof(int);
   PCGB_AS(cudaFuncSetAttribute(k_asm_row_count, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   const unsigned grid = (unsigned)std::min<int64_t>((n + kAsmWarps - 1) / kAsmWarps, (int64_t)num_sms() * 16);
@@ -291,7 +320,10 @@ inline int asm_symbolic(AsmPlan &P, int64_t *d_rowptr, cudaStream_t st) {
   rc = exclusive_scan_i64(cnt, n, d_rowptr, st);
   if (rc != PCGB_OK) return done(rc);
   PCGB_AS(cudaMemcpyAsync(&P.nnz, d_rowptr + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  PCGB_AS(cudaMemcpyAsync(&counted, cnt + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
   PCGB_AS(cudaStreamSynchronize(st));
+  if (P.nnz != counted)
+    return done(fail(PCGB_ERR_CUDA, "pcgb_assemble: row offsets end at %lld, but the row lengths sum to %lld", (long long)P.nnz, (long long)counted));
 #undef PCGB_AS
   return done(PCGB_OK);
 }

@@ -200,6 +200,33 @@ def test_hex_generator_matches_oracle_assembly(cuda):
         np.testing.assert_allclose(M.data, A.data, rtol=1e-13, atol=1e-15)
 
 
+# (ng, e0, ne, material): boxes one element thick on each axis, on the clamped x = 0 face (nx = 1 there leaves one free node
+# layer) and away from it, and non-default E, nu, h
+HEX_BOXES = [
+    ((4, 3, 3), (0, 0, 0), (1, 3, 3), {}),
+    ((4, 3, 3), (2, 0, 0), (1, 3, 3), {}),
+    ((4, 3, 3), (0, 1, 0), (2, 1, 3), {}),
+    ((4, 3, 3), (1, 2, 0), (3, 1, 3), {}),
+    ((4, 3, 3), (0, 0, 2), (4, 3, 1), {}),
+    ((4, 3, 3), (1, 0, 1), (2, 3, 1), {}),
+    ((1, 1, 1), (0, 0, 0), (1, 1, 1), {}),
+    ((3, 3, 3), (1, 1, 1), (1, 1, 1), dict(E=7.5, nu=0.2, h=0.25)),
+    ((5, 4, 3), (0, 0, 0), (5, 4, 3), dict(E=210.0, nu=0.25, h=0.125)),
+    ((6, 4, 4), (2, 1, 1), (3, 2, 2), dict(E=3.5, nu=0.45, h=2.0)),
+]
+
+
+@pytest.mark.parametrize("ng, e0, ne, mat", HEX_BOXES)
+def test_hex_generator_thin_boxes_and_materials(cuda, ng, e0, ne, mat):
+    """csrc/hexgen.cuh against plain scipy assembly on thin boxes and other materials: structure exact."""
+    from pcg_mpi_solver_b200.hexmesh import HexBlock, generate_matrix
+    M = generate_matrix(HexBlock(ng, e0, ne, **mat), device=cuda).to_scipy()
+    A = R.hex_box_csr(ng, e0, ne, **mat)
+    assert M.shape == A.shape and M.nnz == A.nnz
+    assert np.array_equal(M.indptr, A.indptr) and np.array_equal(M.indices, A.indices)
+    np.testing.assert_allclose(M.data, A.data, rtol=1e-13, atol=1e-15 * np.abs(A.data).max())
+
+
 def test_hex_solve_c2_small(cuda):
     """A small instance of config C2 end to end on the device generator + solve."""
     import torch
