@@ -184,9 +184,25 @@ int pcgb_solver_destroy(pcgb_solver_t s);
 /* d_b: right-hand side Fext[LocDofEff]; d_minv: inverse diagonal (InvDiagPreCondVector0) or
  * NULL = identity (ExistDP0 False); d_w: DofWeightVector_Eff or NULL = ones;
  * d_x: in = initial guess X0, out = solution (X, or XMin on the non-converged path, :569-582).
- * d_resvec: optional device buffer of maxiter+2 doubles when record_resvec is set.          */
+ * d_resvec: optional device buffer of maxiter+2 doubles when record_resvec is set.
+ * Weights: d_w weights ||b||, every norm and z.r (:381, :462, :504-506, :532).  p.q is always the UNWEIGHTED sum of the
+ * local products p_i.(K_i p_i), fused into the operator: over several ranks that equals the reference's weighted dot of
+ * the assembled q (p is consistent on shared dofs).  On ONE rank with w != 1 the reference would weight p.q too
+ * (:487) and this solver does not, so alpha differs from the reference there; one rank has no shared dofs and its
+ * natural weights are all 1.                                                                    */
 int pcgb_solve(pcgb_solver_t s, const double *d_b, const double *d_minv, const double *d_w, double *d_x,
                const pcgb_options *opt, double *d_resvec, pcgb_result *res, void *stream);
+/* Opt-in trace of the loop (tests / debugging).  d_trace (device, NULL = off) = a 64-byte header {uint64 records
+ * produced; int32 scratch ...} followed by `capacity` records of pcgb_trace_record_bytes() bytes; records past the
+ * capacity are dropped (the header still counts them).  One record per control step, in order: the head of
+ * iteration 0, every iteration, every host verification, the head that follows a failed verification, and the
+ * finalisation.  Each holds the reduced values the step consumed (and, over several ranks, this rank's local value
+ * before the all-reduce, recomputed from the same partials) and the whole control block after the step
+ * (layout: struct PcgTraceRec, csrc/pcg_kernels.cuh).  d_snapshot (device, may be NULL) = 5*n + 3 doubles: r, p, q
+ * and the two x buffers when the loop exits, before the finalisation, then xcur, xmin, alias.  The setting stays
+ * on the handle until changed; with tracing off the solve launches exactly what it launches without this call. */
+int pcgb_solver_set_trace(pcgb_solver_t s, void *d_trace, int64_t capacity, double *d_snapshot);
+int64_t pcgb_trace_record_bytes(void);
 /* y = A x followed by the interface sum: calcMPFint (pcg_solver.py:339-342) on Eff dofs */
 int pcgb_apply(pcgb_solver_t s, const double *d_x, double *d_y, void *stream);
 

@@ -175,7 +175,7 @@ def _mpi_sum_local(vals):
     return tot
 
 
-def ref_pcg(parts, minv, tol, maxiter, nglob=None, resvec=None, exist_dp0=True, comm=None):
+def ref_pcg(parts, minv, tol, maxiter, nglob=None, resvec=None, exist_dp0=True, comm=None, trace=None, maxstag=3):
     """PCG(RefMeshPart), pcg_solver.py:356-598, for all parts in lock-step.
 
     comm: None = all parts live in this process (lock-step emulation); an oracle/spmd.ShmComm = SPMD mode, `parts`
@@ -183,8 +183,15 @@ def ref_pcg(parts, minv, tol, maxiter, nglob=None, resvec=None, exist_dp0=True, 
     parts: list of CsrPart / EbePart (fields b, x0, w).  minv: list of InvDiagPreCondVector0 per part
     (ignored when exist_dp0 is False, :446-451).  nglob: GlobNDofEff.  Returns a dict with
     X (list per part), Flag, RelRes, Iter and bookkeeping.  If `resvec` is a list, ||r|| per
-    iteration is appended (the reference has this commented out, :428-434, :520-525).
+    iteration is appended (the reference has this commented out, :428-434, :520-525).  If `trace` is a list, one dict
+    per control step is appended with the reduced values it consumed (sums before their sqrt): start (bb, r0r0), head
+    (i, ninf, rz), pq, norms (pp, xx, rr, stag), verify (rr, stop) and final (rr of the XMin residual, 0 when converged);
+    tests/pcg_shadow.py replays them.
     """
+    def _tr(step, **kv):
+        if trace is not None:
+            trace.append(dict(step=step, **kv))
+
     op = Operator(parts, comm)
     _mpi_sum = (lambda vals: comm.allreduce(_mpi_sum_local(vals))) if comm else _mpi_sum_local  # noqa: F811
     P = len(parts)
@@ -196,16 +203,20 @@ def ref_pcg(parts, minv, tol, maxiter, nglob=None, resvec=None, exist_dp0=True, 
     X = [np.array(p.x0, dtype=float) for p in parts]                   # :378-379
     XMin = [x for x in X]                                              # :380  MP_XMin = MP_X: the SAME array ...
     aliased = True                                                     # ... until the first np.array(MP_X) copy (:557)
-    n2b = np.sqrt(_mpi_sum([np.dot(Fext[k], Fext[k] * W[k]) for k in rng]))  # :381-383
+    bb = _mpi_sum([np.dot(Fext[k], Fext[k] * W[k]) for k in rng])
+    n2b = np.sqrt(bb)                                                  # :381-383
     tolb = tol * n2b                                                   # :384
     if n2b == 0:                                                       # :387-395 (returns the initial guess)
         return dict(X=X, Flag=0, RelRes=0.0, Iter=0, iMin=0, matvecs=op.matvecs, normb=0.0)
-    flag, rho, stag, moresteps, maxstag = 1, 1.0, 0, 0, 3              # :399-403
+    flag, rho, stag, moresteps = 1, 1.0, 0, 0                          # :399-402
+    maxstag = maxstag if maxstag > 0 else 3                            # MaxStagSteps = 3 (:403)
     maxmsteps = min([int(nglob / 50), 5, nglob - maxiter])             # :404
     imin, it = 0, 0                                                    # :405-406
     q0 = op.apply(X)                                                   # :411-413
     R = [Fext[k] - q0[k] for k in rng]                                 # :414
-    normr = np.sqrt(_mpi_sum([np.dot(R[k], R[k] * W[k]) for k in rng]))  # :415-416
+    r0r0 = _mpi_sum([np.dot(R[k], R[k] * W[k]) for k in rng])
+    normr = np.sqrt(r0r0)                                              # :415-416
+    _tr("start", bb=float(bb), r0r0=float(r0r0))
     normrmin = normr                                                   # :417
     normr_act = normr                                                  # :418
     if resvec is not None:
@@ -219,12 +230,14 @@ def ref_pcg(parts, minv, tol, maxiter, nglob=None, resvec=None, exist_dp0=True, 
         if exist_dp0:                                                  # :446-451
             Z = [minv[k] * R[k] for k in rng]
             if any(np.any(np.isinf(z)) for z in Z):
+                _tr("head", i=i, ninf=1.0)
                 flag = 2
                 break
         else:
             Z = R
         rho_1 = rho                                                    # :461
         rho = _mpi_sum([np.dot(Z[k], R[k] * W[k]) for k in rng])       # :462-463
+        _tr("head", i=i, ninf=0.0, rz=float(rho))
         if rho == 0 or np.isinf(rho):                                  # :467-469
             flag = 4
             break
@@ -238,6 +251,7 @@ def ref_pcg(parts, minv, tol, maxiter, nglob=None, resvec=None, exist_dp0=True, 
             Pv = [Z[k] + beta * Pv[k] for k in rng]
         Q = op.apply(Pv)                                               # :482-484
         pq = _mpi_sum([np.dot(Pv[k], Q[k] * W[k]) for k in rng])       # :487-488
+        _tr("pq", i=i, pq=float(pq))
         if pq <= 0 or np.isinf(pq):                                    # :492-498
             flag = 4
             break
@@ -254,6 +268,7 @@ def ref_pcg(parts, minv, tol, maxiter, nglob=None, resvec=None, exist_dp0=True, 
             stag += 1
         else:
             stag = 0
+        _tr("norms", i=i, pp=float(sq[0]), xx=float(sq[1]), rr=float(sq[2]), stag=stag)
         X = [X[k] + alpha * Pv[k] for k in rng]                        # :516 in place in the reference, so an XMin that is
         if aliased:                                                    #      still bound to MP_X follows the update
             XMin = X
@@ -263,7 +278,9 @@ def ref_pcg(parts, minv, tol, maxiter, nglob=None, resvec=None, exist_dp0=True, 
         if normr <= tolb or stag >= maxstag or moresteps > 0:          # :527
             fint = op.apply(X)                                         # :528-530
             R = [Fext[k] - fint[k] for k in rng]                       # :531
-            normr_act = np.sqrt(_mpi_sum([np.dot(R[k], R[k] * W[k]) for k in rng]))  # :532-533
+            rr_act = _mpi_sum([np.dot(R[k], R[k] * W[k]) for k in rng])
+            normr_act = np.sqrt(rr_act)                                # :532-533
+            _tr("verify", i=i, rr=float(rr_act), stop=True)
             if resvec is not None:
                 resvec[-1] = normr_act
             if normr_act <= tolb:                                      # :540-543
@@ -278,6 +295,8 @@ def ref_pcg(parts, minv, tol, maxiter, nglob=None, resvec=None, exist_dp0=True, 
                 flag = 3                                               #   after it (Flag=3, Iter=i) are what
                 it = i                                                 #   MATLAB does and what we report
                 break
+            if trace is not None and stag < maxstag:                   # the loop goes on after this verification
+                trace[-1]["stop"] = False
         if normr_act < normrmin:                                       # :555-558
             normrmin = normr_act
             XMin = [np.array(x) for x in X]
@@ -289,10 +308,13 @@ def ref_pcg(parts, minv, tol, maxiter, nglob=None, resvec=None, exist_dp0=True, 
     if flag == 0:                                                      # :566-567
         relres = normr_act / n2b
         Xout = X
+        _tr("final", rr=0.0)
     else:                                                              # :568-582
         fint = op.apply(XMin)
         Rm = [Fext[k] - fint[k] for k in rng]
-        normr_m = np.sqrt(_mpi_sum([np.dot(Rm[k], Rm[k] * W[k]) for k in rng]))
+        rr_m = _mpi_sum([np.dot(Rm[k], Rm[k] * W[k]) for k in rng])
+        normr_m = np.sqrt(rr_m)
+        _tr("final", rr=float(rr_m))
         if normr_m < normr_act:
             it = imin
             relres = normr_m / n2b

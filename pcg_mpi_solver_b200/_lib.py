@@ -83,6 +83,8 @@ SIGNATURES = {
     "pcgb_solver_destroy": (c_int, [c_void_p]),
     "pcgb_solve": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(Options), c_void_p, POINTER(Result), c_void_p]),
     "pcgb_apply": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcgb_solver_set_trace": (c_int, [c_void_p, c_void_p, c_int64, c_void_p]),
+    "pcgb_trace_record_bytes": (c_int64, []),
     "pcgb_ebe_create": (c_int, [c_int64, c_int, POINTER(EbeGroup), POINTER(c_void_p)]),
     "pcgb_ebe_destroy": (c_int, [c_void_p]),
     "pcgb_ebe_apply": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -250,6 +250,63 @@ __global__ void k_ctrl_head(PcgCtrl *ctrl, const double *__restrict__ red /* rz,
   else ctrl_head(ctrl, red[0], red[1]);
 }
 
+// ---- opt-in trace of the control steps (pcgb_solver_set_trace): one fixed-size record per step, appended in order.
+// Records hold the reduced values the step consumed and the whole PcgCtrl after it, so a host restatement of the
+// control logic can replay the loop bit for bit (tests/pcg_shadow.py).  Nothing here runs unless tracing is on.
+enum PcgTraceKind : int { TR_HEAD = 0, TR_ITER = 1, TR_VERIFY = 2, TR_RESUME = 3, TR_FINAL = 4 };
+// in[] / local[] slots: 0 pq | 1 pp | 2 xx | 3 rr | 4 rz | 5 ninf | 6 b.b | 7 r0.r0   (unused slots are 0)
+//   HEAD (iteration 0) and RESUME (head after a failed verification): rz, ninf (+ b.b, r0.r0 for HEAD)
+//   ITER: pq, pp, xx, rr, rz, ninf      VERIFY: rr = sum (b - A x_cur)^2 w      FINAL: rr of b - A x_min (0 when flag 0)
+struct PcgTraceRec {
+  int kind, rank, pad0, pad1;
+  double in[8];     // what the step consumed (all-reduced over the ranks)
+  double local[8];  // this rank's value of the same slots before the all-reduce (= in on one rank)
+  PcgCtrl ctrl;     // control state after the step
+};
+struct PcgTraceHdr {
+  unsigned long long total;  // records produced by the solve (those past the capacity are dropped)
+  int frozen;                // the last record left the loop stopped: later no-op iterations write nothing
+  int pad[13];
+};
+static_assert(sizeof(PcgTraceHdr) == 64, "trace header layout");
+
+__device__ __forceinline__ PcgTraceRec *trace_slot(PcgTraceHdr *hdr, PcgTraceRec *rec, long long cap, int state) {
+  const unsigned long long k = hdr->total;
+  hdr->total = k + 1;
+  hdr->frozen = state != ST_RUN;
+  return k < (unsigned long long)cap ? rec + k : nullptr;
+}
+
+// record of a device-side step (HEAD / ITER / RESUME) from the control block and the reduced scalars in red[0..8)
+__global__ void k_trace_step(PcgTraceHdr *hdr, PcgTraceRec *rec, long long cap, int rank, int kind, const PcgCtrl *ctrl,
+                             const double *red, const double *local, double bb, double r0r0) {
+  if (kind == TR_ITER && hdr->frozen) return;   // the iteration did not run
+  PcgTraceRec *t = trace_slot(hdr, rec, cap, ctrl->state);
+  if (!t) return;
+  double in[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  int mask;
+  if (kind == TR_ITER) { for (int k = 0; k < 6; ++k) in[k] = red[k]; mask = 0x3f; }
+  else { in[4] = red[6]; in[5] = red[7]; in[6] = bb; in[7] = r0r0; mask = 0x30; }
+  t->kind = kind; t->rank = rank; t->pad0 = 0; t->pad1 = 0;
+  for (int k = 0; k < 8; ++k) {
+    t->in[k] = in[k];
+    t->local[k] = local ? (((mask >> k) & 1) ? local[k] : 0.0) : in[k];
+  }
+  t->ctrl = *ctrl;
+}
+
+// record of a host-side step (VERIFY / FINAL): the host's control block by value; snap_tail (may be NULL) receives
+// xcur, xmin, alias of that control block
+__global__ void k_trace_host(PcgTraceHdr *hdr, PcgTraceRec *rec, long long cap, int rank, int kind, PcgCtrl c, double rr,
+                             const double *local, double *snap_tail) {
+  if (snap_tail) { snap_tail[0] = c.xcur; snap_tail[1] = c.xmin; snap_tail[2] = c.alias; }
+  PcgTraceRec *t = trace_slot(hdr, rec, cap, c.state);
+  if (!t) return;
+  t->kind = kind; t->rank = rank; t->pad0 = 0; t->pad1 = 0;
+  for (int k = 0; k < 8; ++k) { t->in[k] = k == 3 ? rr : 0.0; t->local[k] = k == 3 ? (local ? local[3] : rr) : 0.0; }
+  t->ctrl = c;
+}
+
 // out[0] = sqrt(in[0])  (ResVec[0] = ||r0|| without a host round trip)
 __global__ void k_sqrt_store(const double *__restrict__ in, double *__restrict__ out) { out[0] = sqrt(in[0]); }
 

@@ -38,8 +38,11 @@ struct GraphKey {
   const void *minv, *w, *xb0, *resvec;
   int iters;
   int variant;   // what the captured iteration looks like: bit 0 peer transport, bit 1 interface-first split, bit 2 forked unpack
+  const void *trace;   // trace buffer and capacity (kernel arguments of the captured trace records; NULL = tracing off)
+  long long trace_cap;
   bool operator==(const GraphKey &o) const {
-    return minv == o.minv && w == o.w && xb0 == o.xb0 && resvec == o.resvec && iters == o.iters && variant == o.variant;
+    return minv == o.minv && w == o.w && xb0 == o.xb0 && resvec == o.resvec && iters == o.iters && variant == o.variant &&
+           trace == o.trace && trace_cap == o.trace_cap;
   }
 };
 
@@ -63,10 +66,15 @@ struct pcgb_solver_s {
   cudaEvent_t ev_in = nullptr, ev_out = nullptr, ev_l0 = nullptr, ev_l1 = nullptr, ev_s0 = nullptr, ev_s1 = nullptr;
   std::vector<cudaEvent_t> ev_k;  // SpMV brackets (time_kernels)
   cudaGraphExec_t gexec = nullptr;
-  GraphKey gkey{nullptr, nullptr, nullptr, nullptr, 0, 0};
+  GraphKey gkey{nullptr, nullptr, nullptr, nullptr, 0, 0, nullptr, 0};
   int launches = 0;             // launches issued outside graphs (running counter per solve)
   int launches_per_iter = 0;
   bool fork_halo = true;        // PCGB_FORK=0 keeps the unpack on the main stream
+  // opt-in trace of the control steps (pcgb_solver_set_trace); all NULL = off, and the loop is launched exactly as without it
+  PcgTraceHdr *trace = nullptr;
+  long long trace_cap = 0;
+  double *snapshot = nullptr;   // [5][n] + 3: r, p, q, x buffer 0, x buffer 1, then xcur, xmin, alias at the loop exit
+  double *tr_local = nullptr;   // [8] device: this rank's sums before the all-reduce (multi-rank traces)
 };
 
 static int require_device() {
@@ -825,10 +833,21 @@ int pcgb_solver_destroy(pcgb_solver_t s) {
   if (s->ev_s1) cudaEventDestroy(s->ev_s1);
   for (cudaEvent_t e : s->ev_k) cudaEventDestroy(e);
   cudaFree(s->r); cudaFree(s->p); cudaFree(s->q); cudaFree(s->xalt); cudaFree(s->xown); cudaFree(s->partials); cudaFree(s->stage);
-  cudaFree(s->red); cudaFree(s->d_ctrl);
+  cudaFree(s->red); cudaFree(s->d_ctrl); cudaFree(s->tr_local);
   if (s->h_ctrl) cudaFreeHost(s->h_ctrl);
   if (s->h_red) cudaFreeHost(s->h_red);
   delete s;
+  return PCGB_OK;
+}
+
+int64_t pcgb_trace_record_bytes(void) { return (int64_t)sizeof(PcgTraceRec); }
+
+int pcgb_solver_set_trace(pcgb_solver_t s, void *d_trace, int64_t capacity, double *d_snapshot) {
+  if (!s || capacity < 0) return fail(PCGB_ERR_ARG, "pcgb_solver_set_trace: bad argument");
+  if (d_trace && !s->tr_local) PCGB_CUDA(cudaMalloc(&s->tr_local, 8 * sizeof(double)));
+  s->trace = static_cast<PcgTraceHdr *>(d_trace);
+  s->trace_cap = d_trace ? capacity : 0;
+  s->snapshot = d_trace ? d_snapshot : nullptr;
   return PCGB_OK;
 }
 
@@ -891,6 +910,37 @@ int rz_to_device(pcgb_solver_t s, const double *minv, const double *w, cudaStrea
   PCGB_CHECK_LAUNCH();
   s->launches += 1;
   return reduce_to_device(s, grid, 2, 6, st);
+}
+
+// ---- trace (pcgb_solver_set_trace): extra launches only when tracing is on
+inline int trace_rank(pcgb_solver_t s) { return s->comm ? s->comm->rank : 0; }
+// this rank's sum of `nv` rows of the partials of `count` blocks into tr_local[dst..) (the same code as the local half of the
+// all-reduce, hence the same bits)
+int trace_local(pcgb_solver_t s, const double *partials, int count, int row_stride, int nv, int dst, cudaStream_t st, int *nl) {
+  if (!s->trace || !multi_rank(s)) return PCGB_OK;
+  if (nv == 1) k_reduce<1, 0><<<1, 256, 0, st>>>(nullptr, partials, count, row_stride, s->tr_local + dst, nullptr);
+  else if (nv == 2) k_reduce<2, 0><<<1, 256, 0, st>>>(nullptr, partials, count, row_stride, s->tr_local + dst, nullptr);
+  else k_reduce<5, 0><<<1, 256, 0, st>>>(nullptr, partials, count, row_stride, s->tr_local + dst, nullptr);
+  PCGB_CHECK_LAUNCH();
+  *nl += 1;
+  return PCGB_OK;
+}
+int trace_step(pcgb_solver_t s, int kind, double bb, double r0r0, cudaStream_t st, int *nl) {
+  if (!s->trace) return PCGB_OK;
+  k_trace_step<<<1, 1, 0, st>>>(s->trace, reinterpret_cast<PcgTraceRec *>(s->trace + 1), s->trace_cap, trace_rank(s), kind,
+                                s->d_ctrl, s->red, multi_rank(s) ? s->tr_local : nullptr, bb, r0r0);
+  PCGB_CHECK_LAUNCH();
+  *nl += 1;
+  return PCGB_OK;
+}
+// has_local: tr_local[3] holds this rank's share of rr (false when rr is not a reduced sum, e.g. 0 for a converged finalisation)
+int trace_host(pcgb_solver_t s, int kind, const PcgCtrl &c, double rr, bool has_local, double *snap_tail, cudaStream_t st) {
+  if (!s->trace) return PCGB_OK;
+  k_trace_host<<<1, 1, 0, st>>>(s->trace, reinterpret_cast<PcgTraceRec *>(s->trace + 1), s->trace_cap, trace_rank(s), kind, c,
+                                rr, multi_rank(s) && has_local ? s->tr_local : nullptr, snap_tail);
+  PCGB_CHECK_LAUNCH();
+  s->launches += 1;
+  return PCGB_OK;
 }
 
 // one PCG iteration enqueued on st (pcg_solver.py:438-562); every kernel no-ops once the state is frozen.
@@ -967,6 +1017,7 @@ int enqueue_iteration(pcgb_solver_t s, const double *minv, const double *w, doub
     k_reduce_ar<1, 1><<<1, 256, 0, st>>>(win, s->d_ctrl, pq_src, pq_cnt, 0, s->red, nullptr);
     PCGB_CHECK_LAUNCH();
     *nl += 1;
+    PCGB_TRY(trace_local(s, pq_src, pq_cnt, 0, 1, 0, st, nl));   // before k_update: the EBE dot partials share s->partials
     PCGB_MARK(5);
     if (fork) PCGB_CUDA(cudaStreamWaitEvent(st, s->ev_join, 0));
     else if (s->halo) PCGB_TRY(halo_unpack(s->halo, s->q, st, nl));
@@ -978,7 +1029,8 @@ int enqueue_iteration(pcgb_solver_t s, const double *minv, const double *w, doub
     PCGB_CHECK_LAUNCH();
     *nl += 2;
     PCGB_MARK(8);
-    return PCGB_OK;
+    PCGB_TRY(trace_local(s, s->partials, vg, kMaxVecGrid, 5, 1, st, nl));
+    return trace_step(s, TR_ITER, 0.0, 0.0, st, nl);
   }
   if (!multi) {
     k_reduce<1, 1><<<1, 256, 0, st>>>(s->d_ctrl, pq_src, pq_cnt, 0, s->red, nullptr);
@@ -989,6 +1041,7 @@ int enqueue_iteration(pcgb_solver_t s, const double *minv, const double *w, doub
     // NCCL transport: reduction, ncclAllReduce and the scalar logic are three stream operations; the halo is serial
     k_reduce<1, 0><<<1, 256, 0, st>>>(s->d_ctrl, pq_src, pq_cnt, 0, s->red, nullptr);
     PCGB_CHECK_LAUNCH();
+    PCGB_TRY(trace_local(s, pq_src, pq_cnt, 0, 1, 0, st, nl));
     PCGB_TRY(allreduce_sum(s->comm, s->red, 1, st));
     k_ctrl_alpha<<<1, 1, 0, st>>>(s->d_ctrl, s->red);
     PCGB_CHECK_LAUNCH();
@@ -1008,6 +1061,7 @@ int enqueue_iteration(pcgb_solver_t s, const double *minv, const double *w, doub
   } else {
     k_reduce<5, 0><<<1, 256, 0, st>>>(s->d_ctrl, s->partials, vg, kMaxVecGrid, s->red + 1, nullptr);
     PCGB_CHECK_LAUNCH();
+    PCGB_TRY(trace_local(s, s->partials, vg, kMaxVecGrid, 5, 1, st, nl));
     PCGB_TRY(allreduce_sum(s->comm, s->red + 1, 5, st));
     k_ctrl_norms<<<1, 1, 0, st>>>(s->d_ctrl, s->red + 1, resvec);
     PCGB_CHECK_LAUNCH();
@@ -1015,7 +1069,7 @@ int enqueue_iteration(pcgb_solver_t s, const double *minv, const double *w, doub
   }
   PCGB_MARK(8);
 #undef PCGB_MARK
-  return PCGB_OK;
+  return trace_step(s, TR_ITER, 0.0, 0.0, st, nl);
 }
 
 int fetch_ctrl(pcgb_solver_t s, cudaStream_t st) {
@@ -1068,6 +1122,7 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
   double *const xw = s->xown;
   double *xbuf[2] = {xw, s->xalt};
   PCGB_CUDA(cudaEventRecord(s->ev_s0, st));
+  if (s->trace) PCGB_CUDA(cudaMemsetAsync(s->trace, 0, sizeof(PcgTraceHdr), st));
 
   // ---- ||b||  (pcg_solver.py:381-384) and the initial residual (:408-418) with ONE host synchronisation:
   //      sum b*b*w -> red[7], r = b - A x0 and sum r*r*w -> red[6]
@@ -1123,6 +1178,8 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
   k_ctrl_head<<<1, 1, 0, st>>>(s->d_ctrl, s->red + 6, 0);
   PCGB_CHECK_LAUNCH();
   s->launches += 1;
+  PCGB_TRY(trace_local(s, s->partials, vg, kMaxVecGrid, 2, 4, st, &s->launches));
+  PCGB_TRY(trace_step(s, TR_HEAD, s->h_red[1], s->h_red[0], st, &s->launches));
 
   int batch = opt->check_every > 0 ? opt->check_every : 16;
   if (batch > opt->maxiter) batch = opt->maxiter;
@@ -1136,7 +1193,7 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
     // ---- enqueue `batch` iterations
     if (want_graph && batch > 1) {
       const int variant = (peer_path(s) ? 1 : 0) | ((s->A && spmv_split_available(s->A->P)) ? 2 : 0) | (s->fork_halo ? 4 : 0);
-      GraphKey key{d_minv, d_w, xw, d_resvec, batch, variant};
+      GraphKey key{d_minv, d_w, xw, d_resvec, batch, variant, s->trace, s->trace_cap};
       if (!s->gexec || !(s->gkey == key)) {
         if (s->gexec) { cudaGraphExecDestroy(s->gexec); s->gexec = nullptr; }
         cudaGraph_t graph = nullptr;
@@ -1172,24 +1229,39 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
       // ---- verification with the true residual (:527-552)
       double normr_act = 0.0;
       PCGB_TRY(true_residual(s, d_b, d_w, xbuf[c.xcur], &normr_act, st));
+      const double rr_act = s->h_red[0];
+      PCGB_TRY(trace_local(s, s->partials, vg, kMaxVecGrid, 1, 3, st, &s->launches));
       ++matvecs;
       c.normr_act = normr_act;
-      if (normr_act <= tolb) { flag = 0; c.flag = 0; break; }  // :540-543
+      if (normr_act <= tolb) {                                  // :540-543
+        flag = 0; c.flag = 0;
+        PCGB_TRY(trace_host(s, TR_VERIFY, c, rr_act, true, nullptr, st));
+        break;
+      }
       if (c.stag >= maxstag && c.moresteps == 0) c.stag = 0;   // :545
       c.moresteps += 1;                                         // :546
       if (c.moresteps >= maxmsteps) {                           // :548-552 (the reference raises here)
-        too_small = 1; flag = 3; c.flag = 3; break;
+        too_small = 1; flag = 3; c.flag = 3;
+        PCGB_TRY(trace_host(s, TR_VERIFY, c, rr_act, true, nullptr, st));
+        break;
       }
       if (normr_act < c.normrmin) { c.normrmin = normr_act; c.xmin = c.xcur; c.imin = c.iter; c.alias = 0; }  // :555-558
-      if (c.stag >= maxstag) { flag = 3; c.flag = 3; break; }  // :560-562
+      if (c.stag >= maxstag) {                                  // :560-562
+        flag = 3; c.flag = 3;
+        PCGB_TRY(trace_host(s, TR_VERIFY, c, rr_act, true, nullptr, st));
+        break;
+      }
       // continue with the replaced residual: head of the next iteration
       c.state = ST_RUN;
+      PCGB_TRY(trace_host(s, TR_VERIFY, c, rr_act, true, nullptr, st));
       *s->h_ctrl = c;
       PCGB_CUDA(cudaMemcpyAsync(s->d_ctrl, s->h_ctrl, sizeof(PcgCtrl), cudaMemcpyHostToDevice, st));
       PCGB_TRY(rz_to_device(s, d_minv, d_w, st));
       k_ctrl_head<<<1, 1, 0, st>>>(s->d_ctrl, s->red + 6, 1);
       PCGB_CHECK_LAUNCH();
       s->launches += 1;
+      PCGB_TRY(trace_local(s, s->partials, vg, kMaxVecGrid, 2, 4, st, &s->launches));
+      PCGB_TRY(trace_step(s, TR_RESUME, 0.0, 0.0, st, &s->launches));
       batch = 1;  // MoreSteps > 0: every further iteration is verified (:527)
       continue;
     }
@@ -1197,6 +1269,11 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
     break;
   }
   PCGB_CUDA(cudaEventRecord(s->ev_l1, st));
+  if (s->snapshot) {  // the loop's vectors before the finalisation overwrites r and q
+    const double *src[5] = {s->r, s->p, s->q, xbuf[0], xbuf[1]};
+    for (int k = 0; k < 5; ++k)
+      PCGB_CUDA(cudaMemcpyAsync(s->snapshot + (size_t)k * n, src[k], (size_t)n * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  }
 
   // ---- finalisation (:566-584)
   const int i = c.iter;
@@ -1207,10 +1284,15 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
     relres = c.normr_act / n2b;
     iter_out = i;
     xout = c.xcur;
+    PCGB_TRY(trace_host(s, TR_FINAL, c, 0.0, false, s->snapshot ? s->snapshot + 5 * n : nullptr, st));
   } else {
     // XMin is the current iterate while it is still aliased to X (no improvement recorded yet): c.xmin == c.xcur then
     double normr_min = 0.0;
     PCGB_TRY(true_residual(s, d_b, d_w, xbuf[c.xmin], &normr_min, st));
+    if (s->trace) {
+      PCGB_TRY(trace_local(s, s->partials, vg, kMaxVecGrid, 1, 3, st, &s->launches));
+      PCGB_TRY(trace_host(s, TR_FINAL, c, s->h_red[0], true, s->snapshot ? s->snapshot + 5 * n : nullptr, st));
+    }
     ++matvecs;
     if (normr_min < c.normr_act) { iter_out = c.imin; relres = normr_min / n2b; }
     else { iter_out = i; relres = c.normr_act / n2b; }

@@ -132,6 +132,19 @@ class Communicator:
             pass
 
 
+# One record of the opt-in loop trace (struct PcgTraceRec / PcgCtrl in csrc/pcg_kernels.cuh, pcgb_solver_set_trace).
+CTRL_DTYPE = np.dtype([(f, "<f8") for f in ("rho", "rho_prev", "alpha", "beta", "pq", "normr", "normp", "normx", "normr_act",
+                                           "normrmin", "tolb", "n2b", "eps")] +
+                      [(f, "<i4") for f in ("state", "flag", "iter", "stag", "moresteps", "imin", "xcur", "xmin", "maxiter",
+                                            "maxstag", "fixed_iters", "alias")])
+TRACE_DTYPE = np.dtype([("kind", "<i4"), ("rank", "<i4"), ("pad", "<i4", 2), ("inp", "<f8", 8), ("local", "<f8", 8),
+                        ("ctrl", CTRL_DTYPE)])
+TRACE_HEADER_BYTES = 64
+TRACE_KINDS = ("head", "iter", "verify", "resume", "final")
+# slots of inp / local
+TRACE_SLOTS = ("pq", "pp", "xx", "rr", "rz", "ninf", "bb", "r0r0")
+
+
 @dataclass
 class SolveInfo:
     flag: int = 1
@@ -152,6 +165,9 @@ class SolveInfo:
     final_ms: float = 0.0
     phase_ms: dict | None = None
     resvec: np.ndarray | None = None
+    trace: np.ndarray | None = None      # TRACE_DTYPE records (trace=...)
+    trace_total: int = 0                 # records the solve produced (> len(trace) when some were dropped)
+    snapshot: dict | None = None         # r, p, q, x (both buffers), xcur, xmin, alias at the loop exit (snapshot=True)
 
 
 class SubdomainOperator:
@@ -238,8 +254,12 @@ class SubdomainOperator:
 
     def solve(self, b: torch.Tensor, M: torch.Tensor | None, tol: float, maxiter: int, x0: torch.Tensor | None = None,
               w: torch.Tensor | None = None, check_every: int = 16, use_graph: bool = True, fixed_iters: bool = False,
-              record_resvec: bool = False, max_stag: int = 3, time_kernels: bool = False):
-        """PCG on device tensors.  Returns (x, SolveInfo); x is a new tensor (x0 is not modified)."""
+              record_resvec: bool = False, max_stag: int = 3, time_kernels: bool = False, trace=False, snapshot: bool = False):
+        """PCG on device tensors.  Returns (x, SolveInfo); x is a new tensor (x0 is not modified).
+
+        trace: record every control step of the loop (True = room for 3*maxiter+8 records, an int = that capacity) into
+        info.trace; snapshot (with trace): the loop's vectors at its exit into info.snapshot.  Tracing is switched off
+        again when the call returns."""
         lib = _lib.load()
         dev = self.device
         assert b.is_cuda and b.dtype == torch.float64 and b.numel() == self.n
@@ -251,9 +271,26 @@ class SubdomainOperator:
                            time_kernels=1 if time_kernels else 0, x0_zero=1 if x0 is None else 0)
         res = _lib.Result()
         resvec = torch.zeros(maxiter + 2, dtype=torch.float64, device=dev) if record_resvec else None
+        tr = snap = None
+        cap = 0
+        tracing = trace is not None and trace is not False     # trace=0 traces into a buffer of no records
+        if tracing:
+            cap = 3 * int(maxiter) + 8 if trace is True else int(trace)
+            rb = int(lib.pcgb_trace_record_bytes())
+            if rb != TRACE_DTYPE.itemsize:
+                raise _lib.PcgbError(f"trace record layout mismatch: library {rb} B, binding {TRACE_DTYPE.itemsize} B")
+            tr = torch.zeros(TRACE_HEADER_BYTES + cap * rb, dtype=torch.uint8, device=dev)
+            if snapshot:
+                snap = torch.full((5 * self.n + 3,), float("nan"), dtype=torch.float64, device=dev)
         with torch.cuda.device(dev):
-            _lib.check(lib.pcgb_solve(self._solver, _lib.ptr(b), _lib.ptr(M), _lib.ptr(w), _lib.ptr(x), ctypes.byref(opt),
-                                      _lib.ptr(resvec), ctypes.byref(res), _lib.stream_ptr()), "pcgb_solve")
+            if tracing:
+                _lib.check(lib.pcgb_solver_set_trace(self._solver, _lib.ptr(tr), cap, _lib.ptr(snap)), "pcgb_solver_set_trace")
+            try:
+                _lib.check(lib.pcgb_solve(self._solver, _lib.ptr(b), _lib.ptr(M), _lib.ptr(w), _lib.ptr(x), ctypes.byref(opt),
+                                          _lib.ptr(resvec), ctypes.byref(res), _lib.stream_ptr()), "pcgb_solve")
+            finally:
+                if tracing:
+                    _lib.check(lib.pcgb_solver_set_trace(self._solver, None, 0, None), "pcgb_solver_set_trace")
         info = SolveInfo(res.flag, res.iters, res.relres, res.normb, res.imin, res.stag, res.moresteps,
                          bool(res.too_small_tol), res.matvecs, res.launches, res.loop_ms, res.spmv_ms,
                          res.spmv_timed, res.loop_iters, res.setup_ms, res.final_ms)
@@ -262,6 +299,15 @@ class SubdomainOperator:
             info.phase_ms = {k: res.phase_ms[i] / res.spmv_timed for i, k in enumerate(names)}
         if record_resvec:
             info.resvec = resvec[: int(res.loop_iters) + 1].cpu().numpy()   # ||r_0|| .. ||r_k||, k = iterations executed
+        if tracing:
+            raw = tr.cpu().numpy()
+            info.trace_total = int(raw[:8].view(np.uint64)[0])
+            kept = min(info.trace_total, cap)
+            info.trace = raw[TRACE_HEADER_BYTES: TRACE_HEADER_BYTES + kept * TRACE_DTYPE.itemsize].view(TRACE_DTYPE).copy()
+            if snap is not None:
+                v, n = snap.cpu().numpy(), self.n
+                info.snapshot = {"r": v[:n], "p": v[n:2 * n], "q": v[2 * n:3 * n], "x": (v[3 * n:4 * n], v[4 * n:5 * n]),
+                                 "xcur": v[5 * n], "xmin": v[5 * n + 1], "alias": v[5 * n + 2]}
         return x, info
 
     def __del__(self):

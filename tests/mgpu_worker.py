@@ -3,7 +3,9 @@
 Every rank owns one hex box (assembled CSR, or the matrix-free EBE operator with its separate p.q dot), solves with
 the halo exchange + allreduce path and rank 0 compares
 the gathered solution against the CPU oracle's multi-part emulation of the reference
-(oracle/ref_pcg.py ref_pcg over CsrPart boxes with the same interface lists)."""
+(oracle/ref_pcg.py ref_pcg over CsrPart boxes with the same interface lists).  Every rank records the loop trace; rank 0
+checks that the traces agree on every rank, that on the peer transport every reduced value is the rank-order sum of the
+ranks' local values bit for bit, and that the host restatement of the control logic (tests/pcg_shadow.py) replays it."""
 import json
 import os
 import sys
@@ -51,6 +53,42 @@ def concrete_main(out_path, zip_path):
     dist.destroy_process_group()
 
 
+# slots of the trace records that hold a reduced value with a local counterpart, per record kind
+_REDUCED_SLOTS = {0: (4, 5), 1: (0, 1, 2, 3, 4, 5), 2: (3,), 3: (4, 5), 4: (3,)}
+
+
+def trace_checks(gathered, transport, tol, maxiter, n_global):
+    """Rank-0 checks of the traces of all ranks."""
+    from tests import pcg_shadow as S
+    traces = [g["trace"] for g in gathered]
+    out = {"trace_records": len(traces[0]), "trace_complete": all(g["trace_total"] == len(g["trace"]) for g in gathered)}
+    ranks_ok = [all(int(r) == k for r in t["rank"]) for k, t in enumerate(traces)]
+
+    def shared_part(t):
+        t = t.copy()
+        t["rank"] = 0
+        t["local"] = 0.0
+        return t.tobytes()
+
+    out["trace_identical"] = all(ranks_ok) and all(shared_part(t) == shared_part(traces[0]) for t in traces)
+    checked = mismatches = 0
+    if transport == "peer" and out["trace_identical"]:
+        for j, rec in enumerate(traces[0]):
+            for slot in _REDUCED_SLOTS[int(rec["kind"])]:
+                s = 0.0
+                for t in traces:          # the peer all-reduce adds the ranks' values in rank order, starting from 0
+                    s = s + float(t[j]["local"][slot])
+                checked += 1
+                mismatches += 0 if S.same_bits(s, float(rec["inp"][slot])) else 1
+    out["trace_sum_checked"], out["trace_sum_mismatches"] = checked, mismatches
+    try:
+        S.replay(traces[0], tol, maxiter, n_global)
+        out["trace_replayed"] = True
+    except AssertionError as e:
+        out["trace_replayed"] = str(e)[:300]
+    return out
+
+
 def main():
     out_path = sys.argv[1]
     if len(sys.argv) > 2 and sys.argv[2] == "concrete":
@@ -90,7 +128,7 @@ def main():
     b = load_vector(blk, device=dev)
     minv = op.jacobi()
     tol = 1e-12
-    x, info = op.solve(b, minv, tol, 5000, use_graph=use_graph, check_every=8)
+    x, info = op.solve(b, minv, tol, 5000, use_graph=use_graph, check_every=8, trace=True)
     # operator probe: y = K v for a globally consistent v (function of the global dof id)
     gz, gy, gx = np.meshgrid(*[np.arange(blk.e0[a], blk.e0[a] + blk.ne[a] + 1) for a in (2, 1, 0)], indexing="ij")
     keep = gx.ravel() >= 1
@@ -107,7 +145,8 @@ def main():
     else:                                                         # atomics: reproducible to rounding only
         assert np.abs(y - y2).max() <= 1e-14 * np.abs(y).max(), "operator application is not reproducible"
     gathered = [None] * world
-    dist.gather_object({"gdof": gdof, "x": x.cpu().numpy(), "y": y, "w": w, "info": (info.flag, info.iters, info.relres)},
+    dist.gather_object({"gdof": gdof, "x": x.cpu().numpy(), "y": y, "w": w, "info": (info.flag, info.iters, info.relres),
+                        "trace": info.trace, "trace_total": info.trace_total},
                        gathered if rank == 0 else None, dst=0)
     if rank == 0:
         from oracle import ref_pcg as R
@@ -132,7 +171,8 @@ def main():
             Uref[g["gdof"]] = ref["X"][r]
             Y[g["gdof"]] = g["y"]
             Yref[g["gdof"]] = yrefs[r]
-        res = {"world": world, "flag": info.flag, "iters": info.iters, "relres": info.relres, "ref_flag": ref["Flag"],
+        res = {**trace_checks(gathered, comm.transport, tol, 5000, n_global),
+               "world": world, "flag": info.flag, "iters": info.iters, "relres": info.relres, "ref_flag": ref["Flag"],
                "ref_iters": ref["Iter"], "ref_relres": ref["RelRes"],
                "x_rel_err": float(np.linalg.norm(U - Uref) / np.linalg.norm(Uref)),
                "y_rel_err": float(np.linalg.norm(Y - Yref) / np.linalg.norm(Yref)),

@@ -29,6 +29,12 @@ def _check(res):
     assert res["copy_mismatch"] <= 1e-12      # shared dofs stay consistent across ranks
     assert res["weight_sum"] == res["n_global"]  # ownership weights partition the free dofs
     assert all(tuple(i) == tuple(res["all_infos"][0]) for i in res["all_infos"])  # every rank agrees
+    # the loop trace: complete, bit-identical on every rank, replayed by the host restatement of the control logic, and on the
+    # peer transport every reduced value is the rank-order sum of the ranks' local values
+    assert res["trace_records"] > 0 and res["trace_complete"] and res["trace_identical"]
+    assert res["trace_replayed"] is True, res["trace_replayed"]
+    if res["transport"] == "peer":
+        assert res["trace_sum_checked"] > 0 and res["trace_sum_mismatches"] == 0, (res["trace_sum_checked"], res["trace_sum_mismatches"])
 
 
 SHARED = [(2, 1, 6, "csr"), (2, 0, 6, "csr"), (4, 1, 5, "csr"), (2, 1, 6, "ebe"), (2, 0, 6, "ebe"), (4, 1, 5, "ebe")]
