@@ -34,6 +34,7 @@ typedef struct pcgb_solver_s *pcgb_solver_t; /* PCG workspace bound to one opera
 typedef struct pcgb_ebe_s *pcgb_ebe_t;     /* opt-in matrix-free element-by-element operator (f1) */
 typedef struct pcgb_asm_s *pcgb_asm_t;     /* device assembly of K_i[Eff,Eff] from the pattern groups (symbolic phase state) */
 typedef struct pcgb_ebe2_s *pcgb_ebe2_t;   /* coloured (atomics-free, bit-reproducible) variant of the EBE operator */
+typedef struct pcgb_ebe_ordered_s *pcgb_ebe_ordered_t; /* EBE operator with a fixed summation order (bit-reproducible, solver-ready) */
 
 /* error codes */
 #define PCGB_OK 0
@@ -225,6 +226,27 @@ int pcgb_ebe_apply(pcgb_ebe_t E, const double *d_x, double *d_y, void *stream); 
 int64_t pcgb_ebe_bytes(pcgb_ebe_t E);                                            /* algorithmic bytes per application */
 int pcgb_solver_create_ebe(pcgb_ebe_t E, pcgb_halo_t halo /* may be NULL */, pcgb_comm_t comm /* may be NULL */,
                            pcgb_solver_t *out);
+
+/* ---------------------------------------------------------------- opt-in: ordered matrix-free EBE operator
+ * The same operator as pcgb_ebe_create (same group layout), applied in the reference's own two phases
+ * (calcMatVecProd, pcg_solver.py:279-300) with no atomics in the arithmetic, so every application and every solve is
+ * bit-reproducible:
+ *   phase 1  every group g, element e and local index a writes one product into a slot buffer laid out like the
+ *            reference's `Flat`: slot = off_g + a*ne_g + e (off_g = sum of nd*ne over the groups before g), value
+ *            s_a * acc with acc = fma(Ke[a][b], u_b, acc) over b = 0..nd-1 ascending, starting from 0.0, and
+ *            u_b = Ck_e * (s_b * x[idx_b]) (0 for a clamped b).  Ke is row-major, Ke[a][b] = ke_host[a*nd + b].
+ *   phase 2  y_i = ((0.0 + v_1) + v_2) + ... over the slots of dof i in ascending slot position, i.e. in
+ *            (group, local index, element) order - the order in which np.bincount visits `Flat` (:300).  Every y_i is
+ *            written, 0 when no slot names dof i.
+ * Create builds per-dof slot lists on the device (count, scan, fill, per-dof sort) and synchronises the device.
+ * PCGB_ERR_ARG, before anything is allocated: n >= 2^30, a pattern size outside 1..96, null arrays, or 2^31 or more
+ * slots in all (slot positions are int32).  The slot buffer costs 8 bytes per slot, the lists 4 bytes per free slot. */
+int pcgb_ebe_ordered_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, pcgb_ebe_ordered_t *out);
+int pcgb_ebe_ordered_destroy(pcgb_ebe_ordered_t O);
+int pcgb_ebe_ordered_apply(pcgb_ebe_ordered_t O, const double *d_x, double *d_y, void *stream); /* y = K_i x (no interface sum) */
+int64_t pcgb_ebe_ordered_bytes(pcgb_ebe_ordered_t O);                                         /* algorithmic bytes per application */
+int pcgb_solver_create_ebe_ordered(pcgb_ebe_ordered_t O, pcgb_halo_t halo /* may be NULL */, pcgb_comm_t comm /* may be NULL */,
+                                   pcgb_solver_t *out);
 
 /* ---------------------------------------------------------------- device assembly of the CSR operator (f2)
  * A_i = K_i[Eff,Eff] = sum_e P_e^T (Ck_e S_e Ke S_e) P_e  from the reference's pattern type groups (partition_mesh.py:443-491;

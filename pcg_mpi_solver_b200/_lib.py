@@ -90,6 +90,11 @@ SIGNATURES = {
     "pcgb_ebe_apply": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcgb_ebe_bytes": (c_int64, [c_void_p]),
     "pcgb_solver_create_ebe": (c_int, [c_void_p, c_void_p, c_void_p, POINTER(c_void_p)]),
+    "pcgb_ebe_ordered_create": (c_int, [c_int64, c_int, POINTER(EbeGroup), POINTER(c_void_p)]),
+    "pcgb_ebe_ordered_destroy": (c_int, [c_void_p]),
+    "pcgb_ebe_ordered_apply": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcgb_ebe_ordered_bytes": (c_int64, [c_void_p]),
+    "pcgb_solver_create_ebe_ordered": (c_int, [c_void_p, c_void_p, c_void_p, POINTER(c_void_p)]),
     "pcgb_assemble_symbolic": (c_int, [c_int64, c_int, POINTER(EbeGroup), c_void_p, POINTER(c_int64), c_void_p, POINTER(c_void_p)]),
     "pcgb_assemble_numeric": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcgb_assemble_destroy": (c_int, [c_void_p]),

@@ -128,12 +128,14 @@ __global__ void k_asm_fill(AsmGroup g, int gi, const int64_t *__restrict__ inc_p
   inc[inc_ptr[d] + (int64_t)slot] = ((unsigned long long)gi << 48) | ((unsigned long long)e << 8) | (unsigned long long)i;
 }
 // per dof: insertion sort of its (short) list -> order independent of the atomic fill order
-__global__ void k_asm_sort_inc(int64_t n, const int64_t *__restrict__ inc_ptr, unsigned long long *__restrict__ inc) {
+// (K = the incidence keys here, the int32 slot positions of ebe_ordered.cuh)
+template <typename K>
+__global__ void k_asm_sort_inc(int64_t n, const int64_t *__restrict__ inc_ptr, K *__restrict__ inc) {
   const int64_t d = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (d >= n) return;
   const int64_t a = inc_ptr[d], b = inc_ptr[d + 1];
   for (int64_t i = a + 1; i < b; ++i) {
-    const unsigned long long key = inc[i];
+    const K key = inc[i];
     int64_t j = i - 1;
     while (j >= a && inc[j] > key) { inc[j + 1] = inc[j]; --j; }
     inc[j + 1] = key;

@@ -13,6 +13,7 @@
 #include "ebe.cuh"
 #include "ebe_color.cuh"
 #include "assemble.cuh"
+#include "ebe_ordered.cuh"
 
 using namespace pcgb;
 
@@ -34,10 +35,16 @@ struct pcgb_ebe2_s {
   int device = 0;
 };
 
+struct pcgb_ebe_ordered_s {
+  EboPlan O;
+  int device = 0;
+};
+
 struct GraphKey {
   const void *minv, *w, *xb0, *resvec;
   int iters;
-  int variant;   // what the captured iteration looks like: bit 0 peer transport, bit 1 interface-first split, bit 2 forked unpack
+  int variant;   // what the captured iteration looks like: bit 0 peer transport, bit 1 interface-first split, bit 2 forked unpack,
+                 // bit 3 ordered matrix-free product
   const void *trace;   // trace buffer and capacity (kernel arguments of the captured trace records; NULL = tracing off)
   long long trace_cap;
   bool operator==(const GraphKey &o) const {
@@ -48,7 +55,8 @@ struct GraphKey {
 
 struct pcgb_solver_s {
   pcgb_csr_t A = nullptr;
-  pcgb_ebe_t E = nullptr;       // opt-in matrix-free operator (exactly one of A / E is set)
+  pcgb_ebe_t E = nullptr;       // opt-in matrix-free operator (exactly one of A / E / O is set)
+  pcgb_ebe_ordered_t O = nullptr;  // opt-in matrix-free operator with a fixed summation order
   pcgb_halo_t halo = nullptr;
   pcgb_comm_t comm = nullptr;
   int64_t n = 0;
@@ -560,14 +568,11 @@ int pcgb_halo_exchange_add(pcgb_halo_t h, double *d_y, void *stream) {
 
 int64_t pcgb_halo_bytes(pcgb_halo_t h) { return h ? h->m * 8 : 0; }
 
-// ------------------------------------------------------------------------------------ EBE operator (opt-in, f1)
-int pcgb_ebe_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, pcgb_ebe_t *out) {
-  if (!out || n < 0 || ngroups < 0 || (ngroups > 0 && !groups)) return fail(PCGB_ERR_ARG, "pcgb_ebe_create: bad argument");
-  if (n >= (1 << 30)) return fail(PCGB_ERR_ARG, "pcgb_ebe_create: more than 2^30 dofs");
-  PCGB_TRY(require_device());
-  pcgb_ebe_t E = new pcgb_ebe_s();
-  cudaGetDevice(&E->device);
-  EbePlan &P = E->P;
+}  // extern "C"
+
+// Groups of an EBE plan (atomic or ordered operator): device copies of Ke, constant-memory slots of the 24-dof patterns,
+// the warp-kernel block tables.  On failure P holds what was acquired so far, which ebe_plan_free releases.
+static int ebe_plan_build(EbePlan &P, int64_t n, int ngroups, const pcgb_ebe_group *groups, const char *who) {
   P.n = n;
   std::vector<int> blk_group;
   std::vector<int64_t> blk_e0;
@@ -577,7 +582,7 @@ int pcgb_ebe_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, pcgb_e
   for (int g = 0; g < ngroups && rc == PCGB_OK; ++g) {
     const pcgb_ebe_group &src = groups[g];
     if (src.nd <= 0 || src.nd > 96 || src.ne < 0 || !src.ke_host || (src.ne > 0 && (!src.d_idx || !src.d_ck))) {
-      rc = fail(PCGB_ERR_ARG, "pcgb_ebe_create: group %d: pattern size must be 1..96 and arrays non-null", g);
+      rc = fail(PCGB_ERR_ARG, "%s: group %d: pattern size must be 1..96 and arrays non-null", who, g);
       break;
     }
     EbeGroup eg;
@@ -586,7 +591,7 @@ int pcgb_ebe_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, pcgb_e
     if ((ce = cudaMalloc(&dke, (size_t)src.nd * src.nd * sizeof(double))) != cudaSuccess ||
         (ce = cudaMemcpy(dke, src.ke_host, (size_t)src.nd * src.nd * sizeof(double), cudaMemcpyHostToDevice)) != cudaSuccess) {
       cudaFree(dke);
-      rc = fail(PCGB_ERR_CUDA, "pcgb_ebe_create: %s", cudaGetErrorString(ce));
+      rc = fail(PCGB_ERR_CUDA, "%s: %s", who, cudaGetErrorString(ce));
       break;
     }
     eg.ke = dke;
@@ -600,8 +605,29 @@ int pcgb_ebe_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, pcgb_e
     P.nblk_warp = (int)blk_group.size();
     if ((ce = upload(&P.d_groups, P.groups)) != cudaSuccess || (ce = upload(&P.d_blk_group, blk_group)) != cudaSuccess ||
         (ce = upload(&P.d_blk_e0, blk_e0)) != cudaSuccess)
-      rc = fail(PCGB_ERR_CUDA, "pcgb_ebe_create: %s", cudaGetErrorString(ce));
+      rc = fail(PCGB_ERR_CUDA, "%s: %s", who, cudaGetErrorString(ce));
   }
+  return rc;
+}
+
+static void ebe_plan_free(EbePlan &P, int device) {
+  for (EbeGroup &g : P.groups) {
+    cudaFree(const_cast<double *>(g.ke));
+    ebe_slot_release(device, g.slot);
+  }
+  cudaFree(P.d_groups); cudaFree(P.d_blk_group); cudaFree(P.d_blk_e0);
+}
+
+extern "C" {
+
+// ------------------------------------------------------------------------------------ EBE operator (opt-in, f1)
+int pcgb_ebe_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, pcgb_ebe_t *out) {
+  if (!out || n < 0 || ngroups < 0 || (ngroups > 0 && !groups)) return fail(PCGB_ERR_ARG, "pcgb_ebe_create: bad argument");
+  if (n >= (1 << 30)) return fail(PCGB_ERR_ARG, "pcgb_ebe_create: more than 2^30 dofs");
+  PCGB_TRY(require_device());
+  pcgb_ebe_t E = new pcgb_ebe_s();
+  cudaGetDevice(&E->device);
+  const int rc = ebe_plan_build(E->P, n, ngroups, groups, "pcgb_ebe_create");
   if (rc != PCGB_OK) { pcgb_ebe_destroy(E); return rc; }
   *out = E;
   return PCGB_OK;
@@ -609,11 +635,7 @@ int pcgb_ebe_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, pcgb_e
 
 int pcgb_ebe_destroy(pcgb_ebe_t E) {
   if (!E) return PCGB_OK;
-  for (EbeGroup &g : E->P.groups) {
-    cudaFree(const_cast<double *>(g.ke));
-    ebe_slot_release(E->device, g.slot);
-  }
-  cudaFree(E->P.d_groups); cudaFree(E->P.d_blk_group); cudaFree(E->P.d_blk_e0);
+  ebe_plan_free(E->P, E->device);
   delete E;
   return PCGB_OK;
 }
@@ -624,6 +646,51 @@ int pcgb_ebe_apply(pcgb_ebe_t E, const double *d_x, double *d_y, void *stream) {
 }
 
 int64_t pcgb_ebe_bytes(pcgb_ebe_t E) { return E ? E->P.bytes : 0; }
+
+// ------------------------------------------------------------------------------------ ordered EBE operator (bit-reproducible)
+int pcgb_ebe_ordered_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, pcgb_ebe_ordered_t *out) {
+  if (!out || n < 0 || ngroups < 0 || (ngroups > 0 && !groups)) return fail(PCGB_ERR_ARG, "pcgb_ebe_ordered_create: bad argument");
+  if (n >= (1 << 30)) return fail(PCGB_ERR_ARG, "pcgb_ebe_ordered_create: more than 2^30 dofs");
+  // every refusal happens here, before anything is allocated
+  int64_t nslots = 0;
+  for (int g = 0; g < ngroups; ++g) {
+    const pcgb_ebe_group &src = groups[g];
+    if (src.nd <= 0 || src.nd > 96 || src.ne < 0 || !src.ke_host || (src.ne > 0 && (!src.d_idx || !src.d_ck)))
+      return fail(PCGB_ERR_ARG, "pcgb_ebe_ordered_create: group %d: pattern size must be 1..96 and arrays non-null", g);
+    if (src.ne > INT32_MAX || (nslots += (int64_t)src.nd * src.ne) > INT32_MAX)
+      return fail(PCGB_ERR_ARG, "pcgb_ebe_ordered_create: 2^31 or more element slots (slot positions are int32)");
+  }
+  PCGB_TRY(require_device());
+  pcgb_ebe_ordered_t O = new pcgb_ebe_ordered_s();
+  cudaGetDevice(&O->device);
+  EboPlan &Q = O->O;
+  int rc = ebe_plan_build(Q.P, n, ngroups, groups, "pcgb_ebe_ordered_create");
+  if (rc == PCGB_OK) {
+    for (const EbeGroup &g : Q.P.groups) { Q.off.push_back(Q.nslots); Q.nslots += (int64_t)g.nd * g.ne; }
+    rc = ebo_build_lists(Q, nullptr);
+  }
+  if (rc != PCGB_OK) { pcgb_ebe_ordered_destroy(O); return rc; }
+  // phase 1 as the atomic operator (indices, signs, Ck, x, y) plus the products written; phase 2 reads them back with their
+  // positions and the list offsets (y is already counted)
+  Q.P.bytes += 8 * Q.nfree + 12 * Q.nfree + 8 * (n + 1);
+  *out = O;
+  return PCGB_OK;
+}
+
+int pcgb_ebe_ordered_destroy(pcgb_ebe_ordered_t O) {
+  if (!O) return PCGB_OK;
+  ebe_plan_free(O->O.P, O->device);
+  ebo_free_lists(O->O);
+  delete O;
+  return PCGB_OK;
+}
+
+int pcgb_ebe_ordered_apply(pcgb_ebe_ordered_t O, const double *d_x, double *d_y, void *stream) {
+  if (!O || (O->O.P.n > 0 && (!d_x || !d_y))) return fail(PCGB_ERR_ARG, "pcgb_ebe_ordered_apply: null argument");   // n = 0: no vector
+  return ebo_apply(O->O, d_x, d_y, (cudaStream_t)stream);
+}
+
+int64_t pcgb_ebe_ordered_bytes(pcgb_ebe_ordered_t O) { return O ? O->O.P.bytes : 0; }
 
 // ------------------------------------------------------------------------------------ device assembly (f2)
 int pcgb_assemble_symbolic(int64_t n, int ngroups, const pcgb_ebe_group *groups, int64_t *d_rowptr, int64_t *nnz_out, void *stream,
@@ -769,11 +836,11 @@ int pcgb_ebe2_apply(pcgb_ebe2_t E, const double *d_x, double *d_y, void *stream)
 int pcgb_ebe2_launches(pcgb_ebe2_t E) { return E ? (int)E->C.launches.size() : 0; }
 
 // ------------------------------------------------------------------------------------ solver
-static int solver_create_common(pcgb_csr_t A, pcgb_ebe_t E, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
+static int solver_create_common(pcgb_csr_t A, pcgb_ebe_t E, pcgb_ebe_ordered_t O, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
   if (halo && !comm) comm = halo->comm;
   PCGB_TRY(require_device());
   pcgb_solver_t s = new pcgb_solver_s();
-  s->A = A; s->E = E; s->halo = halo; s->comm = comm; s->n = A ? A->P.nrows : E->P.n;
+  s->A = A; s->E = E; s->O = O; s->halo = halo; s->comm = comm; s->n = A ? A->P.nrows : E ? E->P.n : O->O.P.n;
   s->fork_halo = env_int("PCGB_FORK", 1) != 0;
   const size_t nb = (size_t)(s->n > 0 ? s->n : 1) * sizeof(double);
   s->stage_cap = ((A ? A->P.ntiles : 0) + 4095) / 4096 + 1;
@@ -810,12 +877,17 @@ static int solver_create_common(pcgb_csr_t A, pcgb_ebe_t E, pcgb_halo_t halo, pc
 int pcgb_solver_create(pcgb_csr_t A, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
   if (!A || !out) return fail(PCGB_ERR_ARG, "pcgb_solver_create: null argument");
   if (A->P.nrows != A->P.ncols) return fail(PCGB_ERR_ARG, "pcgb_solver_create: operator must be square");
-  return solver_create_common(A, nullptr, halo, comm, out);
+  return solver_create_common(A, nullptr, nullptr, halo, comm, out);
 }
 
 int pcgb_solver_create_ebe(pcgb_ebe_t E, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
   if (!E || !out) return fail(PCGB_ERR_ARG, "pcgb_solver_create_ebe: null argument");
-  return solver_create_common(nullptr, E, halo, comm, out);
+  return solver_create_common(nullptr, E, nullptr, halo, comm, out);
+}
+
+int pcgb_solver_create_ebe_ordered(pcgb_ebe_ordered_t O, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
+  if (!O || !out) return fail(PCGB_ERR_ARG, "pcgb_solver_create_ebe_ordered: null argument");
+  return solver_create_common(nullptr, nullptr, O, halo, comm, out);
 }
 
 int pcgb_solver_destroy(pcgb_solver_t s) {
@@ -862,6 +934,7 @@ inline bool peer_path(pcgb_solver_t s) { return multi_rank(s) && s->comm->use_pe
 // y = A x + interface sum  (calcMPFint, pcg_solver.py:339-342)
 int op_apply(pcgb_solver_t s, const double *x, double *y, cudaStream_t st) {
   if (s->E) PCGB_TRY(ebe_apply(s->E->P, x, y, st, &s->launches));
+  else if (s->O) PCGB_TRY(ebo_apply(s->O->O, x, y, st, &s->launches));
   else PCGB_TRY(spmv_launch(s->A->P, x, y, false, st, &s->launches));
   if (s->halo) PCGB_TRY(halo_exchange_add(s->halo, y, st, &s->launches));
   return PCGB_OK;
@@ -966,8 +1039,9 @@ int enqueue_iteration(pcgb_solver_t s, const double *minv, const double *w, doub
   const double *pq_src;
   int pq_cnt;
   bool halo_done = false;
-  if (s->E) {  // matrix-free operator: product, then a separate unweighted dot of the local product
-    PCGB_TRY(ebe_apply(s->E->P, s->p, s->q, st, nl, &s->d_ctrl->state));
+  if (s->E || s->O) {  // matrix-free operator: product, then a separate unweighted dot of the local product
+    if (s->E) PCGB_TRY(ebe_apply(s->E->P, s->p, s->q, st, nl, &s->d_ctrl->state));
+    else PCGB_TRY(ebo_apply(s->O->O, s->p, s->q, st, nl, &s->d_ctrl->state));
     PCGB_MARK(2); PCGB_MARK(3); PCGB_MARK(4);
     k_dot_w<<<vg, kVecBlock, 0, st>>>(n, s->p, s->q, nullptr, s->partials);
     PCGB_CHECK_LAUNCH();
@@ -1192,7 +1266,8 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
   for (;;) {
     // ---- enqueue `batch` iterations
     if (want_graph && batch > 1) {
-      const int variant = (peer_path(s) ? 1 : 0) | ((s->A && spmv_split_available(s->A->P)) ? 2 : 0) | (s->fork_halo ? 4 : 0);
+      const int variant = (peer_path(s) ? 1 : 0) | ((s->A && spmv_split_available(s->A->P)) ? 2 : 0) | (s->fork_halo ? 4 : 0) |
+                          (s->O ? 8 : 0);
       GraphKey key{d_minv, d_w, xw, d_resvec, batch, variant, s->trace, s->trace_cap};
       if (!s->gexec || !(s->gkey == key)) {
         if (s->gexec) { cudaGraphExecDestroy(s->gexec); s->gexec = nullptr; }

@@ -7,6 +7,10 @@ block tails, signs, clamped and high-valence dofs - entrywise against a long-dou
 overflow and sharing, the EBE solver against the oracle and generate_ebe on every bench box; tests/test_gpu_multi.py:
 the EBE operator across ranks); timing: `bench.py --operator ebe`.  Scatter-adds with fp64 atomics
 (reproducible to rounding only); `EbeMatrixColored` is the bit-reproducible coloured variant (3x slower).  `to_operator(kind="ebe")`.
+
+`EbeMatrixOrdered` (`to_operator(kind="ebe_ordered")`) is the same operator in the reference's own two phases - element
+products into a slot buffer laid out like `Flat`, then a per-dof sum in ascending slot position (csrc/ebe_ordered.cuh,
+include/pcgb200.h) - with no atomics in the arithmetic: bit-reproducible, and usable in the PCG solve like EbeMatrix.
 """
 from __future__ import annotations
 
@@ -20,6 +24,9 @@ from . import _lib
 
 class EbeMatrix:
     """Pattern groups of one subdomain on the device, indices in the free-dof numbering (-1 = clamped)."""
+
+    _fn = ("pcgb_ebe_create", "pcgb_ebe_apply", "pcgb_ebe_bytes", "pcgb_ebe_destroy")   # C entry points of this operator
+    _symmetric_only = True    # the warp kernel reads column i of Ke for row i
 
     def __init__(self, groups, loc_dof_eff: np.ndarray, ndof: int, device="cuda"):
         self.device = torch.device(device)
@@ -35,7 +42,7 @@ class EbeMatrix:
             nd, ne = g.loc_dof.shape
             idx = eff_map[g.loc_dof].astype(np.int32)                       # (nd, ne)
             ke = np.ascontiguousarray(g.ke, dtype=np.float64)
-            if not np.allclose(ke, ke.T, rtol=1e-12, atol=1e-12 * np.abs(ke).max()):
+            if self._symmetric_only and not np.allclose(ke, ke.T, rtol=1e-12, atol=1e-12 * np.abs(ke).max()):
                 raise ValueError("EbeMatrix: pattern matrices must be symmetric")
             d_idx = torch.from_numpy(np.ascontiguousarray(idx)).to(self.device)
             d_ck = torch.from_numpy(np.ascontiguousarray(g.ck, dtype=np.float64)).to(self.device)
@@ -55,7 +62,7 @@ class EbeMatrix:
         self._diag = diag
         self._h = ctypes.c_void_p()
         with torch.cuda.device(self.device):
-            _lib.check(_lib.load().pcgb_ebe_create(n, len(groups), cgroups, ctypes.byref(self._h)), "pcgb_ebe_create")
+            _lib.check(getattr(_lib.load(), self._fn[0])(n, len(groups), cgroups, ctypes.byref(self._h)), self._fn[0])
 
     @property
     def handle(self):
@@ -65,7 +72,7 @@ class EbeMatrix:
         """y = K_i x, no interface sum."""
         y = out if out is not None else torch.empty(self.shape[0], dtype=torch.float64, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(_lib.load().pcgb_ebe_apply(self._h, _lib.ptr(x), _lib.ptr(y), _lib.stream_ptr()), "pcgb_ebe_apply")
+            _lib.check(getattr(_lib.load(), self._fn[1])(self._h, _lib.ptr(x), _lib.ptr(y), _lib.stream_ptr()), self._fn[1])
         return y
 
     spmv = apply_local
@@ -74,15 +81,25 @@ class EbeMatrix:
         return torch.from_numpy(self._diag).to(self.device)
 
     def spmv_bytes(self) -> int:
-        return int(_lib.load().pcgb_ebe_bytes(self._h))
+        return int(getattr(_lib.load(), self._fn[2])(self._h))
 
     def __del__(self):
         try:
             if self._h:
-                _lib.load().pcgb_ebe_destroy(self._h)
+                getattr(_lib.load(), self._fn[3])(self._h)
                 self._h = ctypes.c_void_p()
         except Exception:
             pass
+
+
+class EbeMatrixOrdered(EbeMatrix):
+    """The EbeMatrix operator with a fixed summation order: element products into a slot buffer laid out like the
+    reference's `Flat` (slot = off_g + a*ne_g + e), then every dof sums its slots in ascending position, i.e. in
+    (group, local index, element) order - what np.bincount does (pcg_solver.py:300).  Bit-reproducible; the PCG solve
+    accepts it like EbeMatrix.  Pattern matrices need not be symmetric.  Costs 8 B per element slot and 4 B per free slot of device memory on top."""
+
+    _fn = ("pcgb_ebe_ordered_create", "pcgb_ebe_ordered_apply", "pcgb_ebe_ordered_bytes", "pcgb_ebe_ordered_destroy")
+    _symmetric_only = False   # both kernels read Ke by rows, as Ke @ (Ck * U) does
 
 
 class EbeMatrixColored:

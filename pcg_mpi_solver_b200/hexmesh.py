@@ -149,11 +149,12 @@ def hex_type_group(block: HexBlock):
     return grp, eff, 3 * (nx + 1) * (ny + 1) * (nz + 1)
 
 
-def generate_ebe(block: HexBlock, device="cuda"):
-    """The same box as a matrix-free EBE operator (ebe.EbeMatrix); opt-in companion of generate_matrix (SURVEY 8(f1))."""
-    from .ebe import EbeMatrix
+def generate_ebe(block: HexBlock, device="cuda", ordered: bool = False):
+    """The same box as a matrix-free EBE operator (ebe.EbeMatrix); opt-in companion of generate_matrix (SURVEY 8(f1)).
+    ordered=True builds ebe.EbeMatrixOrdered, the bit-reproducible variant with a fixed summation order."""
+    from .ebe import EbeMatrix, EbeMatrixOrdered
     grp, eff, ndof = hex_type_group(block)
-    return EbeMatrix([grp], eff, ndof, device=device)
+    return (EbeMatrixOrdered if ordered else EbeMatrix)([grp], eff, ndof, device=device)
 
 
 def hex_mdf_model(ng, E: float = 1.0, nu: float = 0.3, h: float | None = None, traction: float = 1.0):

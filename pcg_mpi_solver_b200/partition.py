@@ -104,12 +104,16 @@ class SubdomainData:
 
     def to_operator(self, comm=None, device="cuda", kind: str = "csr"):
         """Upload A and build the halo plan: the `A` argument of solve() for this rank.
-        kind="ebe" selects the opt-in matrix-free operator (ebe.py) instead of the assembled CSR matrix."""
+        kind="ebe" selects the opt-in matrix-free operator (ebe.py) instead of the assembled CSR matrix, kind="ebe_ordered"
+        its bit-reproducible variant with a fixed summation order."""
         from .csr import CsrMatrix
         from .solver import SubdomainOperator
         if kind == "ebe":
             from .ebe import EbeMatrix
             M = EbeMatrix(self.groups, self.loc_dof_eff, self.ndof, device=device)
+        elif kind == "ebe_ordered":
+            from .ebe import EbeMatrixOrdered
+            M = EbeMatrixOrdered(self.groups, self.loc_dof_eff, self.ndof, device=device)
         elif self.A is not None:
             M = CsrMatrix.from_scipy(self.A, device=device)
         else:  # assemble on the device straight from the pattern groups

@@ -223,7 +223,13 @@ class SubdomainOperator:
                             comm.set_transport("nccl")
                         else:
                             raise _lib.PcgbError(f"halo exchange over peer memory is not available ({comm.peer_error}) and the communicator has no NCCL")
-            create = lib.pcgb_solver_create if isinstance(A, CsrMatrix) else lib.pcgb_solver_create_ebe  # EbeMatrix: opt-in matrix-free operator
+            from .ebe import EbeMatrixOrdered
+            if isinstance(A, CsrMatrix):
+                create = lib.pcgb_solver_create
+            elif isinstance(A, EbeMatrixOrdered):                       # matrix-free, fixed summation order
+                create = lib.pcgb_solver_create_ebe_ordered
+            else:                                                      # EbeMatrix: opt-in matrix-free operator
+                create = lib.pcgb_solver_create_ebe
             _lib.check(create(A.handle, self._halo if self._halo else None,
                               comm.handle if comm is not None else None, ctypes.byref(self._solver)), "pcgb_solver_create")
 
