@@ -35,6 +35,7 @@ typedef struct pcgb_ebe_s *pcgb_ebe_t;     /* opt-in matrix-free element-by-elem
 typedef struct pcgb_asm_s *pcgb_asm_t;     /* device assembly of K_i[Eff,Eff] from the pattern groups (symbolic phase state) */
 typedef struct pcgb_ebe2_s *pcgb_ebe2_t;   /* coloured (atomics-free, bit-reproducible) variant of the EBE operator */
 typedef struct pcgb_ebe_ordered_s *pcgb_ebe_ordered_t; /* EBE operator with a fixed summation order (bit-reproducible, solver-ready) */
+typedef struct pcgb_mg_s *pcgb_mg_t;       /* geometric multigrid preconditioner of a hex-box solver (one V-cycle) */
 
 /* error codes */
 #define PCGB_OK 0
@@ -286,6 +287,45 @@ int64_t pcgb_hex_nrows(const pcgb_hex_box *box);
 int pcgb_hex_count(const pcgb_hex_box *box, int64_t *d_rowcount, void *stream);
 int pcgb_hex_fill(const pcgb_hex_box *box, const double *ke_host, double ck, const int64_t *d_rowptr,
                   int32_t *d_col, double *d_val, void *stream);
+
+/* ---------------------------------------------------------------- opt-in: geometric multigrid preconditioner (hex boxes)
+ * z = M r is one symmetric V-cycle over nested hex boxes, for a one-rank solver whose operator (CSR, EBE or ordered EBE) is
+ * the stiffness matrix of `box` in the pcgb_hex_* numbering.  Level l+1 halves every ne of level l while all ne are even and
+ * the halves stay >= 2; its matrix is generated on the device at spacing 2^l h (Ck = E 2^l h), which for nested Q1 spaces
+ * equals the Galerkin product P^T A P.  P is trilinear interpolation of the free nodes, direction by direction (weights 1,
+ * 1/2, 1/4, 1/8); restriction (P^T, <= 27 fine nodes in (dz, dy, dx) ascending order) and prolongation (<= 8 coarse nodes
+ * in ascending order, added to x) are gathers without atomics.  Every level but the coarsest smooths with a degree-`degree`
+ * Chebyshev polynomial in D^-1 A on [lo, 1.1] * lambda, lambda the largest eigenvalue of the tridiagonal matrix of 20
+ * Lanczos steps on D^-1 A (D inner product) from the fixed start vector v_i = 1/2 + ((37 i + 11) mod 101) / 101.  The pre-smoother starts from x = 0 and the
+ * post-smoother applies the same polynomial to b - A x, so M is symmetric.  The coarsest level (at most 1536 dofs) is
+ * solved with a dense Cholesky factor computed on the device at create.  D^-1 of the fine level is a copy of
+ * d_minv_fine (n doubles); the coarse levels use their own diagonals.
+ * PCGB_ERR_ARG before anything is allocated: a solver with a halo plan or communicator, a box with e0 != 0 or ng != ne, a
+ * box that does not coarsen at least once, a coarsest level above 1536 dofs, degree < 1, lo outside (0, 1.1), E or h <= 0,
+ * or an operator whose size is not the box's.  The solver must outlive the handle; destroying the handle also drops the
+ * solver's cached graph of MG iterations.  Create synchronises the device first (d_minv_fine may come from any stream)
+ * and again before it returns.                                                                                          */
+#define PCGB_MG_MAX_LEVELS 32
+int pcgb_mg_create(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, const double *d_minv_fine,
+                   int degree, double lo, pcgb_mg_t *out);
+int pcgb_mg_destroy(pcgb_mg_t mg);
+int pcgb_mg_apply(pcgb_mg_t mg, const double *d_r, double *d_z, void *stream); /* z = M r (one V-cycle) */
+/* levels; n per level, lambda per level (0 for the coarsest) into arrays of PCGB_MG_MAX_LEVELS entries; device bytes the
+ * hierarchy allocated (vectors, coarse CSR, dense factor; the coarse SpMV plans' tile tables are not counted).  Any may be NULL. */
+int pcgb_mg_info(pcgb_mg_t mg, int32_t *nlevels, int64_t *n_level, double *lambda, int64_t *bytes);
+/* the V-cycle's parts, for tests: r_c = P^T r_f and x_f += P e_c between `level` and level+1; one smoothing
+ * x += S (b - A x) on `level` (x = 0 gives the pre-smoother's x = S b); z = A_c^-1 r on the coarsest level */
+int pcgb_mg_restrict(pcgb_mg_t mg, int level, const double *d_fine, double *d_coarse, void *stream);
+int pcgb_mg_prolong_add(pcgb_mg_t mg, int level, const double *d_coarse, double *d_fine, void *stream);
+int pcgb_mg_smooth(pcgb_mg_t mg, int level, const double *d_b, double *d_x, void *stream);
+int pcgb_mg_coarse_solve(pcgb_mg_t mg, const double *d_r, double *d_z, void *stream);
+/* pcgb_solve with z = M r instead of z = Minv .* r: the same loop, options, result and trace.  z counts as infinite
+ * (flag 2) when any entry is not finite, since a V-cycle spreads one NaN over all of z.  res->matvecs counts the solver
+ * operator's applications by the loop itself (one per iteration plus the true residuals), as in pcgb_solve; the
+ * V-cycles' own products (2 * degree of the fine operator per cycle, plus the coarse levels) are not in it.  With
+ * time_kernels, phase_ms[5] ("fused update") includes the V-cycle that follows the update.                        */
+int pcgb_solve_mg(pcgb_solver_t s, pcgb_mg_t mg, const double *d_b, const double *d_w, double *d_x, const pcgb_options *opt,
+                  double *d_resvec, pcgb_result *res, void *stream);
 
 #ifdef __cplusplus
 }

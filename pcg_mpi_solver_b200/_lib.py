@@ -16,6 +16,7 @@ LIB_PATH = os.path.join(_HERE, "csrc", "libpcgb200.so")
 UNIQUE_ID_BYTES = 128
 IPC_BLOB_BYTES = 64
 TRANSPORT_NCCL, TRANSPORT_PEER = 0, 1
+MG_MAX_LEVELS = 32
 
 
 class PcgbError(RuntimeError):
@@ -102,6 +103,15 @@ SIGNATURES = {
     "pcgb_ebe2_destroy": (c_int, [c_void_p]),
     "pcgb_ebe2_apply": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcgb_ebe2_launches": (c_int, [c_void_p]),
+    "pcgb_mg_create": (c_int, [c_void_p, POINTER(HexBox), POINTER(c_double), c_double, c_double, c_void_p, c_int, c_double, POINTER(c_void_p)]),
+    "pcgb_mg_destroy": (c_int, [c_void_p]),
+    "pcgb_mg_apply": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcgb_mg_info": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int64), POINTER(c_double), POINTER(c_int64)]),
+    "pcgb_mg_restrict": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "pcgb_mg_prolong_add": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "pcgb_mg_smooth": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
+    "pcgb_mg_coarse_solve": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcgb_solve_mg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(Options), c_void_p, POINTER(Result), c_void_p]),
     "pcgb_hex_nrows": (c_int64, [POINTER(HexBox)]),
     "pcgb_hex_count": (c_int, [POINTER(HexBox), c_void_p, c_void_p]),
     "pcgb_hex_fill": (c_int, [POINTER(HexBox), POINTER(c_double), c_double, c_void_p, c_void_p, c_void_p, c_void_p]),

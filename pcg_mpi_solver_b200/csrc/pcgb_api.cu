@@ -14,6 +14,7 @@
 #include "ebe_color.cuh"
 #include "assemble.cuh"
 #include "ebe_ordered.cuh"
+#include "gmg.cuh"
 
 using namespace pcgb;
 
@@ -47,9 +48,10 @@ struct GraphKey {
                  // bit 3 ordered matrix-free product
   const void *trace;   // trace buffer and capacity (kernel arguments of the captured trace records; NULL = tracing off)
   long long trace_cap;
+  const void *mg;      // multigrid preconditioner of the captured V-cycles (NULL = diagonal Minv)
   bool operator==(const GraphKey &o) const {
     return minv == o.minv && w == o.w && xb0 == o.xb0 && resvec == o.resvec && iters == o.iters && variant == o.variant &&
-           trace == o.trace && trace_cap == o.trace_cap;
+           trace == o.trace && trace_cap == o.trace_cap && mg == o.mg;
   }
 };
 
@@ -74,7 +76,7 @@ struct pcgb_solver_s {
   cudaEvent_t ev_in = nullptr, ev_out = nullptr, ev_l0 = nullptr, ev_l1 = nullptr, ev_s0 = nullptr, ev_s1 = nullptr;
   std::vector<cudaEvent_t> ev_k;  // SpMV brackets (time_kernels)
   cudaGraphExec_t gexec = nullptr;
-  GraphKey gkey{nullptr, nullptr, nullptr, nullptr, 0, 0, nullptr, 0};
+  GraphKey gkey{nullptr, nullptr, nullptr, nullptr, 0, 0, nullptr, 0, nullptr};
   int launches = 0;             // launches issued outside graphs (running counter per solve)
   int launches_per_iter = 0;
   bool fork_halo = true;        // PCGB_FORK=0 keeps the unpack on the main stream
@@ -977,8 +979,15 @@ int true_residual(pcgb_solver_t s, const double *b, const double *w, const doubl
 }
 
 // (sum z.(r w), #inf z) of the current r into s->red[6..7] (device, all-reduced)
-int rz_to_device(pcgb_solver_t s, const double *minv, const double *w, cudaStream_t st) {
+int mg_rz(pcgb_solver_t s, pcgb_mg_t mg, const double *w, double *partials, cudaStream_t st, int *nl, const int *skip);
+
+// (mg: z = M r by the V-cycle, the same launches as inside the iteration)
+int rz_to_device(pcgb_solver_t s, const double *minv, const double *w, cudaStream_t st, pcgb_mg_t mg = nullptr) {
   const int grid = vec_grid(s->n);
+  if (mg) {
+    PCGB_TRY(mg_rz(s, mg, w, s->partials, st, &s->launches, &s->d_ctrl->state));
+    return reduce_to_device(s, grid, 2, 6, st);
+  }
   k_rz<<<grid, kVecBlock, 0, st>>>(s->n, s->r, minv, w, s->partials);
   PCGB_CHECK_LAUNCH();
   s->launches += 1;
@@ -1016,20 +1025,127 @@ int trace_host(pcgb_solver_t s, int kind, const PcgCtrl &c, double rr, bool has_
   return PCGB_OK;
 }
 
+}  // namespace
+
+// ---- geometric multigrid preconditioner (pcgb_mg_*): one symmetric V-cycle z = M r
+struct MgLevel {
+  HexGeom g{};
+  int64_t n = 0;
+  void *rowptr = nullptr;   // coarse levels above the coarsest: device-generated CSR (int32 offsets below 2^31 non-zeros)
+  int *col = nullptr;
+  double *val = nullptr;
+  CsrPlan P;
+  bool has_plan = false;
+  double *dinv = nullptr;                                    // inverse diagonal (level 0: a copy of the caller's Minv)
+  double *b = nullptr, *x = nullptr;                         // right-hand side and correction (level 0: the caller's r and z)
+  double *r = nullptr, *d = nullptr, *q = nullptr;           // smoother residual, direction, operator product
+  double lambda = 0.0, inv_theta = 0.0;
+  std::vector<double> c1, c2;                                // Chebyshev recurrence of steps 1 .. degree-1
+};
+
+struct pcgb_mg_s {
+  pcgb_solver_t s = nullptr;
+  std::vector<MgLevel> lv;
+  int degree = 2;
+  double lo = 0.25;
+  int nc = 0;
+  double *chol = nullptr;   // coarsest level: dense Cholesky factor, L in the lower triangle mirrored into the upper
+  double *z = nullptr;      // z = M r of the PCG loop
+  double *partials = nullptr, *red = nullptr, *h_red = nullptr;
+  int *d_bad = nullptr;
+  int64_t bytes = 0;
+};
+
+namespace {
+
+constexpr int kMgLanczosSteps = 20;
+
+int mg_op(pcgb_mg_t mg, int l, const double *x, double *y, cudaStream_t st, int *nl, const int *skip) {
+  if (l > 0) return spmv_launch(mg->lv[(size_t)l].P, x, y, false, st, nl, skip);
+  pcgb_solver_t s = mg->s;
+  if (s->E) return ebe_apply(s->E->P, x, y, st, nl, skip);
+  if (s->O) return ebo_apply(s->O->O, x, y, st, nl, skip);
+  return spmv_launch(s->A->P, x, y, false, st, nl, skip);
+}
+
+// Chebyshev smoothing of D^-1 A on level l: zero_start: x = S b (no operator application for x = 0); otherwise
+// x += S (b - A x).  S is the same polynomial in both forms, so pre- and post-smoothing keep the V-cycle symmetric.
+// resid (pre-smoother): one more product leaves r = b - A x for the restriction.
+int mg_smooth(pcgb_mg_t mg, int l, const double *b, double *x, bool zero_start, bool resid, cudaStream_t st, int *nl, const int *skip) {
+  MgLevel &L = mg->lv[(size_t)l];
+  const int grid = vec_grid(L.n);
+  if (!zero_start) PCGB_TRY(mg_op(mg, l, x, L.q, st, nl, skip));
+  k_mg_cheb_first<<<grid, 256, 0, st>>>(L.n, b, zero_start ? nullptr : L.q, L.dinv, L.inv_theta, L.r, L.d, x, skip);
+  PCGB_CHECK_LAUNCH();
+  *nl += 1;
+  for (int j = 0; j < (int)L.c1.size() + (resid ? 1 : 0); ++j) {
+    const bool last = j == (int)L.c1.size();
+    PCGB_TRY(mg_op(mg, l, L.d, L.q, st, nl, skip));
+    k_mg_cheb_step<<<grid, 256, 0, st>>>(L.n, L.q, L.dinv, last ? 0.0 : L.c1[(size_t)j], last ? 0.0 : L.c2[(size_t)j], last ? 1 : 0,
+                                         L.r, L.d, x, skip);
+    PCGB_CHECK_LAUNCH();
+    *nl += 1;
+  }
+  return PCGB_OK;
+}
+
+inline unsigned mg_node_grid(const HexGeom &g) { return (unsigned)((g.nfree_nodes + 255) / 256); }
+
+int mg_coarse_solve(pcgb_mg_t mg, const double *r, double *z, cudaStream_t st, int *nl, const int *skip) {
+  k_mg_chol_solve<<<1, kMgCholThreads, 0, st>>>(mg->nc, mg->chol, r, z, skip);
+  PCGB_CHECK_LAUNCH();
+  *nl += 1;
+  return PCGB_OK;
+}
+
+// z = M r: pre-smooth and restrict down to the coarsest level, solve there, prolong and post-smooth back up
+int mg_vcycle(pcgb_mg_t mg, const double *rin, double *zout, cudaStream_t st, int *nl, const int *skip) {
+  const int L = (int)mg->lv.size();
+  for (int l = 0; l + 1 < L; ++l) {
+    MgLevel &A = mg->lv[(size_t)l], &C = mg->lv[(size_t)l + 1];
+    PCGB_TRY(mg_smooth(mg, l, l ? A.b : rin, l ? A.x : zout, true, true, st, nl, skip));
+    k_mg_restrict<<<mg_node_grid(C.g), 256, 0, st>>>(A.g, C.g, A.r, C.b, skip);
+    PCGB_CHECK_LAUNCH();
+    *nl += 1;
+  }
+  PCGB_TRY(mg_coarse_solve(mg, mg->lv.back().b, mg->lv.back().x, st, nl, skip));
+  for (int l = L - 2; l >= 0; --l) {
+    MgLevel &A = mg->lv[(size_t)l], &C = mg->lv[(size_t)l + 1];
+    double *x = l ? A.x : zout;
+    k_mg_prolong_add<<<mg_node_grid(A.g), 256, 0, st>>>(A.g, C.g, C.x, x, skip);
+    PCGB_CHECK_LAUNCH();
+    *nl += 1;
+    PCGB_TRY(mg_smooth(mg, l, l ? A.b : rin, x, false, false, st, nl, skip));
+  }
+  return PCGB_OK;
+}
+
+// z = M r of the solver's current residual, then the (rz, #non-finite z) partials into partials rows dst, dst+1
+int mg_rz(pcgb_solver_t s, pcgb_mg_t mg, const double *w, double *partials, cudaStream_t st, int *nl, const int *skip) {
+  PCGB_TRY(mg_vcycle(mg, s->r, mg->z, st, nl, skip));
+  k_mg_rz<<<vec_grid(s->n), 256, 0, st>>>(skip, s->n, s->r, mg->z, w, partials);
+  PCGB_CHECK_LAUNCH();
+  *nl += 1;
+  return PCGB_OK;
+}
+
 // one PCG iteration enqueued on st (pcg_solver.py:438-562); every kernel no-ops once the state is frozen.
+// mg (one rank only): z = M r by a V-cycle instead of z = Minv .* r: p is updated from the z of the previous iteration
+// (k_pupdate with z in place of r and no Minv), k_update runs without Minv and its z sums (rows 3, 4) are replaced by
+// k_mg_rz after the V-cycle on the new r.
 // ev[0..kEvPerIter): optional events at the phase boundaries of this iteration (time_kernels):
 //   0 start | 1 after p-update | 2 after SpMV (interface tiles when split) | 3 after halo pack | 4 after the interior tiles |
 //   5 after the p.q reduction + all-reduce + alpha | 6 after halo unpack-add | 7 after the fused update | 8 after the norms reduction
 constexpr int kEvPerIter = 9;
 int enqueue_iteration(pcgb_solver_t s, const double *minv, const double *w, double *xb0, double *resvec, cudaStream_t st, int *nl,
-                      cudaEvent_t *ev = nullptr) {
+                      cudaEvent_t *ev = nullptr, pcgb_mg_t mg = nullptr) {
   const int64_t n = s->n;
   const int vg = vec_grid(n);
   const bool multi = multi_rank(s);
   const bool peer = peer_path(s);
 #define PCGB_MARK(k) do { if (ev) PCGB_CUDA(cudaEventRecord(ev[k], st)); } while (0)
   PCGB_MARK(0);
-  k_pupdate<<<vg, kVecBlock, 0, st>>>(s->d_ctrl, n, s->r, minv, s->p);
+  k_pupdate<<<vg, kVecBlock, 0, st>>>(s->d_ctrl, n, mg ? mg->z : s->r, mg ? nullptr : minv, s->p);
   PCGB_CHECK_LAUNCH();
   *nl += 1;
   PCGB_MARK(1);
@@ -1124,9 +1240,10 @@ int enqueue_iteration(pcgb_solver_t s, const double *minv, const double *w, doub
     if (s->halo) PCGB_TRY(halo_exchange_add(s->halo, s->q, st, nl));
     PCGB_MARK(6);
   }
-  k_update<<<vg, kVecBlock, 0, st>>>(s->d_ctrl, n, s->r, s->q, s->p, minv, w, xb0, s->xalt, s->partials);
+  k_update<<<vg, kVecBlock, 0, st>>>(s->d_ctrl, n, s->r, s->q, s->p, mg ? nullptr : minv, w, xb0, s->xalt, s->partials);
   PCGB_CHECK_LAUNCH();
   *nl += 1;
+  if (mg) PCGB_TRY(mg_rz(s, mg, w, s->partials + 3 * kMaxVecGrid, st, nl, &s->d_ctrl->state));
   PCGB_MARK(7);
   if (!multi) {
     k_reduce<5, 2><<<1, 256, 0, st>>>(s->d_ctrl, s->partials, vg, kMaxVecGrid, s->red + 1, resvec);
@@ -1165,7 +1282,7 @@ int pcgb_apply(pcgb_solver_t s, const double *d_x, double *d_y, void *stream) {
 }
 
 static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, const double *d_w, double *d_x,
-                    const pcgb_options *opt, double *d_resvec, pcgb_result *res, cudaStream_t st);
+                    const pcgb_options *opt, double *d_resvec, pcgb_result *res, cudaStream_t st, pcgb_mg_t mg = nullptr);
 
 int pcgb_solve(pcgb_solver_t s, const double *d_b, const double *d_minv, const double *d_w, double *d_x,
                const pcgb_options *opt, double *d_resvec, pcgb_result *res, void *stream) {
@@ -1184,7 +1301,7 @@ int pcgb_solve(pcgb_solver_t s, const double *d_b, const double *d_minv, const d
 }
 
 static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, const double *d_w, double *d_x,
-                    const pcgb_options *opt, double *d_resvec, pcgb_result *res, cudaStream_t st) {
+                    const pcgb_options *opt, double *d_resvec, pcgb_result *res, cudaStream_t st, pcgb_mg_t mg) {
   const int64_t n = s->n;
   const int vg = vec_grid(n);
   memset(res, 0, sizeof(*res));
@@ -1248,7 +1365,7 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
   // (pinned source, stream-ordered: the next write to h_ctrl is the D2H copy of fetch_ctrl on the same stream)
   PCGB_CUDA(cudaMemcpyAsync(s->d_ctrl, s->h_ctrl, sizeof(PcgCtrl), cudaMemcpyHostToDevice, st));
   // head of iteration 0: rho = z.r (:446-469)
-  PCGB_TRY(rz_to_device(s, d_minv, d_w, st));
+  PCGB_TRY(rz_to_device(s, d_minv, d_w, st, mg));
   k_ctrl_head<<<1, 1, 0, st>>>(s->d_ctrl, s->red + 6, 0);
   PCGB_CHECK_LAUNCH();
   s->launches += 1;
@@ -1268,13 +1385,13 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
     if (want_graph && batch > 1) {
       const int variant = (peer_path(s) ? 1 : 0) | ((s->A && spmv_split_available(s->A->P)) ? 2 : 0) | (s->fork_halo ? 4 : 0) |
                           (s->O ? 8 : 0);
-      GraphKey key{d_minv, d_w, xw, d_resvec, batch, variant, s->trace, s->trace_cap};
+      GraphKey key{d_minv, d_w, xw, d_resvec, batch, variant, s->trace, s->trace_cap, mg};
       if (!s->gexec || !(s->gkey == key)) {
         if (s->gexec) { cudaGraphExecDestroy(s->gexec); s->gexec = nullptr; }
         cudaGraph_t graph = nullptr;
         PCGB_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
         int rc = PCGB_OK, nl = 0;
-        for (int k = 0; k < batch && rc == PCGB_OK; ++k) rc = enqueue_iteration(s, d_minv, d_w, xw, d_resvec, st, &nl);
+        for (int k = 0; k < batch && rc == PCGB_OK; ++k) rc = enqueue_iteration(s, d_minv, d_w, xw, d_resvec, st, &nl, nullptr, mg);
         cudaError_t ce = cudaStreamEndCapture(st, &graph);
         if (rc != PCGB_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
         PCGB_CUDA(ce);
@@ -1293,7 +1410,7 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
           while (s->ev_k.size() < (size_t)kEvPerIter * (ktimed + 1)) { cudaEvent_t e; PCGB_CUDA(cudaEventCreate(&e)); s->ev_k.push_back(e); }
           ev = &s->ev_k[(size_t)kEvPerIter * ktimed]; ++ktimed;
         }
-        PCGB_TRY(enqueue_iteration(s, d_minv, d_w, xw, d_resvec, st, &nl, ev));
+        PCGB_TRY(enqueue_iteration(s, d_minv, d_w, xw, d_resvec, st, &nl, ev, mg));
         s->launches += nl;
       }
     }
@@ -1331,7 +1448,7 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
       PCGB_TRY(trace_host(s, TR_VERIFY, c, rr_act, true, nullptr, st));
       *s->h_ctrl = c;
       PCGB_CUDA(cudaMemcpyAsync(s->d_ctrl, s->h_ctrl, sizeof(PcgCtrl), cudaMemcpyHostToDevice, st));
-      PCGB_TRY(rz_to_device(s, d_minv, d_w, st));
+      PCGB_TRY(rz_to_device(s, d_minv, d_w, st, mg));
       k_ctrl_head<<<1, 1, 0, st>>>(s->d_ctrl, s->red + 6, 1);
       PCGB_CHECK_LAUNCH();
       s->launches += 1;
@@ -1411,6 +1528,320 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
   res->matvecs = matvecs + (int64_t)(c.iter + 1);
   res->launches = s->launches + graph_launch_kernels;
   return PCGB_OK;
+}
+
+// ------------------------------------------------------------------------------------ geometric multigrid (hex boxes)
+int pcgb_mg_destroy(pcgb_mg_t mg) {
+  if (!mg) return PCGB_OK;
+  // The solver's cached graph of MG iterations holds this handle's buffers and coefficients as kernel arguments, and its key
+  // knows the handle only by address, which a later pcgb_mg_create may receive again: drop the graph with the handle.
+  pcgb_solver_t s = mg->s;
+  if (s && s->gexec && s->gkey.mg == mg) {
+    cudaGraphExecDestroy(s->gexec);
+    s->gexec = nullptr;
+    s->gkey = GraphKey{nullptr, nullptr, nullptr, nullptr, 0, 0, nullptr, 0, nullptr};
+  }
+  for (size_t l = 0; l < mg->lv.size(); ++l) {
+    MgLevel &L = mg->lv[l];
+    if (L.has_plan) free_plan(L.P);
+    cudaFree(L.rowptr); cudaFree(L.col); cudaFree(L.val); cudaFree(L.dinv);
+    if (l > 0) { cudaFree(L.b); cudaFree(L.x); }
+    cudaFree(L.r); cudaFree(L.d); cudaFree(L.q);
+  }
+  cudaFree(mg->chol); cudaFree(mg->z); cudaFree(mg->partials); cudaFree(mg->red); cudaFree(mg->d_bad);
+  if (mg->h_red) cudaFreeHost(mg->h_red);
+  delete mg;
+  return PCGB_OK;
+}
+
+namespace {
+// Stiffness matrix of level L's box as device CSR (int64 row offsets; the caller frees them): k_hex_count, a host scan,
+// k_hex_fill with Ck = ck
+int mg_hex_csr(const HexGeom &g, const double *ke_host, double ck, int64_t **rp, int **col, double **val, int64_t *nnz) {
+  const int64_t n = 3 * g.nfree_nodes;
+  std::vector<int64_t> cnt((size_t)n + 1);
+  PCGB_CUDA(cudaMalloc(rp, (size_t)(n + 1) * sizeof(int64_t)));
+  k_hex_count<<<(unsigned)((g.nfree_nodes + 255) / 256), 256>>>(g, *rp);
+  PCGB_CHECK_LAUNCH();
+  PCGB_CUDA(cudaMemcpy(cnt.data(), *rp, cnt.size() * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  for (size_t i = 1; i < cnt.size(); ++i) cnt[i] += cnt[i - 1];
+  *nnz = cnt.back();
+  PCGB_CUDA(cudaMemcpy(*rp, cnt.data(), cnt.size() * sizeof(int64_t), cudaMemcpyHostToDevice));
+  PCGB_CUDA(cudaMalloc(col, (size_t)*nnz * sizeof(int)));
+  PCGB_CUDA(cudaMalloc(val, (size_t)*nnz * sizeof(double)));
+  PCGB_CUDA(cudaMemcpyToSymbol(c_hex_ke, ke_host, 24 * 24 * sizeof(double)));
+  k_hex_fill<<<(unsigned)((g.nfree_nodes * 32 + 255) / 256), 256>>>(g, ck, *rp, *col, *val);
+  PCGB_CHECK_LAUNCH();
+  return PCGB_OK;
+}
+
+// largest eigenvalue of the symmetric tridiagonal matrix (diagonal a, off-diagonal b) by bisection on the Sturm count
+double tridiag_max_eig(const std::vector<double> &a, const std::vector<double> &b) {
+  const size_t k = a.size();
+  double lo = 0.0, hi = 0.0;
+  for (size_t i = 0; i < k; ++i) {
+    const double r = (i > 0 ? std::fabs(b[i - 1]) : 0.0) + (i + 1 < k ? std::fabs(b[i]) : 0.0);
+    if (!std::isfinite(a[i]) || !std::isfinite(r)) return NAN;
+    lo = i ? std::min(lo, a[i] - r) : a[i] - r;
+    hi = i ? std::max(hi, a[i] + r) : a[i] + r;
+  }
+  for (int it = 0; it < 200 && lo < hi; ++it) {
+    const double mid = 0.5 * (lo + hi);
+    if (mid <= lo || mid >= hi) break;
+    size_t below = 0;   // eigenvalues < mid: sign changes of the LDL^T pivots of T - mid I
+    double d = 1.0;
+    for (size_t i = 0; i < k; ++i) {
+      d = a[i] - mid - (i ? b[i - 1] * b[i - 1] / d : 0.0);
+      if (d == 0.0) d = -1e-300;
+      if (d < 0.0) ++below;
+    }
+    if (below == k) hi = mid; else lo = mid;
+  }
+  return hi;
+}
+
+// largest eigenvalue of D^-1 A on level l: kMgLanczosSteps Lanczos steps (D inner product) from a fixed start vector, the
+// largest eigenvalue of their tridiagonal matrix.  Then the Chebyshev coefficients of the level.
+int mg_estimate(pcgb_mg_t mg, int l) {
+  MgLevel &L = mg->lv[(size_t)l];
+  const int grid = vec_grid(L.n);
+  int nl = 0;
+  auto fetch = [&](double *out) -> int {
+    k_reduce<1, 0><<<1, 256>>>(nullptr, mg->partials, grid, kMaxVecGrid, mg->red, nullptr);
+    PCGB_CHECK_LAUNCH();
+    PCGB_CUDA(cudaMemcpy(mg->h_red, mg->red, sizeof(double), cudaMemcpyDeviceToHost));
+    *out = mg->h_red[0];
+    return PCGB_OK;
+  };
+  PCGB_CUDA(cudaMemset(L.d, 0, (size_t)L.n * sizeof(double)));
+  k_mg_lanczos_start<<<grid, 256>>>(L.n, L.q);
+  k_mg_lanczos_w<<<grid, 256>>>(L.n, L.q, nullptr, nullptr, L.dinv, 0.0, 0.0, 0, L.r, mg->partials);
+  PCGB_CHECK_LAUNCH();
+  double bb = 0.0;
+  PCGB_TRY(fetch(&bb));
+  double beta = std::sqrt(bb);
+  k_mg_lanczos_next<<<grid, 256>>>(L.n, 1.0 / beta, L.d, L.r);   // v1 = start / |start|_D, v0 = 0
+  PCGB_CHECK_LAUNCH();
+  std::vector<double> al, be;
+  beta = 0.0;
+  for (int it = 0; it < kMgLanczosSteps; ++it) {
+    PCGB_TRY(mg_op(mg, l, L.d, L.q, 0, &nl, nullptr));
+    k_dot_w<<<grid, kVecBlock>>>(L.n, L.d, L.q, nullptr, mg->partials);
+    PCGB_CHECK_LAUNCH();
+    double alpha = 0.0;
+    PCGB_TRY(fetch(&alpha));
+    al.push_back(alpha);
+    if (it + 1 == kMgLanczosSteps) break;
+    k_mg_lanczos_w<<<grid, 256>>>(L.n, L.q, L.d, L.r, L.dinv, alpha, beta, 1, L.r, mg->partials);
+    PCGB_CHECK_LAUNCH();
+    PCGB_TRY(fetch(&bb));
+    beta = std::sqrt(bb);
+    if (!(beta > 0.0) || !std::isfinite(beta)) {   // invariant subspace (or a non-finite Minv)
+      if (!std::isfinite(beta)) al.back() = NAN;
+      break;
+    }
+    be.push_back(beta);
+    k_mg_lanczos_next<<<grid, 256>>>(L.n, 1.0 / beta, L.d, L.r);
+    PCGB_CHECK_LAUNCH();
+  }
+  L.lambda = tridiag_max_eig(al, be);
+  // Chebyshev on [lo, 1.1] * lambda: theta = centre, delta = half width, sigma = theta / delta
+  const double a = mg->lo * L.lambda, b = 1.1 * L.lambda;
+  const double theta = 0.5 * (b + a), delta = 0.5 * (b - a), sigma = theta / delta;
+  double rho = 1.0 / sigma;
+  L.inv_theta = 1.0 / theta;
+  for (int j = 1; j < mg->degree; ++j) {
+    const double rn = 1.0 / (2.0 * sigma - rho);
+    L.c1.push_back(rn * rho);
+    L.c2.push_back(2.0 * rn / delta);
+    rho = rn;
+  }
+  return PCGB_OK;
+}
+
+int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const double *d_minv_fine,
+             const std::vector<HexGeom> &geo) {
+  const int nlev = (int)geo.size();
+  auto alloc = [&](double **p, int64_t n) -> cudaError_t {
+    mg->bytes += 8 * n;
+    return cudaMalloc(p, (size_t)std::max<int64_t>(n, 1) * sizeof(double));
+  };
+  mg->lv.resize((size_t)nlev);
+  // set-up runs on the legacy stream, which does not wait for non-blocking streams: finish whatever work of the caller may
+  // still be writing d_minv_fine (or the operator's arrays) before the first read
+  PCGB_CUDA(cudaDeviceSynchronize());
+  PCGB_CUDA(cudaMallocHost(&mg->h_red, 4 * sizeof(double)));
+  PCGB_CUDA(cudaMalloc(&mg->partials, kMaxVecGrid * sizeof(double)));
+  PCGB_CUDA(cudaMalloc(&mg->red, 4 * sizeof(double)));
+  PCGB_CUDA(cudaMalloc(&mg->d_bad, sizeof(int)));
+  PCGB_CUDA(cudaMemset(mg->d_bad, 0, sizeof(int)));
+  for (int l = 0; l < nlev; ++l) {
+    MgLevel &L = mg->lv[(size_t)l];
+    L.g = geo[(size_t)l];
+    L.n = 3 * L.g.nfree_nodes;
+    const double ck = E * h * (double)(1ll << l);
+    if (l == 0) {
+      PCGB_CUDA(alloc(&mg->z, L.n));
+      PCGB_CUDA(alloc(&L.dinv, L.n));
+      PCGB_CUDA(cudaMemcpy(L.dinv, d_minv_fine, (size_t)L.n * sizeof(double), cudaMemcpyDeviceToDevice));
+    } else {
+      PCGB_CUDA(alloc(&L.b, L.n));
+      PCGB_CUDA(alloc(&L.x, L.n));
+    }
+    if (l == nlev - 1) {   // coarsest: dense Cholesky factor of its matrix
+      int64_t *rp = nullptr, nnz = 0;
+      int *col = nullptr;
+      double *val = nullptr;
+      int rc = mg_hex_csr(L.g, ke_host, ck, &rp, &col, &val, &nnz);
+      mg->nc = (int)L.n;
+      if (rc == PCGB_OK && alloc(&mg->chol, L.n * L.n) == cudaSuccess && cudaMemset(mg->chol, 0, (size_t)(L.n * L.n) * sizeof(double)) == cudaSuccess) {
+        k_mg_densify<<<(unsigned)((L.n + 255) / 256), 256>>>(L.n, rp, col, val, mg->chol);
+        k_mg_chol_factor<<<1, kMgCholThreads>>>(mg->nc, mg->chol, mg->d_bad);
+        if (cudaGetLastError() != cudaSuccess) rc = fail(PCGB_ERR_CUDA, "pcgb_mg_create: coarse factorisation launch failed");
+      } else if (rc == PCGB_OK) {
+        rc = fail(PCGB_ERR_CUDA, "pcgb_mg_create: coarse matrix allocation failed");
+      }
+      cudaDeviceSynchronize();
+      cudaFree(rp); cudaFree(col); cudaFree(val);
+      PCGB_TRY(rc);
+      int bad = 0;
+      PCGB_CUDA(cudaMemcpy(&bad, mg->d_bad, sizeof(int), cudaMemcpyDeviceToHost));
+      if (bad) return fail(PCGB_ERR_ARG, "pcgb_mg_create: the coarsest matrix is not positive definite");
+      break;
+    }
+    PCGB_CUDA(alloc(&L.r, L.n));
+    PCGB_CUDA(alloc(&L.d, L.n));
+    PCGB_CUDA(alloc(&L.q, L.n));
+    if (l > 0) {
+      int64_t *rp = nullptr, nnz = 0;
+      const int rc = mg_hex_csr(L.g, ke_host, ck, &rp, &L.col, &L.val, &nnz);
+      L.rowptr = rp;
+      PCGB_TRY(rc);
+      mg->bytes += 12 * nnz + 8 * (L.n + 1);
+      L.P.nrows = L.n; L.P.ncols = L.n; L.P.nnz = nnz; L.P.rowptr = rp; L.P.rp64 = true; L.P.col = L.col; L.P.val = L.val;
+      if (nnz < INT32_MAX) {   // int32 row offsets, as the fine hex matrices use below 2^31 non-zeros
+        std::vector<int64_t> r64((size_t)L.n + 1);
+        PCGB_CUDA(cudaMemcpy(r64.data(), rp, r64.size() * sizeof(int64_t), cudaMemcpyDeviceToHost));
+        std::vector<int32_t> r32(r64.begin(), r64.end());
+        int32_t *rp32 = nullptr;
+        PCGB_CUDA(upload(&rp32, r32));
+        cudaFree(rp);
+        L.rowptr = rp32; L.P.rowptr = rp32; L.P.rp64 = false;
+        mg->bytes -= 4 * (L.n + 1);
+      }
+      L.has_plan = true;
+      PCGB_TRY(L.P.rp64 ? build_plan_t<int64_t>(L.P, 0) : build_plan_t<int32_t>(L.P, 0));
+      PCGB_CUDA(alloc(&L.dinv, L.n));
+      PCGB_TRY(csr_diag_compute(L.P, L.r, 0));
+      k_reciprocal<<<vec_grid(L.n), 256>>>(L.n, L.r, L.dinv);
+      PCGB_CHECK_LAUNCH();
+    }
+    PCGB_TRY(mg_estimate(mg, l));
+  }
+  PCGB_CUDA(cudaDeviceSynchronize());
+  return PCGB_OK;
+}
+}  // namespace
+
+int pcgb_mg_create(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, const double *d_minv_fine,
+                   int degree, double lo, pcgb_mg_t *out) {
+  PCGB_TRY(require_device());
+  if (!s || !box || !ke_host || !d_minv_fine || !out) return fail(PCGB_ERR_ARG, "pcgb_mg_create: null argument");
+  if (s->halo || s->comm) return fail(PCGB_ERR_ARG, "pcgb_mg_create: one rank only (the solver has a halo plan or a communicator)");
+  if (degree < 1 || !(lo > 0.0 && lo < 1.1) || !(E > 0.0) || !(h > 0.0))
+    return fail(PCGB_ERR_ARG, "pcgb_mg_create: degree >= 1, 0 < lo < 1.1, E > 0 and h > 0 required");
+  for (int a = 0; a < 3; ++a)
+    if (box->e0[a] != 0 || box->ng[a] != box->ne[a] || box->ne[a] <= 0)
+      return fail(PCGB_ERR_ARG, "pcgb_mg_create: the box must be the whole mesh (e0 = 0, ng = ne)");
+  std::vector<HexGeom> geo{hex_geom(box)};
+  if (3 * geo[0].nfree_nodes != s->n) return fail(PCGB_ERR_ARG, "pcgb_mg_create: the solver's operator has %lld rows, the box %lld",
+                                                  (long long)s->n, (long long)(3 * geo[0].nfree_nodes));
+  for (;;) {
+    HexGeom g = geo.back();
+    if (g.nx % 2 || g.ny % 2 || g.nz % 2 || g.nx < 4 || g.ny < 4 || g.nz < 4) break;
+    pcgb_hex_box cb = *box;
+    const int ne[3] = {g.nx, g.ny, g.nz};
+    for (int a = 0; a < 3; ++a) { cb.ne[a] = ne[a] / 2; cb.ng[a] = cb.ne[a]; }
+    geo.push_back(hex_geom(&cb));
+  }
+  if (geo.size() < 2) return fail(PCGB_ERR_ARG, "pcgb_mg_create: the box does not coarsen (every ne must be even and >= 4)");
+  if (3 * geo.back().nfree_nodes > kMgMaxCoarse)
+    return fail(PCGB_ERR_ARG, "pcgb_mg_create: the coarsest level has %lld dofs (at most %d)", (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
+  if (geo.size() > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "pcgb_mg_create: more than %d levels", PCGB_MG_MAX_LEVELS);
+  pcgb_mg_t mg = new pcgb_mg_s();
+  mg->s = s; mg->degree = degree; mg->lo = lo;
+  const int rc = mg_build(mg, ke_host, E, h, d_minv_fine, geo);
+  if (rc != PCGB_OK) { pcgb_mg_destroy(mg); return rc; }
+  *out = mg;
+  return PCGB_OK;
+}
+
+int pcgb_mg_apply(pcgb_mg_t mg, const double *d_r, double *d_z, void *stream) {
+  PCGB_TRY(require_device());
+  if (!mg || !d_r || !d_z) return fail(PCGB_ERR_ARG, "pcgb_mg_apply: null argument");
+  int nl = 0;
+  return mg_vcycle(mg, d_r, d_z, (cudaStream_t)stream, &nl, nullptr);
+}
+
+int pcgb_mg_info(pcgb_mg_t mg, int32_t *nlevels, int64_t *n_level, double *lambda, int64_t *bytes) {
+  PCGB_TRY(require_device());
+  if (!mg) return fail(PCGB_ERR_ARG, "pcgb_mg_info: null argument");
+  if (nlevels) *nlevels = (int32_t)mg->lv.size();
+  for (size_t l = 0; l < mg->lv.size(); ++l) {
+    if (n_level) n_level[l] = mg->lv[l].n;
+    if (lambda) lambda[l] = mg->lv[l].lambda;
+  }
+  if (bytes) *bytes = mg->bytes;
+  return PCGB_OK;
+}
+
+int pcgb_mg_restrict(pcgb_mg_t mg, int level, const double *d_fine, double *d_coarse, void *stream) {
+  PCGB_TRY(require_device());
+  if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || !d_fine || !d_coarse) return fail(PCGB_ERR_ARG, "pcgb_mg_restrict: bad argument");
+  const MgLevel &F = mg->lv[(size_t)level], &C = mg->lv[(size_t)level + 1];
+  k_mg_restrict<<<mg_node_grid(C.g), 256, 0, (cudaStream_t)stream>>>(F.g, C.g, d_fine, d_coarse, nullptr);
+  PCGB_CHECK_LAUNCH();
+  return PCGB_OK;
+}
+
+int pcgb_mg_prolong_add(pcgb_mg_t mg, int level, const double *d_coarse, double *d_fine, void *stream) {
+  PCGB_TRY(require_device());
+  if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || !d_fine || !d_coarse) return fail(PCGB_ERR_ARG, "pcgb_mg_prolong_add: bad argument");
+  const MgLevel &F = mg->lv[(size_t)level], &C = mg->lv[(size_t)level + 1];
+  k_mg_prolong_add<<<mg_node_grid(F.g), 256, 0, (cudaStream_t)stream>>>(F.g, C.g, d_coarse, d_fine, nullptr);
+  PCGB_CHECK_LAUNCH();
+  return PCGB_OK;
+}
+
+int pcgb_mg_smooth(pcgb_mg_t mg, int level, const double *d_b, double *d_x, void *stream) {
+  PCGB_TRY(require_device());
+  if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || !d_b || !d_x) return fail(PCGB_ERR_ARG, "pcgb_mg_smooth: bad argument");
+  int nl = 0;
+  return mg_smooth(mg, level, d_b, d_x, false, false, (cudaStream_t)stream, &nl, nullptr);
+}
+
+int pcgb_mg_coarse_solve(pcgb_mg_t mg, const double *d_r, double *d_z, void *stream) {
+  PCGB_TRY(require_device());
+  if (!mg || !d_r || !d_z) return fail(PCGB_ERR_ARG, "pcgb_mg_coarse_solve: null argument");
+  int nl = 0;
+  return mg_coarse_solve(mg, d_r, d_z, (cudaStream_t)stream, &nl, nullptr);
+}
+
+int pcgb_solve_mg(pcgb_solver_t s, pcgb_mg_t mg, const double *d_b, const double *d_w, double *d_x, const pcgb_options *opt,
+                  double *d_resvec, pcgb_result *res, void *stream) {
+  PCGB_TRY(require_device());
+  if (!s || !mg || !d_b || !d_x || !opt || !res) return fail(PCGB_ERR_ARG, "pcgb_solve_mg: null argument");
+  if (mg->s != s) return fail(PCGB_ERR_ARG, "pcgb_solve_mg: the preconditioner was built for another solver");
+  if (opt->maxiter <= 0) return fail(PCGB_ERR_ARG, "pcgb_solve_mg: maxiter must be positive");
+  cudaStream_t user = (cudaStream_t)stream;
+  PCGB_CUDA(cudaEventRecord(s->ev_in, user));
+  PCGB_CUDA(cudaStreamWaitEvent(s->own, s->ev_in, 0));
+  const int rc = solve_on(s, d_b, nullptr, d_w, d_x, opt, d_resvec, res, s->own, mg);
+  if (rc == PCGB_OK) {
+    PCGB_CUDA(cudaEventRecord(s->ev_out, s->own));
+    PCGB_CUDA(cudaStreamWaitEvent(user, s->ev_out, 0));
+  }
+  return rc;
 }
 
 // ------------------------------------------------------------------------------------ hex generator

@@ -10,7 +10,8 @@ Mapping of solve()'s arguments onto the reference's per-rank state:
     A        K[Eff,Eff] of this rank (CsrMatrix / SubdomainOperator with its halo plan)
     b        Fext[LocDofEff]
     M        InvDiagPreCondVector0 (the INVERSE diagonal, applied as z = M*r, :447); None = identity
-             (ExistDP0 False, :451); the string "jacobi" builds it from A like updatePreconditioner
+             (ExistDP0 False, :451); the string "jacobi" builds it from A like updatePreconditioner;
+             a multigrid.HexMultigrid built on A applies z = M r as one V-cycle (opt-in, one rank)
     tol      GlobData['Tol']        maxiter  GlobData['MaxIter']
     x0       Un[LocDofEff]          w        DofWeightVector_Eff (taken from the operator if omitted)
 Return value (x, flag, relres, iters) follows MATLAB pcg like the reference: flag 0 converged,
@@ -155,7 +156,7 @@ class SolveInfo:
     stag: int = 0
     moresteps: int = 0
     too_small_tol: bool = False
-    matvecs: int = 0
+    matvecs: int = 0                     # operator applications of the loop (with a HexMultigrid M, not the V-cycles')
     launches: int = 0
     loop_ms: float = 0.0
     spmv_ms: float = 0.0
@@ -163,7 +164,7 @@ class SolveInfo:
     loop_iters: int = 0
     setup_ms: float = 0.0
     final_ms: float = 0.0
-    phase_ms: dict | None = None
+    phase_ms: dict | None = None         # with a HexMultigrid M, 'fused_update' includes the V-cycle
     resvec: np.ndarray | None = None
     trace: np.ndarray | None = None      # TRACE_DTYPE records (trace=...)
     trace_total: int = 0                 # records the solve produced (> len(trace) when some were dropped)
@@ -265,8 +266,12 @@ class SubdomainOperator:
 
         trace: record every control step of the loop (True = room for 3*maxiter+8 records, an int = that capacity) into
         info.trace; snapshot (with trace): the loop's vectors at its exit into info.snapshot.  Tracing is switched off
-        again when the call returns."""
+        again when the call returns.  M may be a multigrid.HexMultigrid built on this operator (z = M r by a V-cycle)."""
+        from .multigrid import HexMultigrid
         lib = _lib.load()
+        mg = M if isinstance(M, HexMultigrid) else None
+        if mg is not None and mg.op is not self:
+            raise ValueError("solve: the HexMultigrid was built on another operator")
         dev = self.device
         assert b.is_cuda and b.dtype == torch.float64 and b.numel() == self.n
         x = x0.clone() if x0 is not None else torch.zeros(self.n, dtype=torch.float64, device=dev)
@@ -292,8 +297,12 @@ class SubdomainOperator:
             if tracing:
                 _lib.check(lib.pcgb_solver_set_trace(self._solver, _lib.ptr(tr), cap, _lib.ptr(snap)), "pcgb_solver_set_trace")
             try:
-                _lib.check(lib.pcgb_solve(self._solver, _lib.ptr(b), _lib.ptr(M), _lib.ptr(w), _lib.ptr(x), ctypes.byref(opt),
-                                          _lib.ptr(resvec), ctypes.byref(res), _lib.stream_ptr()), "pcgb_solve")
+                if mg is not None:
+                    _lib.check(lib.pcgb_solve_mg(self._solver, mg.handle, _lib.ptr(b), _lib.ptr(w), _lib.ptr(x), ctypes.byref(opt),
+                                                 _lib.ptr(resvec), ctypes.byref(res), _lib.stream_ptr()), "pcgb_solve_mg")
+                else:
+                    _lib.check(lib.pcgb_solve(self._solver, _lib.ptr(b), _lib.ptr(M), _lib.ptr(w), _lib.ptr(x), ctypes.byref(opt),
+                                              _lib.ptr(resvec), ctypes.byref(res), _lib.stream_ptr()), "pcgb_solve")
             finally:
                 if tracing:
                     _lib.check(lib.pcgb_solver_set_trace(self._solver, None, 0, None), "pcgb_solver_set_trace")
@@ -363,7 +372,12 @@ def solve(A, b, M=None, tol: float = 1e-8, maxiter: int = 10000, x0=None, w=None
             return torch.from_numpy(np.ascontiguousarray(v, dtype=np.float64)).to(op.device, non_blocking=True)
         return v.to(op.device, torch.float64).contiguous()
 
-    if isinstance(M, str):
+    from .multigrid import HexMultigrid
+    if isinstance(M, HexMultigrid):
+        if M.op is not op:
+            raise ValueError("solve: M is a HexMultigrid built on another operator; pass that operator as A")
+        Md = M
+    elif isinstance(M, str):
         if M.lower() != "jacobi":
             raise ValueError("solve: M must be an inverse-diagonal vector, None or 'jacobi'")
         Md = op.jacobi()
