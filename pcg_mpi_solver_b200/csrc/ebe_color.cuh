@@ -21,7 +21,6 @@ struct EbeLaunch {
 struct EbeColorPlan {
   EbePlan P;                       // groups (one per pattern group x colour), device tables
   std::vector<EbeLaunch> launches; // in phase order
-  int nphases = 0;
 };
 
 template <bool SIGN>

@@ -41,24 +41,39 @@ struct pcgb_ebe_ordered_s {
   int device = 0;
 };
 
+// What may differ between two solves on one handle and changes the captured iterations (the operator, the x buffers and
+// PCGB_FORK are fixed when the solver is created).
 struct GraphKey {
-  const void *minv, *w, *xb0, *resvec;
-  int iters;
-  int variant;   // what the captured iteration looks like: bit 0 peer transport, bit 1 interface-first split, bit 2 forked unpack,
-                 // bit 3 ordered matrix-free product
-  const void *trace;   // trace buffer and capacity (kernel arguments of the captured trace records; NULL = tracing off)
-  long long trace_cap;
-  const void *mg;      // multigrid preconditioner of the captured V-cycles (NULL = diagonal Minv)
+  const void *minv = nullptr, *w = nullptr, *resvec = nullptr;
+  int iters = 0;
+  bool peer = false;              // peer transport
+  bool split = false;             // the product runs interface-first (split_product)
+  const void *trace = nullptr;    // trace buffer and capacity (kernel arguments of the captured trace records; NULL = tracing off)
+  long long trace_cap = 0;
+  const void *mg = nullptr;       // multigrid preconditioner of the captured V-cycles (NULL = diagonal Minv)
   bool operator==(const GraphKey &o) const {
-    return minv == o.minv && w == o.w && xb0 == o.xb0 && resvec == o.resvec && iters == o.iters && variant == o.variant &&
+    return minv == o.minv && w == o.w && resvec == o.resvec && iters == o.iters && peer == o.peer && split == o.split &&
            trace == o.trace && trace_cap == o.trace_cap && mg == o.mg;
   }
 };
 
-struct pcgb_solver_s {
+// The solver's operator K: exactly one handle is set.  rows() and apply() are the only code that asks which; the iteration's
+// product reads A for the CSR dot partials and the interface-first split.
+struct FineOp {
   pcgb_csr_t A = nullptr;
-  pcgb_ebe_t E = nullptr;       // opt-in matrix-free operator (exactly one of A / E / O is set)
-  pcgb_ebe_ordered_t O = nullptr;  // opt-in matrix-free operator with a fixed summation order
+  pcgb_ebe_t E = nullptr;           // opt-in matrix-free operator
+  pcgb_ebe_ordered_t O = nullptr;   // opt-in matrix-free operator with a fixed summation order
+  int64_t rows() const { return A ? A->P.nrows : E ? E->P.n : O->O.P.n; }
+  // y = K x, without the interface sum
+  int apply(const double *x, double *y, cudaStream_t st, int *nl, const int *skip) const {
+    if (E) return ebe_apply(E->P, x, y, st, nl, skip);
+    if (O) return ebo_apply(O->O, x, y, st, nl, skip);
+    return spmv_launch(A->P, x, y, false, st, nl, skip);
+  }
+};
+
+struct pcgb_solver_s {
+  FineOp op;
   pcgb_halo_t halo = nullptr;
   pcgb_comm_t comm = nullptr;
   int64_t n = 0;
@@ -76,7 +91,7 @@ struct pcgb_solver_s {
   cudaEvent_t ev_in = nullptr, ev_out = nullptr, ev_l0 = nullptr, ev_l1 = nullptr, ev_s0 = nullptr, ev_s1 = nullptr;
   std::vector<cudaEvent_t> ev_k;  // SpMV brackets (time_kernels)
   cudaGraphExec_t gexec = nullptr;
-  GraphKey gkey{nullptr, nullptr, nullptr, nullptr, 0, 0, nullptr, 0, nullptr};
+  GraphKey gkey;
   int launches = 0;             // launches issued outside graphs (running counter per solve)
   int launches_per_iter = 0;
   bool fork_halo = true;        // PCGB_FORK=0 keeps the unpack on the main stream
@@ -282,11 +297,12 @@ int pcgb_spmv_split(pcgb_csr_t A, const double *d_x, double *d_y, double *d_out_
 }
 
 // ------------------------------------------------------------------------------------ vector kernels
-static int reduce_rows(const double *partials, int count, int nv, double *d_out, cudaStream_t st) {
+// sum `nv` (1, 2 or 5) rows, `row_stride` apart, of the partials of `count` blocks into d_out[0 .. nv)
+static int reduce_rows(const double *partials, int count, int row_stride, int nv, double *d_out, cudaStream_t st) {
   switch (nv) {
-    case 1: k_reduce<1, 0><<<1, 256, 0, st>>>(nullptr, partials, count, kMaxVecGrid, d_out, nullptr); break;
-    case 2: k_reduce<2, 0><<<1, 256, 0, st>>>(nullptr, partials, count, kMaxVecGrid, d_out, nullptr); break;
-    default: k_reduce<5, 0><<<1, 256, 0, st>>>(nullptr, partials, count, kMaxVecGrid, d_out, nullptr); break;
+    case 1: k_reduce<1, 0><<<1, 256, 0, st>>>(nullptr, partials, count, row_stride, d_out, nullptr); break;
+    case 2: k_reduce<2, 0><<<1, 256, 0, st>>>(nullptr, partials, count, row_stride, d_out, nullptr); break;
+    default: k_reduce<5, 0><<<1, 256, 0, st>>>(nullptr, partials, count, row_stride, d_out, nullptr); break;
   }
   PCGB_CHECK_LAUNCH();
   return PCGB_OK;
@@ -301,7 +317,7 @@ int pcgb_dot_w(int64_t n, const double *d_a, const double *d_b, const double *d_
   PCGB_CUDA(cudaMallocAsync(&scratch, kMaxVecGrid * sizeof(double), st));
   const int grid = vec_grid(n);
   k_dot_w<<<grid, kVecBlock, 0, st>>>(n, d_a, d_b, d_w, scratch);
-  int rc = cudaGetLastError() == cudaSuccess ? reduce_rows(scratch, grid, 1, d_out, st) : fail(PCGB_ERR_CUDA, "pcgb_dot_w: launch failed");
+  int rc = cudaGetLastError() == cudaSuccess ? reduce_rows(scratch, grid, kMaxVecGrid, 1, d_out, st) : fail(PCGB_ERR_CUDA, "pcgb_dot_w: launch failed");
   cudaFreeAsync(scratch, st);
   return rc;
 }
@@ -572,44 +588,50 @@ int64_t pcgb_halo_bytes(pcgb_halo_t h) { return h ? h->m * 8 : 0; }
 
 }  // extern "C"
 
-// Groups of an EBE plan (atomic or ordered operator): device copies of Ke, constant-memory slots of the 24-dof patterns,
-// the warp-kernel block tables.  On failure P holds what was acquired so far, which ebe_plan_free releases.
+// The caller's pattern group g: a size of 1..max_nd, at most max_ne elements, and the arrays its elements need.
+static int check_group(const pcgb_ebe_group &src, int g, int max_nd, int64_t max_ne, const char *who) {
+  if (src.nd <= 0 || src.nd > max_nd || src.ne < 0 || src.ne > max_ne || !src.ke_host || (src.ne > 0 && (!src.d_idx || !src.d_ck)))
+    return fail(PCGB_ERR_ARG, "%s: group %d: pattern size must be 1..%d and arrays non-null", who, g, max_nd);
+  return PCGB_OK;
+}
+
+// device copy of the group's pattern matrix Ke (nd x nd)
+static int upload_ke(const pcgb_ebe_group &src, const double **d_ke, const char *who) {
+  const size_t bytes = (size_t)src.nd * src.nd * sizeof(double);
+  double *d = nullptr;
+  cudaError_t ce = cudaMalloc(&d, bytes);
+  if (ce == cudaSuccess) ce = cudaMemcpy(d, src.ke_host, bytes, cudaMemcpyHostToDevice);
+  if (ce != cudaSuccess) { cudaFree(d); return fail(PCGB_ERR_CUDA, "%s: %s", who, cudaGetErrorString(ce)); }
+  *d_ke = d;
+  return PCGB_OK;
+}
+
+// Groups of an EBE plan (atomic, ordered or coloured operator): device copies of Ke, constant-memory slots of the 24-dof
+// patterns, the warp-kernel block tables (blocks in group order).  On failure P holds what was acquired so far, which
+// ebe_plan_free releases.
 static int ebe_plan_build(EbePlan &P, int64_t n, int ngroups, const pcgb_ebe_group *groups, const char *who) {
   P.n = n;
   std::vector<int> blk_group;
   std::vector<int64_t> blk_e0;
   P.bytes = 16 * n;
-  int rc = PCGB_OK;
-  cudaError_t ce = cudaSuccess;
-  for (int g = 0; g < ngroups && rc == PCGB_OK; ++g) {
+  for (int g = 0; g < ngroups; ++g) {
     const pcgb_ebe_group &src = groups[g];
-    if (src.nd <= 0 || src.nd > 96 || src.ne < 0 || !src.ke_host || (src.ne > 0 && (!src.d_idx || !src.d_ck))) {
-      rc = fail(PCGB_ERR_ARG, "%s: group %d: pattern size must be 1..96 and arrays non-null", who, g);
-      break;
-    }
+    PCGB_TRY(check_group(src, g, 96, INT64_MAX, who));
     EbeGroup eg;
     eg.nd = src.nd; eg.ne = src.ne; eg.idx = src.d_idx; eg.sign = src.d_sign; eg.ck = src.d_ck;
-    double *dke = nullptr;
-    if ((ce = cudaMalloc(&dke, (size_t)src.nd * src.nd * sizeof(double))) != cudaSuccess ||
-        (ce = cudaMemcpy(dke, src.ke_host, (size_t)src.nd * src.nd * sizeof(double), cudaMemcpyHostToDevice)) != cudaSuccess) {
-      cudaFree(dke);
-      rc = fail(PCGB_ERR_CUDA, "%s: %s", who, cudaGetErrorString(ce));
-      break;
-    }
-    eg.ke = dke;
+    PCGB_TRY(upload_ke(src, &eg.ke, who));
     if (src.nd == 24) eg.slot = ebe_slot_acquire(src.ke_host);
     if (eg.slot < 0)
       for (int64_t e0 = 0; e0 < src.ne; e0 += kEbeWarpsPerBlock) { blk_group.push_back((int)P.groups.size()); blk_e0.push_back(e0); }
     P.bytes += src.ne * ((int64_t)src.nd * (4 + (src.d_sign ? 1 : 0)) + 8);
     P.groups.push_back(eg);
   }
-  if (rc == PCGB_OK) {
-    P.nblk_warp = (int)blk_group.size();
-    if ((ce = upload(&P.d_groups, P.groups)) != cudaSuccess || (ce = upload(&P.d_blk_group, blk_group)) != cudaSuccess ||
-        (ce = upload(&P.d_blk_e0, blk_e0)) != cudaSuccess)
-      rc = fail(PCGB_ERR_CUDA, "%s: %s", who, cudaGetErrorString(ce));
-  }
-  return rc;
+  P.nblk_warp = (int)blk_group.size();
+  cudaError_t ce = cudaSuccess;
+  if ((ce = upload(&P.d_groups, P.groups)) != cudaSuccess || (ce = upload(&P.d_blk_group, blk_group)) != cudaSuccess ||
+      (ce = upload(&P.d_blk_e0, blk_e0)) != cudaSuccess)
+    return fail(PCGB_ERR_CUDA, "%s: %s", who, cudaGetErrorString(ce));
+  return PCGB_OK;
 }
 
 static void ebe_plan_free(EbePlan &P, int device) {
@@ -657,8 +679,7 @@ int pcgb_ebe_ordered_create(int64_t n, int ngroups, const pcgb_ebe_group *groups
   int64_t nslots = 0;
   for (int g = 0; g < ngroups; ++g) {
     const pcgb_ebe_group &src = groups[g];
-    if (src.nd <= 0 || src.nd > 96 || src.ne < 0 || !src.ke_host || (src.ne > 0 && (!src.d_idx || !src.d_ck)))
-      return fail(PCGB_ERR_ARG, "pcgb_ebe_ordered_create: group %d: pattern size must be 1..96 and arrays non-null", g);
+    PCGB_TRY(check_group(src, g, 96, INT64_MAX, "pcgb_ebe_ordered_create"));
     if (src.ne > INT32_MAX || (nslots += (int64_t)src.nd * src.ne) > INT32_MAX)
       return fail(PCGB_ERR_ARG, "pcgb_ebe_ordered_create: 2^31 or more element slots (slot positions are int32)");
   }
@@ -705,18 +726,11 @@ int pcgb_assemble_symbolic(int64_t n, int ngroups, const pcgb_ebe_group *groups,
   int rc = PCGB_OK;
   for (int g = 0; g < ngroups && rc == PCGB_OK; ++g) {
     const pcgb_ebe_group &src = groups[g];
-    if (src.nd <= 0 || src.nd > 255 || src.ne < 0 || src.ne >= (1ll << 40) || !src.ke_host || (src.ne > 0 && (!src.d_idx || !src.d_ck))) {
-      rc = fail(PCGB_ERR_ARG, "pcgb_assemble_symbolic: group %d: pattern size must be 1..255 and arrays non-null", g);
-      break;
-    }
     AsmGroup ag;
     ag.nd = src.nd; ag.ne = src.ne; ag.idx = src.d_idx; ag.sign = src.d_sign; ag.ck = src.d_ck;
-    double *dke = nullptr;
-    cudaError_t ce = cudaMalloc(&dke, (size_t)src.nd * src.nd * sizeof(double));
-    if (ce == cudaSuccess) ce = cudaMemcpy(dke, src.ke_host, (size_t)src.nd * src.nd * sizeof(double), cudaMemcpyHostToDevice);
-    if (ce != cudaSuccess) { cudaFree(dke); rc = fail(PCGB_ERR_CUDA, "pcgb_assemble_symbolic: %s", cudaGetErrorString(ce)); break; }
-    ag.ke = dke;
-    a->P.groups.push_back(ag);
+    if ((rc = check_group(src, g, 255, (1ll << 40) - 1, "pcgb_assemble_symbolic")) == PCGB_OK &&
+        (rc = upload_ke(src, &ag.ke, "pcgb_assemble_symbolic")) == PCGB_OK)
+      a->P.groups.push_back(ag);
   }
   if (rc == PCGB_OK) rc = asm_symbolic(a->P, d_rowptr, (cudaStream_t)stream);
   if (rc != PCGB_OK) { pcgb_assemble_destroy(a); return rc; }
@@ -739,69 +753,7 @@ int pcgb_assemble_destroy(pcgb_asm_t a) {
 
 // ------------------------------------------------------------------------------------ coloured EBE operator (operator level)
 // groups[] holds one entry per (pattern group, colour), sorted by colour; phase[g] is the colour.  Pattern matrices of
-// the 24-dof groups are de-duplicated into the constant-memory slots by content of ke_host (same pointer = same slot).
-// Fills E; on failure E holds exactly what was acquired so far (slots, device copies), which pcgb_ebe2_destroy releases.
-static int ebe2_build(pcgb_ebe2_t E, int64_t n, int ngroups, const pcgb_ebe_group *groups, const int32_t *phase) {
-  EbePlan &P = E->C.P;
-  P.n = n;
-  P.bytes = 16 * n;
-  std::vector<int> blk_group;
-  std::vector<int64_t> blk_e0;
-  std::vector<std::pair<const double *, double *>> ke_dev;   // host pointer -> device copy (shared between colours)
-  int open_warp_phase = -1, open_warp_begin = 0;
-  auto flush_warp = [&]() {
-    if (open_warp_phase >= 0 && (int)blk_group.size() > open_warp_begin) E->C.launches.push_back({1, open_warp_begin, (int)blk_group.size()});
-    open_warp_phase = -1;
-  };
-  for (int g = 0; g < ngroups; ++g) {
-    const pcgb_ebe_group &src = groups[g];
-    if (src.nd <= 0 || src.nd > 96 || src.ne < 0 || !src.ke_host || (src.ne > 0 && (!src.d_idx || !src.d_ck)))
-      return fail(PCGB_ERR_ARG, "pcgb_ebe2_create: group %d: pattern size must be 1..96 and arrays non-null", g);
-    EbeGroup eg;
-    eg.nd = src.nd; eg.ne = src.ne; eg.idx = src.d_idx; eg.sign = src.d_sign; eg.ck = src.d_ck;
-    double *dke = nullptr;
-    for (auto &kv : ke_dev) if (kv.first == src.ke_host) dke = kv.second;
-    if (!dke) {
-      PCGB_CUDA(cudaMalloc(&dke, (size_t)src.nd * src.nd * sizeof(double)));
-      const cudaError_t ce = cudaMemcpy(dke, src.ke_host, (size_t)src.nd * src.nd * sizeof(double), cudaMemcpyHostToDevice);
-      if (ce != cudaSuccess) { cudaFree(dke); return fail(PCGB_ERR_CUDA, "pcgb_ebe2_create: %s", cudaGetErrorString(ce)); }
-      ke_dev.push_back({src.ke_host, dke});
-    }
-    eg.ke = dke;
-    bool t24 = false;
-    if (src.nd == 24) {
-      const int slot = ebe_slot_acquire(src.ke_host);   // shared per-device table: never overwrites a live operator's matrices
-      if (slot >= 0) { eg.slot = slot; t24 = true; }
-    }
-    if (t24) {
-      if (open_warp_phase >= 0 && open_warp_phase != phase[g]) flush_warp();
-      if (src.ne > 0) E->C.launches.push_back({0, (int)P.groups.size(), 0});
-    } else {
-      if (open_warp_phase >= 0 && open_warp_phase != phase[g]) flush_warp();
-      if (open_warp_phase < 0) { open_warp_phase = phase[g]; open_warp_begin = (int)blk_group.size(); }
-      for (int64_t e0 = 0; e0 < src.ne; e0 += kEbeWarpsPerBlock) { blk_group.push_back((int)P.groups.size()); blk_e0.push_back(e0); }
-    }
-    P.bytes += src.ne * ((int64_t)src.nd * (4 + (src.d_sign ? 1 : 0)) + 8);
-    P.groups.push_back(eg);
-    E->C.nphases = phase[g] + 1;
-  }
-  flush_warp();
-  // a t24 launch of phase c and a warp launch of the same phase may touch the same dofs only if the colouring was
-  // done per pattern group; the Python side colours ALL elements of the subdomain together, so they cannot.
-  if (!P.groups.empty()) {
-    PCGB_CUDA(cudaMalloc(&P.d_groups, P.groups.size() * sizeof(EbeGroup)));
-    PCGB_CUDA(cudaMemcpy(P.d_groups, P.groups.data(), P.groups.size() * sizeof(EbeGroup), cudaMemcpyHostToDevice));
-  }
-  P.nblk_warp = (int)blk_group.size();
-  if (P.nblk_warp > 0) {
-    PCGB_CUDA(cudaMalloc(&P.d_blk_group, blk_group.size() * sizeof(int)));
-    PCGB_CUDA(cudaMalloc(&P.d_blk_e0, blk_e0.size() * sizeof(int64_t)));
-    PCGB_CUDA(cudaMemcpy(P.d_blk_group, blk_group.data(), blk_group.size() * sizeof(int), cudaMemcpyHostToDevice));
-    PCGB_CUDA(cudaMemcpy(P.d_blk_e0, blk_e0.data(), blk_e0.size() * sizeof(int64_t), cudaMemcpyHostToDevice));
-  }
-  return PCGB_OK;
-}
-
+// the 24-dof groups are de-duplicated into the constant-memory slots by content of ke_host.
 int pcgb_ebe2_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, const int32_t *phase, pcgb_ebe2_t *out) {
   if (!out || n < 0 || ngroups < 0 || (ngroups > 0 && (!groups || !phase))) return fail(PCGB_ERR_ARG, "pcgb_ebe2_create: bad argument");
   if (n >= (1 << 30)) return fail(PCGB_ERR_ARG, "pcgb_ebe2_create: more than 2^30 dofs");
@@ -810,22 +762,29 @@ int pcgb_ebe2_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, const
     if (phase[g] < phase[g - 1]) return fail(PCGB_ERR_ARG, "pcgb_ebe2_create: groups must be sorted by phase (colour)");
   pcgb_ebe2_t E = new pcgb_ebe2_s();
   cudaGetDevice(&E->device);
-  const int rc = ebe2_build(E, n, ngroups, groups, phase);
+  const int rc = ebe_plan_build(E->C.P, n, ngroups, groups, "pcgb_ebe2_create");
   if (rc != PCGB_OK) { pcgb_ebe2_destroy(E); return rc; }
+  // Launches in colour order: the colour's t24 groups in group order, then one warp launch over the colour's blocks, which
+  // are contiguous in the block tables because the groups arrive sorted by colour.  A t24 launch and a warp launch of one
+  // colour may touch the same dofs only if the colouring was done per pattern group; the Python side colours ALL elements
+  // of the subdomain together, so they cannot.
+  int blk = 0;
+  for (int g = 0; g < ngroups;) {
+    const int blk0 = blk;
+    for (const int c = phase[g]; g < ngroups && phase[g] == c; ++g) {
+      const EbeGroup &eg = E->C.P.groups[(size_t)g];
+      if (eg.slot < 0) blk += (int)((eg.ne + kEbeWarpsPerBlock - 1) / kEbeWarpsPerBlock);
+      else if (eg.ne > 0) E->C.launches.push_back({0, g, 0});
+    }
+    if (blk > blk0) E->C.launches.push_back({1, blk0, blk});
+  }
   *out = E;
   return PCGB_OK;
 }
 
 int pcgb_ebe2_destroy(pcgb_ebe2_t E) {
   if (!E) return PCGB_OK;
-  std::vector<const double *> freed;
-  for (EbeGroup &g : E->C.P.groups) {
-    bool done = false;
-    for (const double *f : freed) done |= (f == g.ke);
-    if (!done) { cudaFree(const_cast<double *>(g.ke)); freed.push_back(g.ke); }
-    ebe_slot_release(E->device, g.slot);
-  }
-  cudaFree(E->C.P.d_groups); cudaFree(E->C.P.d_blk_group); cudaFree(E->C.P.d_blk_e0);
+  ebe_plan_free(E->C.P, E->device);
   delete E;
   return PCGB_OK;
 }
@@ -838,14 +797,14 @@ int pcgb_ebe2_apply(pcgb_ebe2_t E, const double *d_x, double *d_y, void *stream)
 int pcgb_ebe2_launches(pcgb_ebe2_t E) { return E ? (int)E->C.launches.size() : 0; }
 
 // ------------------------------------------------------------------------------------ solver
-static int solver_create_common(pcgb_csr_t A, pcgb_ebe_t E, pcgb_ebe_ordered_t O, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
+static int solver_create_common(FineOp op, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
   if (halo && !comm) comm = halo->comm;
   PCGB_TRY(require_device());
   pcgb_solver_t s = new pcgb_solver_s();
-  s->A = A; s->E = E; s->O = O; s->halo = halo; s->comm = comm; s->n = A ? A->P.nrows : E ? E->P.n : O->O.P.n;
+  s->op = op; s->halo = halo; s->comm = comm; s->n = op.rows();
   s->fork_halo = env_int("PCGB_FORK", 1) != 0;
   const size_t nb = (size_t)(s->n > 0 ? s->n : 1) * sizeof(double);
-  s->stage_cap = ((A ? A->P.ntiles : 0) + 4095) / 4096 + 1;
+  s->stage_cap = ((op.A ? op.A->P.ntiles : 0) + 4095) / 4096 + 1;
   cudaError_t ce = cudaSuccess;
   int rc = PCGB_OK;
   if ((ce = cudaMalloc(&s->r, nb)) == cudaSuccess && (ce = cudaMalloc(&s->p, nb)) == cudaSuccess &&
@@ -869,8 +828,8 @@ static int solver_create_common(pcgb_csr_t A, pcgb_ebe_t E, pcgb_ebe_ordered_t O
   // interface-first tile order: the tiles owning exchanged rows run first, their values travel while the rest computes
   // Opt-in (PCGB_OVERLAP=1): with the peer-store halo the exchange costs a few microseconds and is not worth a second
   // persistent launch (measured slower than the unsplit launch at 2 GPUs, 128^3 per GPU).
-  if (rc == PCGB_OK && A && halo && halo->ndof > 0 && env_int("PCGB_OVERLAP", 0) != 0)
-    rc = spmv_set_boundary_rows(A->P, halo->d_dof, halo->ndof, s->own);
+  if (rc == PCGB_OK && op.A && halo && halo->ndof > 0 && env_int("PCGB_OVERLAP", 0) != 0)
+    rc = spmv_set_boundary_rows(op.A->P, halo->d_dof, halo->ndof, s->own);
   if (rc != PCGB_OK) { pcgb_solver_destroy(s); return rc; }
   *out = s;
   return PCGB_OK;
@@ -879,17 +838,17 @@ static int solver_create_common(pcgb_csr_t A, pcgb_ebe_t E, pcgb_ebe_ordered_t O
 int pcgb_solver_create(pcgb_csr_t A, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
   if (!A || !out) return fail(PCGB_ERR_ARG, "pcgb_solver_create: null argument");
   if (A->P.nrows != A->P.ncols) return fail(PCGB_ERR_ARG, "pcgb_solver_create: operator must be square");
-  return solver_create_common(A, nullptr, nullptr, halo, comm, out);
+  return solver_create_common(FineOp{A}, halo, comm, out);
 }
 
 int pcgb_solver_create_ebe(pcgb_ebe_t E, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
   if (!E || !out) return fail(PCGB_ERR_ARG, "pcgb_solver_create_ebe: null argument");
-  return solver_create_common(nullptr, E, nullptr, halo, comm, out);
+  return solver_create_common(FineOp{nullptr, E}, halo, comm, out);
 }
 
 int pcgb_solver_create_ebe_ordered(pcgb_ebe_ordered_t O, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
   if (!O || !out) return fail(PCGB_ERR_ARG, "pcgb_solver_create_ebe_ordered: null argument");
-  return solver_create_common(nullptr, nullptr, O, halo, comm, out);
+  return solver_create_common(FineOp{nullptr, nullptr, O}, halo, comm, out);
 }
 
 int pcgb_solver_destroy(pcgb_solver_t s) {
@@ -935,16 +894,14 @@ inline bool peer_path(pcgb_solver_t s) { return multi_rank(s) && s->comm->use_pe
 
 // y = A x + interface sum  (calcMPFint, pcg_solver.py:339-342)
 int op_apply(pcgb_solver_t s, const double *x, double *y, cudaStream_t st) {
-  if (s->E) PCGB_TRY(ebe_apply(s->E->P, x, y, st, &s->launches));
-  else if (s->O) PCGB_TRY(ebo_apply(s->O->O, x, y, st, &s->launches));
-  else PCGB_TRY(spmv_launch(s->A->P, x, y, false, st, &s->launches));
+  PCGB_TRY(s->op.apply(x, y, st, &s->launches, nullptr));
   if (s->halo) PCGB_TRY(halo_exchange_add(s->halo, y, st, &s->launches));
   return PCGB_OK;
 }
 
 // sum `nv` (<= 2) rows of s->partials over blocks and ranks into the device scalars s->red[dst .. dst+nv)
 int reduce_to_device(pcgb_solver_t s, int count, int nv, int dst, cudaStream_t st) {
-  PCGB_TRY(reduce_rows(s->partials, count, nv, s->red + dst, st));
+  PCGB_TRY(reduce_rows(s->partials, count, kMaxVecGrid, nv, s->red + dst, st));
   s->launches += 1;
   if (multi_rank(s)) {
     PCGB_TRY(allreduce_sum(s->comm, s->red + dst, nv, st));
@@ -978,32 +935,13 @@ int true_residual(pcgb_solver_t s, const double *b, const double *w, const doubl
   return PCGB_OK;
 }
 
-// (sum z.(r w), #inf z) of the current r into s->red[6..7] (device, all-reduced)
-int mg_rz(pcgb_solver_t s, pcgb_mg_t mg, const double *w, double *partials, cudaStream_t st, int *nl, const int *skip);
-
-// (mg: z = M r by the V-cycle, the same launches as inside the iteration)
-int rz_to_device(pcgb_solver_t s, const double *minv, const double *w, cudaStream_t st, pcgb_mg_t mg = nullptr) {
-  const int grid = vec_grid(s->n);
-  if (mg) {
-    PCGB_TRY(mg_rz(s, mg, w, s->partials, st, &s->launches, &s->d_ctrl->state));
-    return reduce_to_device(s, grid, 2, 6, st);
-  }
-  k_rz<<<grid, kVecBlock, 0, st>>>(s->n, s->r, minv, w, s->partials);
-  PCGB_CHECK_LAUNCH();
-  s->launches += 1;
-  return reduce_to_device(s, grid, 2, 6, st);
-}
-
 // ---- trace (pcgb_solver_set_trace): extra launches only when tracing is on
 inline int trace_rank(pcgb_solver_t s) { return s->comm ? s->comm->rank : 0; }
 // this rank's sum of `nv` rows of the partials of `count` blocks into tr_local[dst..) (the same code as the local half of the
 // all-reduce, hence the same bits)
 int trace_local(pcgb_solver_t s, const double *partials, int count, int row_stride, int nv, int dst, cudaStream_t st, int *nl) {
   if (!s->trace || !multi_rank(s)) return PCGB_OK;
-  if (nv == 1) k_reduce<1, 0><<<1, 256, 0, st>>>(nullptr, partials, count, row_stride, s->tr_local + dst, nullptr);
-  else if (nv == 2) k_reduce<2, 0><<<1, 256, 0, st>>>(nullptr, partials, count, row_stride, s->tr_local + dst, nullptr);
-  else k_reduce<5, 0><<<1, 256, 0, st>>>(nullptr, partials, count, row_stride, s->tr_local + dst, nullptr);
-  PCGB_CHECK_LAUNCH();
+  PCGB_TRY(reduce_rows(partials, count, row_stride, nv, s->tr_local + dst, st));
   *nl += 1;
   return PCGB_OK;
 }
@@ -1062,10 +1000,7 @@ constexpr int kMgLanczosSteps = 20;
 
 int mg_op(pcgb_mg_t mg, int l, const double *x, double *y, cudaStream_t st, int *nl, const int *skip) {
   if (l > 0) return spmv_launch(mg->lv[(size_t)l].P, x, y, false, st, nl, skip);
-  pcgb_solver_t s = mg->s;
-  if (s->E) return ebe_apply(s->E->P, x, y, st, nl, skip);
-  if (s->O) return ebo_apply(s->O->O, x, y, st, nl, skip);
-  return spmv_launch(s->A->P, x, y, false, st, nl, skip);
+  return mg->s->op.apply(x, y, st, nl, skip);
 }
 
 // Chebyshev smoothing of D^-1 A on level l: zero_start: x = S b (no operator application for x = 0); otherwise
@@ -1129,72 +1064,92 @@ int mg_rz(pcgb_solver_t s, pcgb_mg_t mg, const double *w, double *partials, cuda
   return PCGB_OK;
 }
 
-// one PCG iteration enqueued on st (pcg_solver.py:438-562); every kernel no-ops once the state is frozen.
-// mg (one rank only): z = M r by a V-cycle instead of z = Minv .* r: p is updated from the z of the previous iteration
-// (k_pupdate with z in place of r and no Minv), k_update runs without Minv and its z sums (rows 3, 4) are replaced by
-// k_mg_rz after the V-cycle on the new r.
-// ev[0..kEvPerIter): optional events at the phase boundaries of this iteration (time_kernels):
+// Head of an iteration (pcg_solver.py:446-469) with the loop state c: rho = z.r, with z = Minv .* r or, with mg, z = M r
+// by the V-cycle (the same launches as inside the iteration).  resume = 0 for iteration 0 (the trace record carries bb and
+// r0r0), 1 after a failed verification.
+int enqueue_head(pcgb_solver_t s, const PcgCtrl &c, const double *minv, const double *w, pcgb_mg_t mg, int resume, double bb,
+                 double r0r0, cudaStream_t st) {
+  const int grid = vec_grid(s->n);
+  *s->h_ctrl = c;
+  // (pinned source, stream-ordered: the next write to h_ctrl is the D2H copy of fetch_ctrl on the same stream)
+  PCGB_CUDA(cudaMemcpyAsync(s->d_ctrl, s->h_ctrl, sizeof(PcgCtrl), cudaMemcpyHostToDevice, st));
+  if (mg) {
+    PCGB_TRY(mg_rz(s, mg, w, s->partials, st, &s->launches, &s->d_ctrl->state));
+  } else {
+    k_rz<<<grid, kVecBlock, 0, st>>>(s->n, s->r, minv, w, s->partials);
+    PCGB_CHECK_LAUNCH();
+    s->launches += 1;
+  }
+  PCGB_TRY(reduce_to_device(s, grid, 2, 6, st));
+  k_ctrl_head<<<1, 1, 0, st>>>(s->d_ctrl, s->red + 6, resume);
+  PCGB_CHECK_LAUNCH();
+  s->launches += 1;
+  PCGB_TRY(trace_local(s, s->partials, grid, kMaxVecGrid, 2, 4, st, &s->launches));
+  return trace_step(s, resume ? TR_RESUME : TR_HEAD, bb, r0r0, st, &s->launches);
+}
+
+// ev[0..kEvPerIter): optional events at the phase boundaries of an iteration (time_kernels):
 //   0 start | 1 after p-update | 2 after SpMV (interface tiles when split) | 3 after halo pack | 4 after the interior tiles |
 //   5 after the p.q reduction + all-reduce + alpha | 6 after halo unpack-add | 7 after the fused update | 8 after the norms reduction
 constexpr int kEvPerIter = 9;
-int enqueue_iteration(pcgb_solver_t s, const double *minv, const double *w, double *xb0, double *resvec, cudaStream_t st, int *nl,
-                      cudaEvent_t *ev = nullptr, pcgb_mg_t mg = nullptr) {
-  const int64_t n = s->n;
-  const int vg = vec_grid(n);
-  const bool multi = multi_rank(s);
-  const bool peer = peer_path(s);
 #define PCGB_MARK(k) do { if (ev) PCGB_CUDA(cudaEventRecord(ev[k], st)); } while (0)
-  PCGB_MARK(0);
-  k_pupdate<<<vg, kVecBlock, 0, st>>>(s->d_ctrl, n, mg ? mg->z : s->r, mg ? nullptr : minv, s->p);
-  PCGB_CHECK_LAUNCH();
-  *nl += 1;
-  PCGB_MARK(1);
-  // p.q : per-tile partials -> (stage) -> scalar.  In the multi-GPU case the partials are those of the
-  // UNASSEMBLED local product, whose rank sum equals the reference's weighted dot of the assembled q
-  // (p is consistent on shared dofs and K = sum of the subdomain matrices); see DESIGN.md.
-  const double *pq_src;
-  int pq_cnt;
-  bool halo_done = false;
-  if (s->E || s->O) {  // matrix-free operator: product, then a separate unweighted dot of the local product
-    if (s->E) PCGB_TRY(ebe_apply(s->E->P, s->p, s->q, st, nl, &s->d_ctrl->state));
-    else PCGB_TRY(ebo_apply(s->O->O, s->p, s->q, st, nl, &s->d_ctrl->state));
+
+// the CSR product of an iteration runs interface-first: interface tiles -> halo pack -> interior tiles
+inline bool split_product(pcgb_solver_t s, bool peer) {
+  return peer && s->op.A && s->halo && s->halo->m > 0 && spmv_split_available(s->op.A->P);
+}
+
+// q = K p of an iteration (marks 2-4) and the partials of p.q it leaves: *src, *count.  *packed: the halo pack of q is
+// enqueued.  In the multi-GPU case the partials are those of the UNASSEMBLED local product, whose rank sum equals the
+// reference's weighted dot of the assembled q (p is consistent on shared dofs and K = sum of the subdomain matrices); see
+// DESIGN.md.
+int enqueue_product(pcgb_solver_t s, bool peer, cudaStream_t st, int *nl, cudaEvent_t *ev, const double **src, int *count,
+                    bool *packed) {
+  const int *skip = &s->d_ctrl->state;
+  *packed = false;
+  if (!s->op.A) {  // matrix-free operator: product, then a separate unweighted dot of the local product
+    PCGB_TRY(s->op.apply(s->p, s->q, st, nl, skip));
     PCGB_MARK(2); PCGB_MARK(3); PCGB_MARK(4);
-    k_dot_w<<<vg, kVecBlock, 0, st>>>(n, s->p, s->q, nullptr, s->partials);
+    const int vg = vec_grid(s->n);
+    k_dot_w<<<vg, kVecBlock, 0, st>>>(s->n, s->p, s->q, nullptr, s->partials);
     PCGB_CHECK_LAUNCH();
     *nl += 1;
-    pq_src = s->partials; pq_cnt = vg;
-  } else {
-    const CsrPlan &P = s->A->P;
-    if (peer && s->halo && s->halo->m > 0 && spmv_split_available(P)) {
-      // interface tiles -> pack (peer stores fly over NVLink) -> interior tiles; the unpack follows the p.q all-reduce
-      PCGB_TRY(spmv_launch_part(P, 0, s->p, s->q, true, st, nl, &s->d_ctrl->state));
-      PCGB_MARK(2);
-      PCGB_TRY(halo_pack(s->halo, s->q, st, nl));
-      PCGB_MARK(3);
-      PCGB_TRY(spmv_launch_part(P, 1, s->p, s->q, true, st, nl, &s->d_ctrl->state));
-      PCGB_MARK(4);
-      pq_src = P.dot_partials_split; pq_cnt = spmv_split_dot_count(P);
-      halo_done = true;
-    } else {
-      PCGB_TRY(spmv_launch(P, s->p, s->q, true, st, nl, &s->d_ctrl->state));
-      PCGB_MARK(2);
-      if (peer && s->halo) { PCGB_TRY(halo_pack(s->halo, s->q, st, nl)); halo_done = true; }
-      PCGB_MARK(3); PCGB_MARK(4);
-      pq_src = P.dot_partials;
-      pq_cnt = P.persist ? P.grid_persist : P.ntiles;
-      if (pq_cnt > 8192) {
-        const int sb = (pq_cnt + 4095) / 4096;
-        k_stage_reduce<<<sb, 256, 0, st>>>(P.dot_partials, pq_cnt, s->stage);
-        PCGB_CHECK_LAUNCH();
-        *nl += 1;
-        pq_src = s->stage; pq_cnt = sb;
-      }
-    }
+    *src = s->partials; *count = vg;
+    return PCGB_OK;
   }
+  const CsrPlan &P = s->op.A->P;
+  if (split_product(s, peer)) {   // the peer stores of the pack fly over NVLink; the unpack follows the p.q all-reduce
+    PCGB_TRY(spmv_launch_part(P, 0, s->p, s->q, true, st, nl, skip));
+    PCGB_MARK(2);
+    PCGB_TRY(halo_pack(s->halo, s->q, st, nl));
+    PCGB_MARK(3);
+    PCGB_TRY(spmv_launch_part(P, 1, s->p, s->q, true, st, nl, skip));
+    PCGB_MARK(4);
+    *src = P.dot_partials_split; *count = spmv_split_dot_count(P); *packed = true;
+    return PCGB_OK;
+  }
+  PCGB_TRY(spmv_launch(P, s->p, s->q, true, st, nl, skip));
+  PCGB_MARK(2);
+  if (peer && s->halo) { PCGB_TRY(halo_pack(s->halo, s->q, st, nl)); *packed = true; }
+  PCGB_MARK(3); PCGB_MARK(4);
+  // per-tile partials -> (stage) -> scalar
+  *src = P.dot_partials;
+  *count = P.persist ? P.grid_persist : P.ntiles;
+  if (*count > 8192) {
+    const int sb = (*count + 4095) / 4096;
+    k_stage_reduce<<<sb, 256, 0, st>>>(P.dot_partials, *count, s->stage);
+    PCGB_CHECK_LAUNCH();
+    *nl += 1;
+    *src = s->stage; *count = sb;
+  }
+  return PCGB_OK;
+}
+
+// p.q over blocks and ranks into red[0] and alpha (mark 5), then the halo unpack-add of q (mark 6)
+int pq_reduce(pcgb_solver_t s, bool peer, const double *src, int count, bool packed, cudaStream_t st, int *nl, cudaEvent_t *ev) {
   if (peer) {
     // own kernels over peer memory: the all-reduce is fused into the reduction kernel, the scalar logic follows in the same CTA
-    if (s->halo && !halo_done) PCGB_TRY(halo_pack(s->halo, s->q, st, nl));
-    const PeerWin win = s->comm->window();
+    if (s->halo && !packed) PCGB_TRY(halo_pack(s->halo, s->q, st, nl));
     // fork: the unpack-add of the interface values (waits for the neighbours' stores) runs beside the p.q all-reduce (waits
     // for the other ranks' sums); both only need the pack above, which never waits - so no order of execution can deadlock
     const bool fork = s->halo && s->halo->m > 0 && s->side != nullptr && s->fork_halo;
@@ -1204,48 +1159,45 @@ int enqueue_iteration(pcgb_solver_t s, const double *minv, const double *w, doub
       PCGB_TRY(halo_unpack(s->halo, s->q, s->side, nl));
       PCGB_CUDA(cudaEventRecord(s->ev_join, s->side));
     }
-    k_reduce_ar<1, 1><<<1, 256, 0, st>>>(win, s->d_ctrl, pq_src, pq_cnt, 0, s->red, nullptr);
+    k_reduce_ar<1, 1><<<1, 256, 0, st>>>(s->comm->window(), s->d_ctrl, src, count, 0, s->red, nullptr);
     PCGB_CHECK_LAUNCH();
     *nl += 1;
-    PCGB_TRY(trace_local(s, pq_src, pq_cnt, 0, 1, 0, st, nl));   // before k_update: the EBE dot partials share s->partials
+    PCGB_TRY(trace_local(s, src, count, 0, 1, 0, st, nl));   // before k_update: the EBE dot partials share s->partials
     PCGB_MARK(5);
     if (fork) PCGB_CUDA(cudaStreamWaitEvent(st, s->ev_join, 0));
     else if (s->halo) PCGB_TRY(halo_unpack(s->halo, s->q, st, nl));
-    PCGB_MARK(6);
-    k_update<<<vg, kVecBlock, 0, st>>>(s->d_ctrl, n, s->r, s->q, s->p, minv, w, xb0, s->xalt, s->partials);
-    PCGB_CHECK_LAUNCH();
-    PCGB_MARK(7);
-    k_reduce_ar<5, 2><<<1, 256, 0, st>>>(win, s->d_ctrl, s->partials, vg, kMaxVecGrid, s->red + 1, resvec);
-    PCGB_CHECK_LAUNCH();
-    *nl += 2;
-    PCGB_MARK(8);
-    PCGB_TRY(trace_local(s, s->partials, vg, kMaxVecGrid, 5, 1, st, nl));
-    return trace_step(s, TR_ITER, 0.0, 0.0, st, nl);
-  }
-  if (!multi) {
-    k_reduce<1, 1><<<1, 256, 0, st>>>(s->d_ctrl, pq_src, pq_cnt, 0, s->red, nullptr);
+  } else if (!multi_rank(s)) {
+    k_reduce<1, 1><<<1, 256, 0, st>>>(s->d_ctrl, src, count, 0, s->red, nullptr);
     PCGB_CHECK_LAUNCH();
     *nl += 1;
-    PCGB_MARK(5); PCGB_MARK(6);
+    PCGB_MARK(5);
   } else {
     // NCCL transport: reduction, ncclAllReduce and the scalar logic are three stream operations; the halo is serial
-    k_reduce<1, 0><<<1, 256, 0, st>>>(s->d_ctrl, pq_src, pq_cnt, 0, s->red, nullptr);
+    k_reduce<1, 0><<<1, 256, 0, st>>>(s->d_ctrl, src, count, 0, s->red, nullptr);
     PCGB_CHECK_LAUNCH();
-    PCGB_TRY(trace_local(s, pq_src, pq_cnt, 0, 1, 0, st, nl));
+    PCGB_TRY(trace_local(s, src, count, 0, 1, 0, st, nl));
     PCGB_TRY(allreduce_sum(s->comm, s->red, 1, st));
     k_ctrl_alpha<<<1, 1, 0, st>>>(s->d_ctrl, s->red);
     PCGB_CHECK_LAUNCH();
     *nl += 2;
     PCGB_MARK(5);
     if (s->halo) PCGB_TRY(halo_exchange_add(s->halo, s->q, st, nl));
-    PCGB_MARK(6);
   }
-  k_update<<<vg, kVecBlock, 0, st>>>(s->d_ctrl, n, s->r, s->q, s->p, mg ? nullptr : minv, w, xb0, s->xalt, s->partials);
-  PCGB_CHECK_LAUNCH();
-  *nl += 1;
-  if (mg) PCGB_TRY(mg_rz(s, mg, w, s->partials + 3 * kMaxVecGrid, st, nl, &s->d_ctrl->state));
-  PCGB_MARK(7);
-  if (!multi) {
+  PCGB_MARK(6);
+  return PCGB_OK;
+}
+
+// pp, xx, rr, rz, #inf over blocks and ranks into red[1..6) and the control step that consumes them (mark 8)
+int norms_reduce(pcgb_solver_t s, bool peer, double *resvec, cudaStream_t st, int *nl, cudaEvent_t *ev) {
+  const int vg = vec_grid(s->n);
+  if (peer) {
+    k_reduce_ar<5, 2><<<1, 256, 0, st>>>(s->comm->window(), s->d_ctrl, s->partials, vg, kMaxVecGrid, s->red + 1, resvec);
+    PCGB_CHECK_LAUNCH();
+    *nl += 1;
+    PCGB_MARK(8);
+    return trace_local(s, s->partials, vg, kMaxVecGrid, 5, 1, st, nl);
+  }
+  if (!multi_rank(s)) {
     k_reduce<5, 2><<<1, 256, 0, st>>>(s->d_ctrl, s->partials, vg, kMaxVecGrid, s->red + 1, resvec);
     PCGB_CHECK_LAUNCH();
     *nl += 1;
@@ -1259,9 +1211,36 @@ int enqueue_iteration(pcgb_solver_t s, const double *minv, const double *w, doub
     *nl += 2;
   }
   PCGB_MARK(8);
-#undef PCGB_MARK
+  return PCGB_OK;
+}
+
+// one PCG iteration enqueued on st (pcg_solver.py:438-562); every kernel no-ops once the state is frozen.
+// mg (one rank only): z = M r by a V-cycle instead of z = Minv .* r: p is updated from the z of the previous iteration
+// (k_pupdate with z in place of r and no Minv), k_update runs without Minv and its z sums (rows 3, 4) are replaced by
+// k_mg_rz after the V-cycle on the new r.
+int enqueue_iteration(pcgb_solver_t s, const double *minv, const double *w, double *resvec, cudaStream_t st, int *nl,
+                      cudaEvent_t *ev, pcgb_mg_t mg) {
+  const int vg = vec_grid(s->n);
+  const bool peer = peer_path(s);
+  PCGB_MARK(0);
+  k_pupdate<<<vg, kVecBlock, 0, st>>>(s->d_ctrl, s->n, mg ? mg->z : s->r, mg ? nullptr : minv, s->p);
+  PCGB_CHECK_LAUNCH();
+  *nl += 1;
+  PCGB_MARK(1);
+  const double *pq_src = nullptr;
+  int pq_cnt = 0;
+  bool packed = false;
+  PCGB_TRY(enqueue_product(s, peer, st, nl, ev, &pq_src, &pq_cnt, &packed));
+  PCGB_TRY(pq_reduce(s, peer, pq_src, pq_cnt, packed, st, nl, ev));
+  k_update<<<vg, kVecBlock, 0, st>>>(s->d_ctrl, s->n, s->r, s->q, s->p, mg ? nullptr : minv, w, s->xown, s->xalt, s->partials);
+  PCGB_CHECK_LAUNCH();
+  *nl += 1;
+  if (mg) PCGB_TRY(mg_rz(s, mg, w, s->partials + 3 * kMaxVecGrid, st, nl, &s->d_ctrl->state));
+  PCGB_MARK(7);
+  PCGB_TRY(norms_reduce(s, peer, resvec, st, nl, ev));
   return trace_step(s, TR_ITER, 0.0, 0.0, st, nl);
 }
+#undef PCGB_MARK
 
 int fetch_ctrl(pcgb_solver_t s, cudaStream_t st) {
   PCGB_CUDA(cudaMemcpyAsync(s->h_ctrl, s->d_ctrl, sizeof(PcgCtrl), cudaMemcpyDeviceToHost, st));
@@ -1279,25 +1258,6 @@ extern "C" {
 int pcgb_apply(pcgb_solver_t s, const double *d_x, double *d_y, void *stream) {
   if (!s || !d_x || !d_y) return fail(PCGB_ERR_ARG, "pcgb_apply: null argument");
   return op_apply(s, d_x, d_y, (cudaStream_t)stream);
-}
-
-static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, const double *d_w, double *d_x,
-                    const pcgb_options *opt, double *d_resvec, pcgb_result *res, cudaStream_t st, pcgb_mg_t mg = nullptr);
-
-int pcgb_solve(pcgb_solver_t s, const double *d_b, const double *d_minv, const double *d_w, double *d_x,
-               const pcgb_options *opt, double *d_resvec, pcgb_result *res, void *stream) {
-  if (!s || !d_b || !d_x || !opt || !res) return fail(PCGB_ERR_ARG, "pcgb_solve: null argument");
-  if (opt->maxiter <= 0) return fail(PCGB_ERR_ARG, "pcgb_solve: maxiter must be positive");
-  // order the solver's own stream after the caller's stream, run, and order the caller's stream after us
-  cudaStream_t user = (cudaStream_t)stream;
-  PCGB_CUDA(cudaEventRecord(s->ev_in, user));
-  PCGB_CUDA(cudaStreamWaitEvent(s->own, s->ev_in, 0));
-  const int rc = solve_on(s, d_b, d_minv, d_w, d_x, opt, d_resvec, res, s->own);
-  if (rc == PCGB_OK) {
-    PCGB_CUDA(cudaEventRecord(s->ev_out, s->own));
-    PCGB_CUDA(cudaStreamWaitEvent(user, s->ev_out, 0));
-  }
-  return rc;
 }
 
 static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, const double *d_w, double *d_x,
@@ -1361,16 +1321,7 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
   c.state = ST_RUN; c.flag = 1; c.iter = 0; c.stag = 0; c.moresteps = 0; c.imin = 0; c.xcur = 0; c.xmin = 0;
   c.alias = 1;   // MP_XMin = MP_X (:379-380): the same array until the first improvement is recorded
   c.maxiter = opt->maxiter; c.maxstag = maxstag; c.fixed_iters = opt->fixed_iters ? 1 : 0;
-  *s->h_ctrl = c;
-  // (pinned source, stream-ordered: the next write to h_ctrl is the D2H copy of fetch_ctrl on the same stream)
-  PCGB_CUDA(cudaMemcpyAsync(s->d_ctrl, s->h_ctrl, sizeof(PcgCtrl), cudaMemcpyHostToDevice, st));
-  // head of iteration 0: rho = z.r (:446-469)
-  PCGB_TRY(rz_to_device(s, d_minv, d_w, st, mg));
-  k_ctrl_head<<<1, 1, 0, st>>>(s->d_ctrl, s->red + 6, 0);
-  PCGB_CHECK_LAUNCH();
-  s->launches += 1;
-  PCGB_TRY(trace_local(s, s->partials, vg, kMaxVecGrid, 2, 4, st, &s->launches));
-  PCGB_TRY(trace_step(s, TR_HEAD, s->h_red[1], s->h_red[0], st, &s->launches));
+  PCGB_TRY(enqueue_head(s, c, d_minv, d_w, mg, 0, s->h_red[1], s->h_red[0], st));
 
   int batch = opt->check_every > 0 ? opt->check_every : 16;
   if (batch > opt->maxiter) batch = opt->maxiter;
@@ -1383,15 +1334,14 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
   for (;;) {
     // ---- enqueue `batch` iterations
     if (want_graph && batch > 1) {
-      const int variant = (peer_path(s) ? 1 : 0) | ((s->A && spmv_split_available(s->A->P)) ? 2 : 0) | (s->fork_halo ? 4 : 0) |
-                          (s->O ? 8 : 0);
-      GraphKey key{d_minv, d_w, xw, d_resvec, batch, variant, s->trace, s->trace_cap, mg};
+      const bool peer = peer_path(s);
+      const GraphKey key{d_minv, d_w, d_resvec, batch, peer, split_product(s, peer), s->trace, s->trace_cap, mg};
       if (!s->gexec || !(s->gkey == key)) {
         if (s->gexec) { cudaGraphExecDestroy(s->gexec); s->gexec = nullptr; }
         cudaGraph_t graph = nullptr;
         PCGB_CUDA(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
         int rc = PCGB_OK, nl = 0;
-        for (int k = 0; k < batch && rc == PCGB_OK; ++k) rc = enqueue_iteration(s, d_minv, d_w, xw, d_resvec, st, &nl, nullptr, mg);
+        for (int k = 0; k < batch && rc == PCGB_OK; ++k) rc = enqueue_iteration(s, d_minv, d_w, d_resvec, st, &nl, nullptr, mg);
         cudaError_t ce = cudaStreamEndCapture(st, &graph);
         if (rc != PCGB_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
         PCGB_CUDA(ce);
@@ -1410,7 +1360,7 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
           while (s->ev_k.size() < (size_t)kEvPerIter * (ktimed + 1)) { cudaEvent_t e; PCGB_CUDA(cudaEventCreate(&e)); s->ev_k.push_back(e); }
           ev = &s->ev_k[(size_t)kEvPerIter * ktimed]; ++ktimed;
         }
-        PCGB_TRY(enqueue_iteration(s, d_minv, d_w, xw, d_resvec, st, &nl, ev, mg));
+        PCGB_TRY(enqueue_iteration(s, d_minv, d_w, d_resvec, st, &nl, ev, mg));
         s->launches += nl;
       }
     }
@@ -1446,14 +1396,7 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
       // continue with the replaced residual: head of the next iteration
       c.state = ST_RUN;
       PCGB_TRY(trace_host(s, TR_VERIFY, c, rr_act, true, nullptr, st));
-      *s->h_ctrl = c;
-      PCGB_CUDA(cudaMemcpyAsync(s->d_ctrl, s->h_ctrl, sizeof(PcgCtrl), cudaMemcpyHostToDevice, st));
-      PCGB_TRY(rz_to_device(s, d_minv, d_w, st, mg));
-      k_ctrl_head<<<1, 1, 0, st>>>(s->d_ctrl, s->red + 6, 1);
-      PCGB_CHECK_LAUNCH();
-      s->launches += 1;
-      PCGB_TRY(trace_local(s, s->partials, vg, kMaxVecGrid, 2, 4, st, &s->launches));
-      PCGB_TRY(trace_step(s, TR_RESUME, 0.0, 0.0, st, &s->launches));
+      PCGB_TRY(enqueue_head(s, c, d_minv, d_w, mg, 1, 0.0, 0.0, st));
       batch = 1;  // MoreSteps > 0: every further iteration is verified (:527)
       continue;
     }
@@ -1530,6 +1473,25 @@ static int solve_on(pcgb_solver_t s, const double *d_b, const double *d_minv, co
   return PCGB_OK;
 }
 
+// order the solver's own stream after the caller's stream, run, and order the caller's stream after us
+static int solve_fenced(pcgb_solver_t s, pcgb_mg_t mg, const double *d_b, const double *d_minv, const double *d_w, double *d_x,
+                        const pcgb_options *opt, double *d_resvec, pcgb_result *res, void *stream) {
+  cudaStream_t user = (cudaStream_t)stream;
+  PCGB_CUDA(cudaEventRecord(s->ev_in, user));
+  PCGB_CUDA(cudaStreamWaitEvent(s->own, s->ev_in, 0));
+  PCGB_TRY(solve_on(s, d_b, d_minv, d_w, d_x, opt, d_resvec, res, s->own, mg));
+  PCGB_CUDA(cudaEventRecord(s->ev_out, s->own));
+  PCGB_CUDA(cudaStreamWaitEvent(user, s->ev_out, 0));
+  return PCGB_OK;
+}
+
+int pcgb_solve(pcgb_solver_t s, const double *d_b, const double *d_minv, const double *d_w, double *d_x,
+               const pcgb_options *opt, double *d_resvec, pcgb_result *res, void *stream) {
+  if (!s || !d_b || !d_x || !opt || !res) return fail(PCGB_ERR_ARG, "pcgb_solve: null argument");
+  if (opt->maxiter <= 0) return fail(PCGB_ERR_ARG, "pcgb_solve: maxiter must be positive");
+  return solve_fenced(s, nullptr, d_b, d_minv, d_w, d_x, opt, d_resvec, res, stream);
+}
+
 // ------------------------------------------------------------------------------------ geometric multigrid (hex boxes)
 int pcgb_mg_destroy(pcgb_mg_t mg) {
   if (!mg) return PCGB_OK;
@@ -1539,7 +1501,7 @@ int pcgb_mg_destroy(pcgb_mg_t mg) {
   if (s && s->gexec && s->gkey.mg == mg) {
     cudaGraphExecDestroy(s->gexec);
     s->gexec = nullptr;
-    s->gkey = GraphKey{nullptr, nullptr, nullptr, nullptr, 0, 0, nullptr, 0, nullptr};
+    s->gkey = {};
   }
   for (size_t l = 0; l < mg->lv.size(); ++l) {
     MgLevel &L = mg->lv[l];
@@ -1833,15 +1795,7 @@ int pcgb_solve_mg(pcgb_solver_t s, pcgb_mg_t mg, const double *d_b, const double
   if (!s || !mg || !d_b || !d_x || !opt || !res) return fail(PCGB_ERR_ARG, "pcgb_solve_mg: null argument");
   if (mg->s != s) return fail(PCGB_ERR_ARG, "pcgb_solve_mg: the preconditioner was built for another solver");
   if (opt->maxiter <= 0) return fail(PCGB_ERR_ARG, "pcgb_solve_mg: maxiter must be positive");
-  cudaStream_t user = (cudaStream_t)stream;
-  PCGB_CUDA(cudaEventRecord(s->ev_in, user));
-  PCGB_CUDA(cudaStreamWaitEvent(s->own, s->ev_in, 0));
-  const int rc = solve_on(s, d_b, nullptr, d_w, d_x, opt, d_resvec, res, s->own, mg);
-  if (rc == PCGB_OK) {
-    PCGB_CUDA(cudaEventRecord(s->ev_out, s->own));
-    PCGB_CUDA(cudaStreamWaitEvent(user, s->ev_out, 0));
-  }
-  return rc;
+  return solve_fenced(s, mg, d_b, nullptr, d_w, d_x, opt, d_resvec, res, stream);
 }
 
 // ------------------------------------------------------------------------------------ hex generator
