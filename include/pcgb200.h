@@ -129,8 +129,15 @@ int pcgb_allreduce_sum(pcgb_comm_t c, double *d_buf, int count, void *stream);
  *   idx[k]             local row index (in the Eff numbering of A) of the k-th shared dof,
  *                      ordered by ascending GLOBAL node id then direction on both sides
  *                      (OvrlpLocalDofVecList, partition_mesh.py:822-827)
- * The unpack adds the received values in neighbour order j = 0..n_nbr-1, i.e. the same
- * summation order as the reference loop at pcg_solver.py:333-334 (deterministic).        */
+ * Lists are positional pairs: entry t of my list for rank s and entry t of s's list for me
+ * name the same dof, so both lists have the same length.  nbr_ptr[0] is 0, the neighbour
+ * ranks are distinct (not this rank, in 0..nranks-1), and the indices of one list are
+ * distinct and in 0..nlocal-1; anything else is PCGB_ERR_ARG before anything is allocated.
+ * An empty list is dropped (both sides drop it alike), so a rank whose lists are all empty
+ * has no neighbours and nobody waits for it.
+ * The exchange computes, for every shared dof, y[dof] first, then the neighbours' copies
+ * added in the caller's neighbour order j = 0..n_nbr-1 (one per list the dof is in), i.e.
+ * the summation order of the reference loop at pcg_solver.py:333-334 (deterministic).    */
 int pcgb_halo_create(pcgb_comm_t c, int n_nbr, const int32_t *nbr_rank, const int64_t *nbr_ptr,
                      const int64_t *idx_host, int64_t nlocal, pcgb_halo_t *out);
 int pcgb_halo_destroy(pcgb_halo_t h);

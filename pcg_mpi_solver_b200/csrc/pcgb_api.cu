@@ -460,55 +460,71 @@ int pcgb_halo_create(pcgb_comm_t c, int n_nbr, const int32_t *nbr_rank, const in
                      int64_t nlocal, pcgb_halo_t *out) {
   if (!out || n_nbr < 0 || (n_nbr > 0 && (!c || !nbr_rank || !nbr_ptr))) return fail(PCGB_ERR_ARG, "pcgb_halo_create: bad argument");
   PCGB_TRY(require_device());
-  pcgb_halo_t h = new pcgb_halo_s();
-  h->comm = c; h->n_nbr = n_nbr;
-  h->nbr_rank.assign(nbr_rank, nbr_rank + n_nbr);
-  if (n_nbr > 0) h->nbr_ptr.assign(nbr_ptr, nbr_ptr + n_nbr + 1);
-  else h->nbr_ptr.assign(1, 0);
-  h->m = h->nbr_ptr.back();
-  int rc = PCGB_OK;
-  cudaError_t ce = cudaSuccess;
-  if (h->m > INT32_MAX) rc = fail(PCGB_ERR_ARG, "pcgb_halo_create: too many shared dofs");
-  for (int j = 0; j < n_nbr && rc == PCGB_OK; ++j)
+  // The whole table is checked before anything is allocated.  Neighbours are distinct and so are the indices of one list
+  // (a repeated index would be added twice where the reference's y[list] += recv adds it once).
+  if (n_nbr > 0 && nbr_ptr[0] != 0) return fail(PCGB_ERR_ARG, "pcgb_halo_create: nbr_ptr[0] must be 0");
+  std::vector<char> listed(c ? (size_t)c->nranks : 0, 0);
+  std::vector<int> kept;   // slots with a non-empty list, in the caller's order
+  for (int j = 0; j < n_nbr; ++j) {
     if (nbr_rank[j] < 0 || nbr_rank[j] >= c->nranks || nbr_rank[j] == c->rank || nbr_ptr[j + 1] < nbr_ptr[j])
-      rc = fail(PCGB_ERR_ARG, "pcgb_halo_create: bad neighbour table at slot %d", j);
-  std::vector<int> idx((size_t)h->m), ent_nbr((size_t)h->m), nptr((size_t)n_nbr + 1);
-  if (rc == PCGB_OK && h->m > 0) {
-    for (int j = 0; j < n_nbr; ++j)
-      for (int64_t k = nbr_ptr[j]; k < nbr_ptr[j + 1]; ++k) ent_nbr[(size_t)k] = j;
-    for (int64_t k = 0; k < h->m && rc == PCGB_OK; ++k) {
-      if (idx_host[k] < 0 || idx_host[k] >= nlocal) rc = fail(PCGB_ERR_ARG, "pcgb_halo_create: index %lld out of range", (long long)idx_host[k]);
-      else idx[(size_t)k] = (int)idx_host[k];
-    }
+      return fail(PCGB_ERR_ARG, "pcgb_halo_create: bad neighbour table at slot %d", j);
+    if (listed[(size_t)nbr_rank[j]]) return fail(PCGB_ERR_ARG, "pcgb_halo_create: neighbour rank %d is listed twice", nbr_rank[j]);
+    listed[(size_t)nbr_rank[j]] = 1;
+    if (nbr_ptr[j + 1] > nbr_ptr[j]) kept.push_back(j);
   }
-  if (rc == PCGB_OK) {
-    for (int j = 0; j <= n_nbr; ++j) nptr[(size_t)j] = (int)h->nbr_ptr[(size_t)j];
-    // group the receive positions by dof, neighbour order inside a dof (stable: k ascending = neighbour ascending)
-    std::vector<int> order((size_t)h->m);
-    for (int64_t k = 0; k < h->m; ++k) order[(size_t)k] = (int)k;
-    std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return idx[a] < idx[b]; });
-    std::vector<int> dof, ptr, pos((size_t)h->m);
-    for (int64_t s = 0; s < h->m; ++s) {
-      const int k = order[(size_t)s];
-      if (s == 0 || idx[k] != idx[order[(size_t)s - 1]]) { dof.push_back(idx[k]); ptr.push_back((int)s); }
-      pos[(size_t)s] = k;
+  const int64_t m = n_nbr > 0 ? nbr_ptr[n_nbr] : 0;
+  if (m > INT32_MAX) return fail(PCGB_ERR_ARG, "pcgb_halo_create: too many shared dofs");
+  if (m > 0 && !idx_host) return fail(PCGB_ERR_ARG, "pcgb_halo_create: null index array");
+  std::vector<int> idx((size_t)m), ent_nbr((size_t)m), sorted;
+  for (int jj = 0; jj < (int)kept.size(); ++jj) {
+    const int j = kept[(size_t)jj];
+    for (int64_t k = nbr_ptr[j]; k < nbr_ptr[j + 1]; ++k) {
+      if (idx_host[k] < 0 || idx_host[k] >= nlocal) return fail(PCGB_ERR_ARG, "pcgb_halo_create: index %lld out of range", (long long)idx_host[k]);
+      idx[(size_t)k] = (int)idx_host[k];
+      ent_nbr[(size_t)k] = jj;
     }
-    ptr.push_back((int)h->m);
-    h->ndof = (int64_t)dof.size();
-    // receive block shared with the neighbours: [2][m] doubles + [n_nbr][2] flags (peer transport)
-    h->blk_bytes = (size_t)2 * (size_t)h->m * sizeof(double) + (size_t)2 * (size_t)std::max(n_nbr, 1) * sizeof(unsigned long long);
-    if ((ce = upload(&h->d_idx, idx)) == cudaSuccess && (ce = upload(&h->d_dof, dof)) == cudaSuccess &&
-        (ce = upload(&h->d_ptr, ptr)) == cudaSuccess && (ce = upload(&h->d_pos, pos)) == cudaSuccess &&
-        (ce = upload(&h->d_nbr_ptr, nptr)) == cudaSuccess && (ce = upload(&h->d_ent_nbr, ent_nbr)) == cudaSuccess &&
-        (ce = cudaMalloc(&h->d_send, std::max<size_t>((size_t)h->m, 1) * sizeof(double))) == cudaSuccess &&
-        (ce = cudaMalloc(&h->d_recv, std::max<size_t>((size_t)h->m, 1) * sizeof(double))) == cudaSuccess &&
-        (ce = cudaMalloc(&h->blk, h->blk_bytes)) == cudaSuccess && (ce = cudaMemset(h->blk, 0, h->blk_bytes)) == cudaSuccess &&
-        (ce = cudaMalloc(&h->d_epoch, 2 * sizeof(unsigned long long))) == cudaSuccess &&
-        (ce = cudaMemset(h->d_epoch, 0, 2 * sizeof(unsigned long long))) == cudaSuccess)
-      ce = cudaDeviceSynchronize();
-    if (ce != cudaSuccess) rc = fail(PCGB_ERR_CUDA, "pcgb_halo_create: %s", cudaGetErrorString(ce));
+    sorted.assign(idx.begin() + nbr_ptr[j], idx.begin() + nbr_ptr[j + 1]);
+    std::sort(sorted.begin(), sorted.end());
+    const auto dup = std::adjacent_find(sorted.begin(), sorted.end());
+    if (dup != sorted.end())
+      return fail(PCGB_ERR_ARG, "pcgb_halo_create: index %d appears twice in the list of neighbour rank %d", *dup, nbr_rank[j]);
   }
-  if (rc != PCGB_OK) { pcgb_halo_destroy(h); return rc; }
+  // An empty list is dropped.  Both sides of an interface list the same number of entries, so both drop it, and a rank
+  // whose lists are all empty has no neighbours: nobody waits for an exchange it never starts (m == 0 sends nothing).
+  pcgb_halo_t h = new pcgb_halo_s();
+  h->comm = c; h->n_nbr = (int)kept.size(); h->m = m;
+  h->nbr_ptr.assign(1, 0);
+  for (int j : kept) { h->nbr_rank.push_back(nbr_rank[j]); h->nbr_ptr.push_back(nbr_ptr[j + 1]); }
+  std::vector<int> nptr(h->nbr_ptr.begin(), h->nbr_ptr.end());
+  // group the receive positions by dof, neighbour order inside a dof (stable: k ascending = neighbour ascending)
+  std::vector<int> order((size_t)m);
+  for (int64_t k = 0; k < m; ++k) order[(size_t)k] = (int)k;
+  std::stable_sort(order.begin(), order.end(), [&](int a, int b) { return idx[a] < idx[b]; });
+  std::vector<int> dof, ptr, pos((size_t)m);
+  for (int64_t s = 0; s < m; ++s) {
+    const int k = order[(size_t)s];
+    if (s == 0 || idx[k] != idx[order[(size_t)s - 1]]) { dof.push_back(idx[k]); ptr.push_back((int)s); }
+    pos[(size_t)s] = k;
+  }
+  ptr.push_back((int)m);
+  h->ndof = (int64_t)dof.size();
+  // receive block shared with the neighbours: [2][m] doubles + [n_nbr][2] flags (peer transport)
+  h->blk_bytes = (size_t)2 * (size_t)m * sizeof(double) + (size_t)2 * (size_t)std::max(h->n_nbr, 1) * sizeof(unsigned long long);
+  cudaError_t ce = cudaSuccess;
+  if ((ce = upload(&h->d_idx, idx)) == cudaSuccess && (ce = upload(&h->d_dof, dof)) == cudaSuccess &&
+      (ce = upload(&h->d_ptr, ptr)) == cudaSuccess && (ce = upload(&h->d_pos, pos)) == cudaSuccess &&
+      (ce = upload(&h->d_nbr_ptr, nptr)) == cudaSuccess && (ce = upload(&h->d_ent_nbr, ent_nbr)) == cudaSuccess &&
+      (ce = cudaMalloc(&h->d_send, std::max<size_t>((size_t)m, 1) * sizeof(double))) == cudaSuccess &&
+      (ce = cudaMalloc(&h->d_recv, std::max<size_t>((size_t)m, 1) * sizeof(double))) == cudaSuccess &&
+      (ce = cudaMalloc(&h->blk, h->blk_bytes)) == cudaSuccess && (ce = cudaMemset(h->blk, 0, h->blk_bytes)) == cudaSuccess &&
+      (ce = cudaMalloc(&h->d_epoch, 2 * sizeof(unsigned long long))) == cudaSuccess &&
+      (ce = cudaMemset(h->d_epoch, 0, 2 * sizeof(unsigned long long))) == cudaSuccess)
+    ce = cudaDeviceSynchronize();
+  if (ce != cudaSuccess) {
+    const int rc = fail(PCGB_ERR_CUDA, "pcgb_halo_create: %s", cudaGetErrorString(ce));
+    pcgb_halo_destroy(h);
+    return rc;
+  }
   *out = h;
   return PCGB_OK;
 }

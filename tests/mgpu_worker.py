@@ -6,6 +6,7 @@ the gathered solution against the CPU oracle's multi-part emulation of the refer
 (oracle/ref_pcg.py ref_pcg over CsrPart boxes with the same interface lists).  Every rank records the loop trace; rank 0
 checks that the traces agree on every rank, that on the peer transport every reduced value is the rank-order sum of the
 ranks' local values bit for bit, and that the host restatement of the control logic (tests/pcg_shadow.py) replays it."""
+import hashlib
 import json
 import os
 import sys
@@ -95,7 +96,7 @@ def main():
         return concrete_main(out_path, sys.argv[3])
     block = int(sys.argv[2]) if len(sys.argv) > 2 else 6
     use_graph = bool(int(sys.argv[3])) if len(sys.argv) > 3 else True
-    operator = sys.argv[4] if len(sys.argv) > 4 else "csr"      # csr | ebe (matrix-free, fp64-atomic scatter)
+    operator = sys.argv[4] if len(sys.argv) > 4 else "csr"      # csr | ebe (matrix-free, fp64-atomic scatter) | ebe_ordered
     rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
     local = int(os.environ.get("LOCAL_RANK", rank))
     # PCGB_SHARED_GPU=1: all ranks drive cuda:0 (time-sliced) with a peer-only communicator - exercises the peer-memory
@@ -121,13 +122,13 @@ def main():
     for b_ in blocks:
         b_.h = 1.0 / ng[0]
     blk = blocks[rank]
-    A = generate_matrix(blk, device=dev) if operator == "csr" else generate_ebe(blk, device=dev)
+    A = generate_matrix(blk, device=dev) if operator == "csr" else generate_ebe(blk, device=dev, ordered=operator == "ebe_ordered")
     nbr, lists, w = interface_lists(blocks, rank)
     n_global = 3 * ng[0] * (ng[1] + 1) * (ng[2] + 1)
     op = SubdomainOperator(A, comm, nbr, lists, w, n_global=n_global)
     b = load_vector(blk, device=dev)
     minv = op.jacobi()
-    tol = 1e-12
+    tol = float(sys.argv[5]) if len(sys.argv) > 5 else 1e-12
     x, info = op.solve(b, minv, tol, 5000, use_graph=use_graph, check_every=8, trace=True)
     # operator probe: y = K v for a globally consistent v (function of the global dof id)
     gz, gy, gx = np.meshgrid(*[np.arange(blk.e0[a], blk.e0[a] + blk.ne[a] + 1) for a in (2, 1, 0)], indexing="ij")
@@ -140,13 +141,16 @@ def main():
     comm.allreduce_sum(wsum)
     # a second operator application AFTER the solve: the exchange epochs keep counting across graph replays and direct calls
     y2 = op.apply(torch.from_numpy(v).to(dev)).cpu().numpy()
-    if operator == "csr":
+    if operator != "ebe":
         assert np.array_equal(y, y2), "operator application is not reproducible"
     else:                                                         # atomics: reproducible to rounding only
         assert np.abs(y - y2).max() <= 1e-14 * np.abs(y).max(), "operator application is not reproducible"
     gathered = [None] * world
     dist.gather_object({"gdof": gdof, "x": x.cpu().numpy(), "y": y, "w": w, "info": (info.flag, info.iters, info.relres),
-                        "trace": info.trace, "trace_total": info.trace_total},
+                        "trace": info.trace, "trace_total": info.trace_total,
+                        "x_sha": hashlib.sha256(x.cpu().numpy().tobytes()).hexdigest(),
+                        "trace_sha": hashlib.sha256(info.trace.tobytes()).hexdigest(),
+                        "halo_m": op.halo_bytes() // 8, "halo_ndof": int(len(np.unique(np.concatenate(lists)))) if len(lists) else 0},
                        gathered if rank == 0 else None, dst=0)
     if rank == 0:
         from oracle import ref_pcg as R
@@ -172,12 +176,14 @@ def main():
             Y[g["gdof"]] = g["y"]
             Yref[g["gdof"]] = yrefs[r]
         res = {**trace_checks(gathered, comm.transport, tol, 5000, n_global),
-               "world": world, "flag": info.flag, "iters": info.iters, "relres": info.relres, "ref_flag": ref["Flag"],
+               "world": world, "tol": tol, "flag": info.flag, "iters": info.iters, "relres": info.relres, "ref_flag": ref["Flag"],
                "ref_iters": ref["Iter"], "ref_relres": ref["RelRes"],
                "x_rel_err": float(np.linalg.norm(U - Uref) / np.linalg.norm(Uref)),
                "y_rel_err": float(np.linalg.norm(Y - Yref) / np.linalg.norm(Yref)),
                "copy_mismatch": consistent / float(np.abs(U).max()), "weight_sum": float(wsum.item()), "n_global": n_global,
                "halo_bytes": op.halo_bytes(), "all_infos": [g["info"] for g in gathered], "transport": comm.transport,
+               "x_sha": [g["x_sha"] for g in gathered], "trace_sha": [g["trace_sha"] for g in gathered],
+               "halo_m": [g["halo_m"] for g in gathered], "halo_ndof": [g["halo_ndof"] for g in gathered],
                "plan": A.plan_info() if operator == "csr" else "ebe", "launches": info.launches, "loop_ms": info.loop_ms}
         with open(out_path, "w") as f:
             json.dump(res, f)
