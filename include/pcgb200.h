@@ -296,7 +296,7 @@ int pcgb_hex_fill(const pcgb_hex_box *box, const double *ke_host, double ck, con
                   int32_t *d_col, double *d_val, void *stream);
 
 /* ---------------------------------------------------------------- opt-in: geometric multigrid preconditioner (hex boxes)
- * z = M r is one symmetric V-cycle over nested hex boxes, for a one-rank solver whose operator (CSR, EBE or ordered EBE) is
+ * z = M r is one symmetric V-cycle over nested hex boxes (across ranks: pcgb_mg_create_ranks below), for a one-rank solver whose operator (CSR, EBE or ordered EBE) is
  * the stiffness matrix of `box` in the pcgb_hex_* numbering.  Level l+1 halves every ne of level l while all ne are even and
  * the halves stay >= 2; its matrix is generated on the device at spacing 2^l h (Ck = E 2^l h), which for nested Q1 spaces
  * equals the Galerkin product P^T A P.  P is trilinear interpolation of the free nodes, direction by direction (weights 1,
@@ -333,6 +333,32 @@ int pcgb_mg_coarse_solve(pcgb_mg_t mg, const double *d_r, double *d_z, void *str
  * time_kernels, phase_ms[5] ("fused update") includes the V-cycle that follows the update.                        */
 int pcgb_solve_mg(pcgb_solver_t s, pcgb_mg_t mg, const double *d_b, const double *d_w, double *d_x, const pcgb_options *opt,
                   double *d_resvec, pcgb_result *res, void *stream);
+/* The same preconditioner across ranks, for a solver with a communicator of 2 or more ranks whose boxes tile the global mesh
+ * (the domain decomposition of pcg_solver.py, whose Jacobi z = Minv .* r it replaces).  Collective: every rank calls it with
+ * the same n_ranked.  Levels 0 .. la (la = n_ranked) are ranked: level l holds the rank's box halved l times (ng, e0, ne
+ * all halved; each halving needs ne even and >= 4 and e0, ng even), its sub-assembled matrix at spacing 2^l h, halo plan
+ * level_halos[l-1] (level 0: the solver's) and 0/1 ownership weights d_own[l] (n_l doubles, copied; the owner of a shared
+ * dof is the lowest rank).  Every product and restriction on a ranked level is followed by its exchange-add, so vectors
+ * stay consistent; restriction sums the owned fine nodes only; lambda comes from all-reduced, owner-weighted Lanczos sums
+ * from the start vector at the GLOBAL free index g (so the one-rank lambda of the global mesh, to rounding).  Level la is
+ * not smoothed: its owned entries are gathered into the global box of level la (k_mg_gather, then `gather`, a plan that
+ * lists all of that box's dofs for every other rank: one non-zero term per entry, so every rank holds the same vector
+ * bit for bit), which continues on every rank as the one-rank hierarchy above (whole boxes, dense Cholesky at the
+ * bottom); its result is copied back out to level la.  The global boxes are those of pcgb_mg_create on the global mesh.
+ * PCGB_ERR_ARG before anything is allocated: no multi-rank communicator, a box outside the mesh, an operator whose size
+ * is not the box's, n_ranked < 1, a level that cannot be halved, a halo of the wrong size or communicator, a gather
+ * plan that is not all-to-all over the gathered box, a gathered box above 2^17 dofs, a coarsest level above 1536 dofs,
+ * the scalar arguments of pcgb_mg_create.  The halo plans must outlive the handle.  pcgb_mg_restrict on a ranked level
+ * includes the coarse exchange-add; restrict / prolong_add / smooth refuse level la (use gather / scatter).        */
+int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos, pcgb_halo_t gather,
+                         const double *const *d_own, const double *ke_host, double E, double h, const double *d_minv_fine,
+                         int degree, double lo, pcgb_mg_t *out);
+/* la (-1 for a one-rank handle) and the dofs of its gathered global box; pcgb_mg_info lists levels 0 .. la, then the
+ * replicated levels (lambda 0 for level la and the coarsest) */
+int pcgb_mg_info_ranks(pcgb_mg_t mg, int32_t *gather_level, int64_t *n_gathered);
+/* level la's ranked vector into its global box on every rank (gather + exchange), and the rank's entries back out */
+int pcgb_mg_gather(pcgb_mg_t mg, const double *d_ranked, double *d_global, void *stream);
+int pcgb_mg_scatter(pcgb_mg_t mg, const double *d_global, double *d_ranked, void *stream);
 
 #ifdef __cplusplus
 }

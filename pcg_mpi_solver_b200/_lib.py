@@ -111,6 +111,11 @@ SIGNATURES = {
     "pcgb_mg_prolong_add": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "pcgb_mg_smooth": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "pcgb_mg_coarse_solve": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcgb_mg_create_ranks": (c_int, [c_void_p, POINTER(HexBox), c_int, POINTER(c_void_p), c_void_p, POINTER(c_void_p), POINTER(c_double),
+                                     c_double, c_double, c_void_p, c_int, c_double, POINTER(c_void_p)]),
+    "pcgb_mg_info_ranks": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int64)]),
+    "pcgb_mg_gather": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcgb_mg_scatter": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcgb_solve_mg": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, POINTER(Options), c_void_p, POINTER(Result), c_void_p]),
     "pcgb_hex_nrows": (c_int64, [POINTER(HexBox)]),
     "pcgb_hex_count": (c_int, [POINTER(HexBox), c_void_p, c_void_p]),

@@ -117,6 +117,7 @@ struct pcgb_halo_s {
   std::vector<int64_t> nbr_ptr;
   int64_t m = 0;          // total shared entries (with multiplicity over neighbours)
   int64_t ndof = 0;       // distinct interface dofs
+  int64_t nlocal = 0;     // length of the vectors it exchanges
   int *d_idx = nullptr;   // [m]   gather index for the pack
   int *d_dof = nullptr;   // [ndof] distinct dofs
   int *d_ptr = nullptr;   // [ndof+1]

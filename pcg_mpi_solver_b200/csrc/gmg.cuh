@@ -25,10 +25,24 @@ __device__ __forceinline__ int64_t mg_index(const HexGeom &g, int lx, int ly, in
   return ((int64_t)lz * (g.ny + 1) + ly) * g.nxf + (lx - g.x_lo);
 }
 
+// A rank's box of a level inside the level's global box: local node (lx, ly, lz) is global node (e0 + l).  One rank:
+// e0 = 0 and glob = the box itself, so the global free index of a dof is its local index.
+struct MgPlace {
+  HexGeom glob;
+  int e0x, e0y, e0z;
+};
+__device__ __forceinline__ int64_t mg_global_node(const MgPlace &p, int lx, int ly, int lz) {
+  return mg_index(p.glob, lx + p.e0x, ly + p.e0y, lz + p.e0z);
+}
+
 // r_c = P^T r_f: one thread per coarse free node; the <= 27 fine nodes 2*c + (dx, dy, dz), d in {-1, 0, 1}, are summed
-// in (dz, dy, dx) ascending order from 0.0, each with weight prod_a (d_a == 0 ? 1 : 1/2).
+// in (dz, dy, dx) ascending order from 0.0, each with weight prod_a (d_a == 0 ? 1 : 1/2).  Local indices serve a rank's
+// box as well, because its fine e0 is twice its coarse e0.  own_f (NULL = every node): 0/1 ownership of the fine dofs;
+// only owned fine nodes are summed (selected, not multiplied), so after the coarse level's exchange-add every fine node
+// of the global box has been counted exactly once.
 __global__ void __launch_bounds__(256)
-k_mg_restrict(HexGeom gf, HexGeom gc, const double *__restrict__ rf, double *__restrict__ rc, const int *__restrict__ skip) {
+k_mg_restrict(HexGeom gf, HexGeom gc, const double *__restrict__ rf, const double *__restrict__ own_f, double *__restrict__ rc,
+              const int *__restrict__ skip) {
   if (skip != nullptr && *skip != 0) return;
   const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   if (t >= gc.nfree_nodes) return;
@@ -44,8 +58,10 @@ k_mg_restrict(HexGeom gf, HexGeom gc, const double *__restrict__ rf, double *__r
       for (int dx = -1; dx <= 1; ++dx) {
         const int fx = 2 * cx + dx;
         if (fx < gf.x_lo || fx > gf.nx) continue;
+        const int64_t fi = mg_index(gf, fx, fy, fz);
+        if (own_f != nullptr && own_f[3 * fi] == 0.0) continue;
         const double w = (dx ? 0.5 : 1.0) * (dy ? 0.5 : 1.0) * (dz ? 0.5 : 1.0);
-        const double *src = rf + 3 * mg_index(gf, fx, fy, fz);
+        const double *src = rf + 3 * fi;
         s0 += w * src[0]; s1 += w * src[1]; s2 += w * src[2];
       }
     }
@@ -113,18 +129,23 @@ k_mg_cheb_step(int64_t n, const double *__restrict__ q, const double *__restrict
   }
 }
 
-// Fixed start vector of the Lanczos estimate: v_i = 1/2 + ((37 i + 11) mod 101) / 101.
-__global__ void k_mg_lanczos_start(int64_t n, double *__restrict__ v) {
+// Fixed start vector of the Lanczos estimate: v_i = 1/2 + ((37 g + 11) mod 101) / 101 with g the dof's free index in the
+// level's global box (g = i on one rank), so every rank's copy of a shared dof starts alike.
+__global__ void k_mg_lanczos_start(HexGeom g, MgPlace p, double *__restrict__ v) {
   const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride)
-    v[i] = 0.5 + (double)((37 * i + 11) % 101) / 101.0;
+  for (int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; t < g.nfree_nodes; t += stride) {
+    int lx, ly, lz;
+    mg_node(g, t, lx, ly, lz);
+    const int64_t gn = mg_global_node(p, lx, ly, lz);
+    for (int d = 0; d < 3; ++d) v[3 * t + d] = 0.5 + (double)((37 * (3 * gn + d) + 11) % 101) / 101.0;
+  }
 }
 
 // Lanczos on D^-1 A in the D inner product (v.D v = sum v^2 / dinv): w = (scale ? dinv * y : y) - alpha v - beta vp into
-// w (which may be vp), and partials of w.D w.  v and vp may be NULL (start vector).
+// w (which may be vp), and partials of w.D w over the owned dofs (own NULL = all).  v and vp may be NULL (start vector).
 __global__ void __launch_bounds__(256)
 k_mg_lanczos_w(int64_t n, const double *__restrict__ y, const double *__restrict__ v, const double *vp, const double *__restrict__ dinv,
-               double alpha, double beta, int scale, double *w, double *__restrict__ partials) {
+               const double *__restrict__ own, double alpha, double beta, int scale, double *w, double *__restrict__ partials) {
   __shared__ double red[32];
   double s = 0.0;
   const int64_t stride = (int64_t)gridDim.x * 256;
@@ -132,7 +153,7 @@ k_mg_lanczos_w(int64_t n, const double *__restrict__ y, const double *__restrict
     double wi = scale ? dinv[i] * y[i] : y[i];
     if (v) wi = wi - alpha * v[i] - beta * vp[i];
     w[i] = wi;
-    s = fma(wi, wi / dinv[i], s);
+    if (own == nullptr || own[i] != 0.0) s = fma(wi, wi / dinv[i], s);
   }
   double vv[1] = {s};
   block_sum<1, 256>(vv, red);
@@ -147,6 +168,35 @@ __global__ void k_mg_lanczos_next(int64_t n, double inv_beta, double *__restrict
     vp[i] = v[i];
     v[i] = wi * inv_beta;
   }
+}
+
+// Gather of the last ranked level into its global box: one thread per global free node; the entry is this rank's copy
+// when the rank owns it (selected on ownership, so a non-owned copy, NaN or not, never enters) and 0.0 otherwise.  The
+// exchange-add over the all-to-all gather plan then completes the vector: one non-zero term per entry, exact in any order.
+__global__ void __launch_bounds__(256)
+k_mg_gather(HexGeom g, MgPlace p, const double *__restrict__ v, const double *__restrict__ own, double *__restrict__ out,
+            const int *__restrict__ skip) {
+  if (skip != nullptr && *skip != 0) return;
+  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (t >= p.glob.nfree_nodes) return;
+  int gx, gy, gz;
+  mg_node(p.glob, t, gx, gy, gz);
+  const int lx = gx - p.e0x, ly = gy - p.e0y, lz = gz - p.e0z;
+  const bool in = lx >= g.x_lo && lx <= g.nx && ly >= 0 && ly <= g.ny && lz >= 0 && lz <= g.nz;
+  const int64_t li = in ? mg_index(g, lx, ly, lz) : 0;
+  for (int d = 0; d < 3; ++d) out[3 * t + d] = in && own[3 * li + d] != 0.0 ? v[3 * li + d] : 0.0;
+}
+
+// Scatter back: every local dof (owned or not) takes the global vector's entry, so the ranked vector is consistent.
+__global__ void __launch_bounds__(256)
+k_mg_scatter(HexGeom g, MgPlace p, const double *__restrict__ in, double *__restrict__ v, const int *__restrict__ skip) {
+  if (skip != nullptr && *skip != 0) return;
+  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (t >= g.nfree_nodes) return;
+  int lx, ly, lz;
+  mg_node(g, t, lx, ly, lz);
+  const int64_t gi = mg_global_node(p, lx, ly, lz);
+  for (int d = 0; d < 3; ++d) v[3 * t + d] = in[3 * gi + d];
 }
 
 // rz and the count of non-finite z entries of z = M r: (sum z*(r*w), #(!isfinite z)) into partials[0] / partials[kMaxVecGrid]

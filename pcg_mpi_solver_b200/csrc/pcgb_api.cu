@@ -492,7 +492,7 @@ int pcgb_halo_create(pcgb_comm_t c, int n_nbr, const int32_t *nbr_rank, const in
   // An empty list is dropped.  Both sides of an interface list the same number of entries, so both drop it, and a rank
   // whose lists are all empty has no neighbours: nobody waits for an exchange it never starts (m == 0 sends nothing).
   pcgb_halo_t h = new pcgb_halo_s();
-  h->comm = c; h->n_nbr = (int)kept.size(); h->m = m;
+  h->comm = c; h->n_nbr = (int)kept.size(); h->m = m; h->nlocal = nlocal;
   h->nbr_ptr.assign(1, 0);
   for (int j : kept) { h->nbr_rank.push_back(nbr_rank[j]); h->nbr_ptr.push_back(nbr_ptr[j + 1]); }
   std::vector<int> nptr(h->nbr_ptr.begin(), h->nbr_ptr.end());
@@ -982,8 +982,16 @@ int trace_host(pcgb_solver_t s, int kind, const PcgCtrl &c, double rr, bool has_
 }  // namespace
 
 // ---- geometric multigrid preconditioner (pcgb_mg_*): one symmetric V-cycle z = M r
+// Across ranks (pcgb_mg_create_ranks) levels 0 .. la are ranked: each rank holds its own box, vectors are consistent (every
+// copy of a shared dof holds the full value) and every operator application and restriction is followed by the level's
+// exchange-add.  Level la is not smoothed: its vector is gathered into the global box, which levels la+1 .. hold as a
+// replicated one-rank hierarchy on every rank.  One rank: la = -1 and every level is a whole box.
 struct MgLevel {
   HexGeom g{};
+  MgPlace place{};             // the box inside the level's global box (one rank: the box itself at e0 = 0)
+  int glev = 0;                // level of the global hierarchy (spacing 2^glev h)
+  pcgb_halo_t halo = nullptr;  // ranked levels: exchange-add of the level (level 0: the solver's halo; not owned)
+  double *own = nullptr;       // ranked levels: 0/1 ownership of the dofs (copy)
   int64_t n = 0;
   void *rowptr = nullptr;   // coarse levels above the coarsest: device-generated CSR (int32 offsets below 2^31 non-zeros)
   int *col = nullptr;
@@ -1002,6 +1010,8 @@ struct pcgb_mg_s {
   std::vector<MgLevel> lv;
   int degree = 2;
   double lo = 0.25;
+  int la = -1;                     // gathered ranked level (-1: one rank)
+  pcgb_halo_t gather = nullptr;    // all-to-all plan over the global box of level la (not owned)
   int nc = 0;
   double *chol = nullptr;   // coarsest level: dense Cholesky factor, L in the lower triangle mirrored into the upper
   double *z = nullptr;      // z = M r of the PCG loop
@@ -1014,9 +1024,13 @@ namespace {
 
 constexpr int kMgLanczosSteps = 20;
 
+// y = A x on level l, then the level's exchange-add on a ranked level.  The exchange runs whatever the loop state, like
+// the fine halo of the iteration: every rank enqueues the same exchanges and all ranks stop at the same iteration.
 int mg_op(pcgb_mg_t mg, int l, const double *x, double *y, cudaStream_t st, int *nl, const int *skip) {
-  if (l > 0) return spmv_launch(mg->lv[(size_t)l].P, x, y, false, st, nl, skip);
-  return mg->s->op.apply(x, y, st, nl, skip);
+  const MgLevel &L = mg->lv[(size_t)l];
+  if (l > 0) PCGB_TRY(spmv_launch(L.P, x, y, false, st, nl, skip));
+  else PCGB_TRY(mg->s->op.apply(x, y, st, nl, skip));
+  return L.halo ? halo_exchange_add(L.halo, y, st, nl) : PCGB_OK;
 }
 
 // Chebyshev smoothing of D^-1 A on level l: zero_start: x = S b (no operator application for x = 0); otherwise
@@ -1049,19 +1063,52 @@ int mg_coarse_solve(pcgb_mg_t mg, const double *r, double *z, cudaStream_t st, i
   return PCGB_OK;
 }
 
-// z = M r: pre-smooth and restrict down to the coarsest level, solve there, prolong and post-smooth back up
+// r_c = P^T r_f from level l to l+1; on a ranked level each rank sums its owned fine nodes and the coarse level's
+// exchange-add completes the sum
+int mg_restrict(pcgb_mg_t mg, int l, const double *rf, double *rc, cudaStream_t st, int *nl, const int *skip) {
+  const MgLevel &A = mg->lv[(size_t)l], &C = mg->lv[(size_t)l + 1];
+  k_mg_restrict<<<mg_node_grid(C.g), 256, 0, st>>>(A.g, C.g, rf, A.own, rc, skip);
+  PCGB_CHECK_LAUNCH();
+  *nl += 1;
+  return C.halo ? halo_exchange_add(C.halo, rc, st, nl) : PCGB_OK;
+}
+
+// level la's ranked vector -> the global box of level la (replicated on every rank), and back
+int mg_gather(pcgb_mg_t mg, const double *v, double *out, cudaStream_t st, int *nl, const int *skip) {
+  const MgLevel &A = mg->lv[(size_t)mg->la];
+  k_mg_gather<<<(unsigned)((A.place.glob.nfree_nodes + 255) / 256), 256, 0, st>>>(A.g, A.place, v, A.own, out, skip);
+  PCGB_CHECK_LAUNCH();
+  *nl += 1;
+  return halo_exchange_add(mg->gather, out, st, nl);
+}
+int mg_scatter(pcgb_mg_t mg, const double *in, double *v, cudaStream_t st, int *nl, const int *skip) {
+  const MgLevel &A = mg->lv[(size_t)mg->la];
+  k_mg_scatter<<<mg_node_grid(A.g), 256, 0, st>>>(A.g, A.place, in, v, skip);
+  PCGB_CHECK_LAUNCH();
+  *nl += 1;
+  return PCGB_OK;
+}
+
+// z = M r: pre-smooth and restrict down to the coarsest level, solve there, prolong and post-smooth back up.  Across ranks
+// the gathered level la is not smoothed: its vector goes into the replicated hierarchy below it and comes back out.
 int mg_vcycle(pcgb_mg_t mg, const double *rin, double *zout, cudaStream_t st, int *nl, const int *skip) {
   const int L = (int)mg->lv.size();
   for (int l = 0; l + 1 < L; ++l) {
     MgLevel &A = mg->lv[(size_t)l], &C = mg->lv[(size_t)l + 1];
+    if (l == mg->la) {
+      PCGB_TRY(mg_gather(mg, A.b, C.b, st, nl, skip));
+      continue;
+    }
     PCGB_TRY(mg_smooth(mg, l, l ? A.b : rin, l ? A.x : zout, true, true, st, nl, skip));
-    k_mg_restrict<<<mg_node_grid(C.g), 256, 0, st>>>(A.g, C.g, A.r, C.b, skip);
-    PCGB_CHECK_LAUNCH();
-    *nl += 1;
+    PCGB_TRY(mg_restrict(mg, l, A.r, C.b, st, nl, skip));
   }
   PCGB_TRY(mg_coarse_solve(mg, mg->lv.back().b, mg->lv.back().x, st, nl, skip));
   for (int l = L - 2; l >= 0; --l) {
     MgLevel &A = mg->lv[(size_t)l], &C = mg->lv[(size_t)l + 1];
+    if (l == mg->la) {
+      PCGB_TRY(mg_scatter(mg, C.x, A.x, st, nl, skip));
+      continue;
+    }
     double *x = l ? A.x : zout;
     k_mg_prolong_add<<<mg_node_grid(A.g), 256, 0, st>>>(A.g, C.g, C.x, x, skip);
     PCGB_CHECK_LAUNCH();
@@ -1522,7 +1569,7 @@ int pcgb_mg_destroy(pcgb_mg_t mg) {
   for (size_t l = 0; l < mg->lv.size(); ++l) {
     MgLevel &L = mg->lv[l];
     if (L.has_plan) free_plan(L.P);
-    cudaFree(L.rowptr); cudaFree(L.col); cudaFree(L.val); cudaFree(L.dinv);
+    cudaFree(L.rowptr); cudaFree(L.col); cudaFree(L.val); cudaFree(L.dinv); cudaFree(L.own);
     if (l > 0) { cudaFree(L.b); cudaFree(L.x); }
     cudaFree(L.r); cudaFree(L.d); cudaFree(L.q);
   }
@@ -1579,21 +1626,25 @@ double tridiag_max_eig(const std::vector<double> &a, const std::vector<double> &
 }
 
 // largest eigenvalue of D^-1 A on level l: kMgLanczosSteps Lanczos steps (D inner product) from a fixed start vector, the
-// largest eigenvalue of their tridiagonal matrix.  Then the Chebyshev coefficients of the level.
+// largest eigenvalue of their tridiagonal matrix.  Then the Chebyshev coefficients of the level.  On a ranked level the
+// vectors stay consistent (mg_op exchanges), the inner products sum the owned dofs and are all-reduced (one value per
+// step), and the start vector is indexed by the global free dof, so lambda is the same number on every rank.
 int mg_estimate(pcgb_mg_t mg, int l) {
   MgLevel &L = mg->lv[(size_t)l];
   const int grid = vec_grid(L.n);
+  const bool ranked = l <= mg->la;
   int nl = 0;
   auto fetch = [&](double *out) -> int {
     k_reduce<1, 0><<<1, 256>>>(nullptr, mg->partials, grid, kMaxVecGrid, mg->red, nullptr);
     PCGB_CHECK_LAUNCH();
+    if (ranked) PCGB_TRY(allreduce_sum(mg->s->comm, mg->red, 1, 0));
     PCGB_CUDA(cudaMemcpy(mg->h_red, mg->red, sizeof(double), cudaMemcpyDeviceToHost));
     *out = mg->h_red[0];
     return PCGB_OK;
   };
   PCGB_CUDA(cudaMemset(L.d, 0, (size_t)L.n * sizeof(double)));
-  k_mg_lanczos_start<<<grid, 256>>>(L.n, L.q);
-  k_mg_lanczos_w<<<grid, 256>>>(L.n, L.q, nullptr, nullptr, L.dinv, 0.0, 0.0, 0, L.r, mg->partials);
+  k_mg_lanczos_start<<<grid, 256>>>(L.g, L.place, L.q);
+  k_mg_lanczos_w<<<grid, 256>>>(L.n, L.q, nullptr, nullptr, L.dinv, L.own, 0.0, 0.0, 0, L.r, mg->partials);
   PCGB_CHECK_LAUNCH();
   double bb = 0.0;
   PCGB_TRY(fetch(&bb));
@@ -1604,13 +1655,13 @@ int mg_estimate(pcgb_mg_t mg, int l) {
   beta = 0.0;
   for (int it = 0; it < kMgLanczosSteps; ++it) {
     PCGB_TRY(mg_op(mg, l, L.d, L.q, 0, &nl, nullptr));
-    k_dot_w<<<grid, kVecBlock>>>(L.n, L.d, L.q, nullptr, mg->partials);
+    k_dot_w<<<grid, kVecBlock>>>(L.n, L.d, L.q, L.own, mg->partials);
     PCGB_CHECK_LAUNCH();
     double alpha = 0.0;
     PCGB_TRY(fetch(&alpha));
     al.push_back(alpha);
     if (it + 1 == kMgLanczosSteps) break;
-    k_mg_lanczos_w<<<grid, 256>>>(L.n, L.q, L.d, L.r, L.dinv, alpha, beta, 1, L.r, mg->partials);
+    k_mg_lanczos_w<<<grid, 256>>>(L.n, L.q, L.d, L.r, L.dinv, L.own, alpha, beta, 1, L.r, mg->partials);
     PCGB_CHECK_LAUNCH();
     PCGB_TRY(fetch(&bb));
     beta = std::sqrt(bb);
@@ -1637,14 +1688,29 @@ int mg_estimate(pcgb_mg_t mg, int l) {
   return PCGB_OK;
 }
 
-int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const double *d_minv_fine,
-             const std::vector<HexGeom> &geo) {
-  const int nlev = (int)geo.size();
+// whole boxes below geo.back(): halve every ne while all are even and the halves stay >= 2
+void mg_whole_box_levels(std::vector<HexGeom> &geo) {
+  for (;;) {
+    const HexGeom g = geo.back();
+    if (g.nx % 2 || g.ny % 2 || g.nz % 2 || g.nx < 4 || g.ny < 4 || g.nz < 4) break;
+    pcgb_hex_box cb{};
+    const int ne[3] = {g.nx / 2, g.ny / 2, g.nz / 2};
+    for (int a = 0; a < 3; ++a) { cb.ne[a] = ne[a]; cb.ng[a] = ne[a]; cb.e0[a] = 0; }
+    geo.push_back(hex_geom(&cb));
+  }
+}
+
+// largest global box a multi-rank hierarchy gathers onto every rank
+constexpr int64_t kMgMaxGathered = 1 << 17;
+
+// Builds the levels whose geometry (g, place, glev) and halos the caller has set in mg->lv.  own: ownership weights of
+// the ranked levels 0 .. la (copied).
+int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const double *d_minv_fine, const double *const *own) {
+  const int nlev = (int)mg->lv.size();
   auto alloc = [&](double **p, int64_t n) -> cudaError_t {
     mg->bytes += 8 * n;
     return cudaMalloc(p, (size_t)std::max<int64_t>(n, 1) * sizeof(double));
   };
-  mg->lv.resize((size_t)nlev);
   // set-up runs on the legacy stream, which does not wait for non-blocking streams: finish whatever work of the caller may
   // still be writing d_minv_fine (or the operator's arrays) before the first read
   PCGB_CUDA(cudaDeviceSynchronize());
@@ -1655,9 +1721,8 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
   PCGB_CUDA(cudaMemset(mg->d_bad, 0, sizeof(int)));
   for (int l = 0; l < nlev; ++l) {
     MgLevel &L = mg->lv[(size_t)l];
-    L.g = geo[(size_t)l];
     L.n = 3 * L.g.nfree_nodes;
-    const double ck = E * h * (double)(1ll << l);
+    const double ck = E * h * (double)(1ll << L.glev);
     if (l == 0) {
       PCGB_CUDA(alloc(&mg->z, L.n));
       PCGB_CUDA(alloc(&L.dinv, L.n));
@@ -1665,6 +1730,11 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
     } else {
       PCGB_CUDA(alloc(&L.b, L.n));
       PCGB_CUDA(alloc(&L.x, L.n));
+    }
+    if (l <= mg->la) {
+      PCGB_CUDA(alloc(&L.own, L.n));
+      PCGB_CUDA(cudaMemcpy(L.own, own[l], (size_t)L.n * sizeof(double), cudaMemcpyDeviceToDevice));
+      if (l == mg->la) continue;   // gathered: no operator, no smoother
     }
     if (l == nlev - 1) {   // coarsest: dense Cholesky factor of its matrix
       int64_t *rp = nullptr, nnz = 0;
@@ -1711,6 +1781,7 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
       PCGB_TRY(L.P.rp64 ? build_plan_t<int64_t>(L.P, 0) : build_plan_t<int32_t>(L.P, 0));
       PCGB_CUDA(alloc(&L.dinv, L.n));
       PCGB_TRY(csr_diag_compute(L.P, L.r, 0));
+      if (L.halo) PCGB_TRY(halo_exchange_add(L.halo, L.r, 0));   // assembled diagonal of a ranked level
       k_reciprocal<<<vec_grid(L.n), 256>>>(L.n, L.r, L.dinv);
       PCGB_CHECK_LAUNCH();
     }
@@ -1734,21 +1805,90 @@ int pcgb_mg_create(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_ho
   std::vector<HexGeom> geo{hex_geom(box)};
   if (3 * geo[0].nfree_nodes != s->n) return fail(PCGB_ERR_ARG, "pcgb_mg_create: the solver's operator has %lld rows, the box %lld",
                                                   (long long)s->n, (long long)(3 * geo[0].nfree_nodes));
-  for (;;) {
-    HexGeom g = geo.back();
-    if (g.nx % 2 || g.ny % 2 || g.nz % 2 || g.nx < 4 || g.ny < 4 || g.nz < 4) break;
-    pcgb_hex_box cb = *box;
-    const int ne[3] = {g.nx, g.ny, g.nz};
-    for (int a = 0; a < 3; ++a) { cb.ne[a] = ne[a] / 2; cb.ng[a] = cb.ne[a]; }
-    geo.push_back(hex_geom(&cb));
-  }
+  mg_whole_box_levels(geo);
   if (geo.size() < 2) return fail(PCGB_ERR_ARG, "pcgb_mg_create: the box does not coarsen (every ne must be even and >= 4)");
   if (3 * geo.back().nfree_nodes > kMgMaxCoarse)
     return fail(PCGB_ERR_ARG, "pcgb_mg_create: the coarsest level has %lld dofs (at most %d)", (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
   if (geo.size() > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "pcgb_mg_create: more than %d levels", PCGB_MG_MAX_LEVELS);
   pcgb_mg_t mg = new pcgb_mg_s();
   mg->s = s; mg->degree = degree; mg->lo = lo;
-  const int rc = mg_build(mg, ke_host, E, h, d_minv_fine, geo);
+  mg->lv.resize(geo.size());
+  for (size_t l = 0; l < geo.size(); ++l) {
+    MgLevel &L = mg->lv[l];
+    L.g = geo[l]; L.glev = (int)l; L.place = MgPlace{geo[l], 0, 0, 0};
+  }
+  const int rc = mg_build(mg, ke_host, E, h, d_minv_fine, nullptr);
+  if (rc != PCGB_OK) { pcgb_mg_destroy(mg); return rc; }
+  *out = mg;
+  return PCGB_OK;
+}
+
+int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos, pcgb_halo_t gather,
+                         const double *const *d_own, const double *ke_host, double E, double h, const double *d_minv_fine,
+                         int degree, double lo, pcgb_mg_t *out) {
+  PCGB_TRY(require_device());
+  if (!s || !box || !level_halos || !gather || !d_own || !ke_host || !d_minv_fine || !out)
+    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: null argument");
+  if (!s->comm || s->comm->nranks < 2) return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the solver has no communicator of 2 or more ranks");
+  if (degree < 1 || !(lo > 0.0 && lo < 1.1) || !(E > 0.0) || !(h > 0.0))
+    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: degree >= 1, 0 < lo < 1.1, E > 0 and h > 0 required");
+  for (int a = 0; a < 3; ++a)
+    if (box->ne[a] <= 0 || box->e0[a] < 0 || box->e0[a] + box->ne[a] > box->ng[a])
+      return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the box does not lie in the mesh");
+  if (3 * hex_geom(box).nfree_nodes != s->n)
+    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the solver's operator has %lld rows, the box %lld", (long long)s->n,
+                (long long)(3 * hex_geom(box).nfree_nodes));
+  if (n_ranked < 1) return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the fine level does not coarsen (n_ranked >= 1 required)");
+  // ranked levels 0 .. la: the rank's box halved la times, and the global box around it
+  const int la = n_ranked;
+  std::vector<pcgb_hex_box> rb{*box};
+  for (int l = 1; l <= la; ++l) {
+    const pcgb_hex_box &p = rb.back();
+    pcgb_hex_box c = p;
+    for (int a = 0; a < 3; ++a) {
+      if (p.ne[a] % 2 || p.ne[a] < 4 || p.e0[a] % 2 || p.ng[a] % 2)
+        return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: level %d cannot be halved (ne even and >= 4, e0 and ng even)", l - 1);
+      c.ng[a] = p.ng[a] / 2; c.e0[a] = p.e0[a] / 2; c.ne[a] = p.ne[a] / 2;
+    }
+    rb.push_back(c);
+  }
+  for (int l = 1; l <= la; ++l) {
+    const pcgb_halo_t hl = level_halos[l - 1];
+    if (!hl || hl->comm != s->comm || hl->nlocal != 3 * hex_geom(&rb[(size_t)l]).nfree_nodes)
+      return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the halo of level %d is missing, on another communicator or not of the level's size", l);
+  }
+  pcgb_hex_box gb = rb.back();
+  for (int a = 0; a < 3; ++a) { gb.e0[a] = 0; gb.ne[a] = gb.ng[a]; }
+  std::vector<HexGeom> geo{hex_geom(&gb)};
+  const int64_t ng_dofs = 3 * geo[0].nfree_nodes;
+  if (ng_dofs > kMgMaxGathered)
+    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the gathered level has %lld dofs (at most %lld)", (long long)ng_dofs, (long long)kMgMaxGathered);
+  if (gather->comm != s->comm || gather->nlocal != ng_dofs || gather->n_nbr != s->comm->nranks - 1 ||
+      gather->m != (int64_t)(s->comm->nranks - 1) * ng_dofs)
+    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the gather plan must list all %lld dofs of the gathered level for every other rank",
+                (long long)ng_dofs);
+  for (int l = 0; l <= la; ++l)
+    if (!d_own[l]) return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: null ownership weights of level %d", l);
+  mg_whole_box_levels(geo);
+  if (3 * geo.back().nfree_nodes > kMgMaxCoarse)
+    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the coarsest level has %lld dofs (at most %d)", (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
+  if ((size_t)la + 1 + geo.size() > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: more than %d levels", PCGB_MG_MAX_LEVELS);
+  pcgb_mg_t mg = new pcgb_mg_s();
+  mg->s = s; mg->degree = degree; mg->lo = lo; mg->la = la; mg->gather = gather;
+  mg->lv.resize((size_t)la + 1 + geo.size());
+  for (int l = 0; l <= la; ++l) {
+    MgLevel &L = mg->lv[(size_t)l];
+    const pcgb_hex_box &b = rb[(size_t)l];
+    pcgb_hex_box whole = b;
+    for (int a = 0; a < 3; ++a) { whole.e0[a] = 0; whole.ne[a] = whole.ng[a]; }
+    L.g = hex_geom(&b); L.glev = l; L.place = MgPlace{hex_geom(&whole), b.e0[0], b.e0[1], b.e0[2]};
+    L.halo = l ? level_halos[l - 1] : s->halo;
+  }
+  for (size_t k = 0; k < geo.size(); ++k) {
+    MgLevel &L = mg->lv[(size_t)la + 1 + k];
+    L.g = geo[k]; L.glev = la + (int)k; L.place = MgPlace{geo[k], 0, 0, 0};
+  }
+  const int rc = mg_build(mg, ke_host, E, h, d_minv_fine, d_own);
   if (rc != PCGB_OK) { pcgb_mg_destroy(mg); return rc; }
   *out = mg;
   return PCGB_OK;
@@ -1775,16 +1915,16 @@ int pcgb_mg_info(pcgb_mg_t mg, int32_t *nlevels, int64_t *n_level, double *lambd
 
 int pcgb_mg_restrict(pcgb_mg_t mg, int level, const double *d_fine, double *d_coarse, void *stream) {
   PCGB_TRY(require_device());
-  if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || !d_fine || !d_coarse) return fail(PCGB_ERR_ARG, "pcgb_mg_restrict: bad argument");
-  const MgLevel &F = mg->lv[(size_t)level], &C = mg->lv[(size_t)level + 1];
-  k_mg_restrict<<<mg_node_grid(C.g), 256, 0, (cudaStream_t)stream>>>(F.g, C.g, d_fine, d_coarse, nullptr);
-  PCGB_CHECK_LAUNCH();
-  return PCGB_OK;
+  if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || level == mg->la || !d_fine || !d_coarse)
+    return fail(PCGB_ERR_ARG, "pcgb_mg_restrict: bad argument");
+  int nl = 0;
+  return mg_restrict(mg, level, d_fine, d_coarse, (cudaStream_t)stream, &nl, nullptr);
 }
 
 int pcgb_mg_prolong_add(pcgb_mg_t mg, int level, const double *d_coarse, double *d_fine, void *stream) {
   PCGB_TRY(require_device());
-  if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || !d_fine || !d_coarse) return fail(PCGB_ERR_ARG, "pcgb_mg_prolong_add: bad argument");
+  if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || level == mg->la || !d_fine || !d_coarse)
+    return fail(PCGB_ERR_ARG, "pcgb_mg_prolong_add: bad argument");
   const MgLevel &F = mg->lv[(size_t)level], &C = mg->lv[(size_t)level + 1];
   k_mg_prolong_add<<<mg_node_grid(F.g), 256, 0, (cudaStream_t)stream>>>(F.g, C.g, d_coarse, d_fine, nullptr);
   PCGB_CHECK_LAUNCH();
@@ -1793,9 +1933,31 @@ int pcgb_mg_prolong_add(pcgb_mg_t mg, int level, const double *d_coarse, double 
 
 int pcgb_mg_smooth(pcgb_mg_t mg, int level, const double *d_b, double *d_x, void *stream) {
   PCGB_TRY(require_device());
-  if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || !d_b || !d_x) return fail(PCGB_ERR_ARG, "pcgb_mg_smooth: bad argument");
+  if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || level == mg->la || !d_b || !d_x)
+    return fail(PCGB_ERR_ARG, "pcgb_mg_smooth: bad argument");
   int nl = 0;
   return mg_smooth(mg, level, d_b, d_x, false, false, (cudaStream_t)stream, &nl, nullptr);
+}
+
+int pcgb_mg_info_ranks(pcgb_mg_t mg, int32_t *gather_level, int64_t *n_gathered) {
+  if (!mg) return fail(PCGB_ERR_ARG, "pcgb_mg_info_ranks: null argument");
+  if (gather_level) *gather_level = mg->la;
+  if (n_gathered) *n_gathered = mg->la >= 0 ? mg->lv[(size_t)mg->la + 1].n : 0;
+  return PCGB_OK;
+}
+
+int pcgb_mg_gather(pcgb_mg_t mg, const double *d_ranked, double *d_global, void *stream) {
+  PCGB_TRY(require_device());
+  if (!mg || mg->la < 0 || !d_ranked || !d_global) return fail(PCGB_ERR_ARG, "pcgb_mg_gather: bad argument (or a one-rank handle)");
+  int nl = 0;
+  return mg_gather(mg, d_ranked, d_global, (cudaStream_t)stream, &nl, nullptr);
+}
+
+int pcgb_mg_scatter(pcgb_mg_t mg, const double *d_global, double *d_ranked, void *stream) {
+  PCGB_TRY(require_device());
+  if (!mg || mg->la < 0 || !d_ranked || !d_global) return fail(PCGB_ERR_ARG, "pcgb_mg_scatter: bad argument (or a one-rank handle)");
+  int nl = 0;
+  return mg_scatter(mg, d_global, d_ranked, (cudaStream_t)stream, &nl, nullptr);
 }
 
 int pcgb_mg_coarse_solve(pcgb_mg_t mg, const double *d_r, double *d_z, void *stream) {

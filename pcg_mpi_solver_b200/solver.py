@@ -11,7 +11,7 @@ Mapping of solve()'s arguments onto the reference's per-rank state:
     b        Fext[LocDofEff]
     M        InvDiagPreCondVector0 (the INVERSE diagonal, applied as z = M*r, :447); None = identity
              (ExistDP0 False, :451); the string "jacobi" builds it from A like updatePreconditioner;
-             a multigrid.HexMultigrid built on A applies z = M r as one V-cycle (opt-in, one rank)
+             a multigrid.HexMultigrid built on A applies z = M r as one V-cycle (opt-in; on one rank or, built with `blocks`, across ranks)
     tol      GlobData['Tol']        maxiter  GlobData['MaxIter']
     x0       Un[LocDofEff]          w        DofWeightVector_Eff (taken from the operator if omitted)
 Return value (x, flag, relres, iters) follows MATLAB pcg like the reference: flag 0 converged,
@@ -133,6 +133,42 @@ class Communicator:
             pass
 
 
+def make_halo(comm: Communicator, nbr_ranks, lists, n: int) -> ctypes.c_void_p:
+    """Interface-exchange plan (pcgb_halo_create) of one rank over vectors of length n: neighbour ranks and, per neighbour,
+    the shared local indices.  Collective on the peer transport: every rank exports, all-gathers and imports; if ANY rank
+    fails (no CUDA IPC here) the whole communicator goes back to the NCCL transport so that all ranks stay on the same path.
+    The caller owns the handle (pcgb_halo_destroy) and calls this on the device of comm."""
+    lib = _lib.load()
+    h = ctypes.c_void_p()
+    nn = len(nbr_ranks)
+    ranks = (ctypes.c_int32 * max(nn, 1))(*[int(r) for r in nbr_ranks])
+    ptr = np.zeros(nn + 1, dtype=np.int64)
+    ptr[1:] = np.cumsum([len(v) for v in lists])
+    idx = np.ascontiguousarray(np.concatenate(lists), dtype=np.int64) if nn else np.zeros(1, dtype=np.int64)
+    _lib.check(lib.pcgb_halo_create(comm.handle, nn, ranks, ptr.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
+                                    idx.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), int(n), ctypes.byref(h)), "pcgb_halo_create")
+    if comm.transport == "peer" and comm._allgather is not None:
+        nb = int(lib.pcgb_halo_blob_bytes(h))
+        blob = (ctypes.c_ubyte * nb)()
+        ok = lib.pcgb_halo_export(h, blob) == 0
+        err = None if ok else lib.pcgb_last_error().decode()
+        blobs = comm._allgather(bytes(blob) if ok else b"")
+        if all(len(b) == nb for b in blobs):
+            buf = (ctypes.c_ubyte * (nb * comm.nranks)).from_buffer_copy(b"".join(blobs))
+            ok = lib.pcgb_halo_import(h, buf) == 0
+            err = None if ok else lib.pcgb_last_error().decode()
+        else:
+            ok = False
+        if not all(o == b"1" for o in comm._allgather(b"1" if ok else b"0")):
+            comm.peer_error = err or "a peer rank could not map the halo block"
+            if comm._has_nccl:
+                comm.set_transport("nccl")
+            else:
+                lib.pcgb_halo_destroy(h)
+                raise _lib.PcgbError(f"halo exchange over peer memory is not available ({comm.peer_error}) and the communicator has no NCCL")
+    return h
+
+
 # One record of the opt-in loop trace (struct PcgTraceRec / PcgCtrl in csrc/pcg_kernels.cuh, pcgb_solver_set_trace).
 CTRL_DTYPE = np.dtype([(f, "<f8") for f in ("rho", "rho_prev", "alpha", "beta", "pq", "normr", "normp", "normx", "normr_act",
                                            "normrmin", "tolb", "n2b", "eps")] +
@@ -196,34 +232,7 @@ class SubdomainOperator:
         with torch.cuda.device(self.device):
             if comm is not None and comm.nranks > 1:
                 # every rank builds a plan (also one without neighbours): the peer-transport import is collective
-                nn = len(self.nbr_ranks)
-                ranks = (ctypes.c_int32 * max(nn, 1))(*self.nbr_ranks)
-                ptr = np.zeros(nn + 1, dtype=np.int64)
-                ptr[1:] = np.cumsum([len(v) for v in self.ovrlp])
-                idx = np.ascontiguousarray(np.concatenate(self.ovrlp)) if nn else np.zeros(1, dtype=np.int64)
-                _lib.check(lib.pcgb_halo_create(comm.handle, nn, ranks, ptr.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
-                                                idx.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), self.n,
-                                                ctypes.byref(self._halo)), "pcgb_halo_create")
-                if comm.transport == "peer" and comm._allgather is not None:
-                    # collective: every rank exports, all-gathers and imports; if ANY rank fails (no CUDA IPC here) the whole
-                    # communicator goes back to the NCCL transport so that all ranks stay on the same path
-                    nb = int(lib.pcgb_halo_blob_bytes(self._halo))
-                    blob = (ctypes.c_ubyte * nb)()
-                    ok = lib.pcgb_halo_export(self._halo, blob) == 0
-                    err = None if ok else lib.pcgb_last_error().decode()
-                    blobs = comm._allgather(bytes(blob) if ok else b"")
-                    if all(len(b) == nb for b in blobs):
-                        buf = (ctypes.c_ubyte * (nb * comm.nranks)).from_buffer_copy(b"".join(blobs))
-                        ok = lib.pcgb_halo_import(self._halo, buf) == 0
-                        err = None if ok else lib.pcgb_last_error().decode()
-                    else:
-                        ok = False
-                    if not all(o == b"1" for o in comm._allgather(b"1" if ok else b"0")):
-                        comm.peer_error = err or "a peer rank could not map the halo block"
-                        if comm._has_nccl:
-                            comm.set_transport("nccl")
-                        else:
-                            raise _lib.PcgbError(f"halo exchange over peer memory is not available ({comm.peer_error}) and the communicator has no NCCL")
+                self._halo = make_halo(comm, self.nbr_ranks, self.ovrlp, self.n)
             from .ebe import EbeMatrixOrdered
             if isinstance(A, CsrMatrix):
                 create = lib.pcgb_solver_create
