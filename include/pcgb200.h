@@ -85,6 +85,13 @@ int64_t pcgb_spmv_stream_bytes(pcgb_csr_t A);
  * max row, tma, staged, x windows, staged doubles per tile (cap), max windows per tile, column-triple index (0/1),
  * interface tiles (-1 = no split registered), resident CTAs of the persistent kernel, column array released (0/1) */
 int pcgb_csr_plan_info(pcgb_csr_t A, int64_t info[16]);
+/* Distinct 3x3 blocks D of the value dictionary of the node-block kernel, 0 when the plan has none.  With D > 0 the SpMV
+ * streams a 16-bit block id per block instead of its 72 bytes of values and reads the values from a D-entry copy in
+ * shared memory: products bit-identical to the kernel that streams the values.  The plan builds one for node-block
+ * matrices with at most 1024 bitwise-distinct blocks (a structured mesh of one element type) when the values it replaces
+ * outweigh the per-CTA dictionary loads; PCGB_SPMV_VDICT=0 disables it, =2 drops the size condition.  d_val is still
+ * read by pcgb_csr_diag and must stay allocated. */
+int pcgb_csr_value_dict(pcgb_csr_t A);
 
 /* ---------------------------------------------------------------- vector kernels (a4-a10)
  * out[0] = sum_i a[i]*b[i]*w[i]   (w may be NULL = all ones).  np.dot(a, b*w) of

@@ -83,6 +83,10 @@ class CsrMatrix:
                 "x_cap", "max_windows_per_tile", "index_mode", "interface_tiles", "resident_ctas", "col_released"]
         return dict(zip(keys, [int(v) for v in info]))
 
+    def value_dict_blocks(self) -> int:
+        """Distinct 3x3 blocks in the node-block kernel's value dictionary (0: the kernel streams the values)."""
+        return int(_lib.load().pcgb_csr_value_dict(self._h))
+
     def release_col(self) -> bool:
         """Free the 4-byte column array when the selected SpMV kernel does not read it (the persistent staged-x kernel
         streams its own 16-bit indices): 2 GB at 128^3, 16 GB at 256^3.  The diagonal is cached first.  Returns True

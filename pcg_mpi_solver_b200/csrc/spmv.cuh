@@ -27,6 +27,8 @@ constexpr int kAlignMask = 7;      // tiles are staged from an 8-element aligned
 constexpr int kMaxRuns = 2048;     // staged-x plan: column runs per tile
 constexpr int kMaxWin = 256;       // staged-x plan: x windows per tile
 constexpr int kMaxXLen = 6144;     // staged-x plan: doubles of x staged per tile (48 KB)
+constexpr int kVdictMax = 1024;    // value dictionary: at most this many distinct blocks (72 KB of shared memory per CTA)
+constexpr int kVdictSlots = 4096;  // value dictionary: open-addressing hash table (load <= 1/4 at kVdictMax)
 
 // per-tile descriptor of the persistent kernel: everything a producer warp needs in one 32-byte load
 struct __align__(16) TileDesc {
@@ -78,6 +80,11 @@ struct CsrPlan {
   bool bsr = false;
   uint16_t *bidx = nullptr;        // [nnz/9 + 16]  staged x position of block t of node n at rowptr[3n]/9 + t
   int cap_blocks = 0, cap_nodes = 0, smem_bsr = 0, bsr_stage_bytes = 0, bsr_stages = 0, bsr_prod = 0, grid_bsr = 0, bsr_mode = 1, bsr_cw = 6;
+  // value dictionary of the node-block kernel: when the matrix has few bitwise-distinct 3x3 blocks (a structured mesh of
+  // one element type), each is stored once and every block position streams a 16-bit id instead of its 72 bytes of values
+  int vd = 0;                      // distinct blocks D (0: no dictionary, the kernel streams val)
+  uint16_t *bvid = nullptr;        // [nnz/9 + 16]  dictionary id of the block at bidx's position
+  double *vdict = nullptr;         // [vd * 9]      the blocks, row-major
   // interface-first split (multi-GPU overlap): tiles that own an interface row are listed first in desc_split
   struct TileDesc *desc_split = nullptr;  // [ntiles] permutation of tile_desc
   int nb_tiles = 0;                       // leading boundary tiles of desc_split
@@ -786,13 +793,17 @@ k_spmv_persist(const RP *__restrict__ rowptr, const uint16_t *__restrict__ lidx,
 //     phase 2   (after one named barrier, scratch double-buffered by tile parity) thread r < R adds the partials of its
 //               row in block order -> y[r]: fixed summation order, bit-reproducible, no shuffles, no atomics.
 // Per 9 non-zeros: 13 shared-memory loads + 3 stores instead of 27 loads, and 8 + 2/9 bytes from HBM instead of 10.
-template <bool DOT, int CW, typename RP>
+// VD (value dictionary): the producer copies the tile's 16-bit block ids where it copied val; every CTA holds the nvd
+// distinct blocks in shared memory and phase 1 reads the nine values of block b from vdict[bvid[b]] - the same bits in
+// the same FMA order, so y and x.y are bit-identical to the kernel that streams val.  4 + 2/9 bytes per block from HBM.
+template <bool DOT, int CW, typename RP, bool VD = false>
 __global__ void __launch_bounds__((CW + 4) * 32)
 k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, const double *__restrict__ val,
             const double *__restrict__ x, double *__restrict__ y, const TileDesc *__restrict__ desc,
             const int *__restrict__ win_start, const int *__restrict__ win_off, int ntiles, int64_t nnz, int cap_nnz,
             int cap_nodes, int cap_x, int cap_blocks, int stages, int stage_bytes, int mode, double *__restrict__ dot_partials,
-            const int *__restrict__ skip) {
+            const int *__restrict__ skip, const uint16_t *__restrict__ bvid = nullptr, const double *__restrict__ vdict = nullptr,
+            int nvd = 0) {
   if (skip != nullptr && *skip != 0) return;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   __shared__ uint64_t full_bar[8], empty_bar[8];
@@ -807,18 +818,21 @@ k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, co
   __syncthreads();
 
   // stage layout: sval[cap_nnz] f64 | sx[cap_x] f64 | snp[cap_nodes+2] i64 | sbidx[cap_blocks+16] u16 | meta[8] i32
-  const size_t off_sx = (size_t)cap_nnz * 8, off_snp = off_sx + (size_t)cap_x * 8;
-  const size_t off_sb = off_snp + (size_t)(cap_nodes + 2) * 8, off_meta = (off_sb + (size_t)(cap_blocks + 16) * 2 + 15) & ~(size_t)15;
+  //          VD:                      sx[cap_x] f64 | snp[cap_nodes+2] i64 | sbidx[cap_blocks+16] u16 | svid[cap_blocks+16] u16 | meta
+  const size_t sb_bytes = ((size_t)(cap_blocks + 16) * 2 + 15) & ~(size_t)15;
+  const size_t off_sx = VD ? 0 : (size_t)cap_nnz * 8, off_snp = off_sx + (size_t)cap_x * 8;
+  const size_t off_sb = off_snp + (size_t)(cap_nodes + 2) * 8, off_sv = off_sb + sb_bytes, off_meta = off_sb + (VD ? 2 : 1) * sb_bytes;
   // scratch behind the stages: row partials [2][3*cap_blocks] f64, node block offsets [2][cap_nodes+2] i32
   // (tried and rejected: a warp-segmented scan that leaves only a few partials per tile - no 25 KB scratch, larger stages - but
   //  35 shuffles per pass; 8 lanes per row in phase 2 serialises the two phases)
   // mode bit 1 (default): the row partials of a block OVERWRITE the block's own first-row values in the stage (the thread has all
   // nine values in registers by then) - no separate scratch, which buys a third stage per CTA; the stage is handed back to
-  // the producer only after phase 2 has read the partials.
-  const bool inplace = (mode & 2) != 0;
+  // the producer only after phase 2 has read the partials.  A VD stage holds no values: the scratch is always used.
+  const bool inplace = !VD && (mode & 2) != 0;
   const int part_len = inplace ? 0 : 3 * cap_blocks;
   double *spart = reinterpret_cast<double *>(smem_raw + (size_t)stages * stage_bytes);
   int *snbo = reinterpret_cast<int *>(spart + (size_t)2 * part_len);
+  double *sdict = reinterpret_cast<double *>(snbo + 2 * (cap_nodes + 2));   // VD: nvd blocks behind the scratch (16 B aligned)
 
   if (warp >= CW) {
     // ================= producer warp p (see k_spmv_persist): TMA val + block indices, cp.async node offsets + x windows
@@ -857,21 +871,29 @@ k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, co
       const int64_t ka = k0 & ~(int64_t)kAlignMask;
       mbar_wait(&empty_bar[s], ph ^ 1u);
       if (lane == 0) {
-        int64_t kend = (k1 + kAlignMask) & ~(int64_t)kAlignMask;
-        const int64_t lim = nnz & ~(int64_t)kAlignMask;
-        if (kend > lim) kend = lim;
-        const int nb = (int)(kend - ka);
-        // bidx is padded by 16 entries: the aligned window [ba, bend) never leaves the array
+        // bidx (and bvid) are padded by 16 entries: the aligned window [ba, bend) never leaves the array
         const int64_t b0 = k0 / 9, ba = b0 & ~(int64_t)kAlignMask;
         const int64_t bend = (b0 + cnt / 9 + kAlignMask) & ~(int64_t)kAlignMask;
         const uint32_t ib = (uint32_t)(bend - ba) * 2u;
-        mbar_expect_tx(&full_bar[s], (nb > 0 ? (uint32_t)nb * 8u : 0u) + ib);
-        if (nb > 0) bulk_g2s(sval, val + ka, (uint32_t)nb * 8u, &full_bar[s], pol);
-        if (ib > 0) bulk_g2s(sb, bidx + ba, ib, &full_bar[s], pol);
+        if (VD) {
+          mbar_expect_tx(&full_bar[s], 2u * ib);
+          if (ib > 0) {
+            bulk_g2s(sb, bidx + ba, ib, &full_bar[s], pol);
+            bulk_g2s(base + off_sv, bvid + ba, ib, &full_bar[s], pol);
+          }
+        } else {
+          int64_t kend = (k1 + kAlignMask) & ~(int64_t)kAlignMask;
+          const int64_t lim = nnz & ~(int64_t)kAlignMask;
+          if (kend > lim) kend = lim;
+          const int nb = (int)(kend - ka);
+          mbar_expect_tx(&full_bar[s], (nb > 0 ? (uint32_t)nb * 8u : 0u) + ib);
+          if (nb > 0) bulk_g2s(sval, val + ka, (uint32_t)nb * 8u, &full_bar[s], pol);
+          if (ib > 0) bulk_g2s(sb, bidx + ba, ib, &full_bar[s], pol);
+        }
         meta[0] = r0; meta[1] = R; meta[2] = tile; meta[3] = cnt;
         meta[4] = (int)(k0 & 0xffffffff); meta[5] = (int)(k0 >> 32); meta[6] = (int)(b0 - ba); meta[7] = uni;
       }
-      {
+      if (!VD) {
         const int64_t lim = nnz & ~(int64_t)kAlignMask;
         const int64_t kt = (lim > ka ? lim : ka) + lane;
         if (lane <= kAlignMask && kt >= lim && kt < k1) sval[kt - ka] = val[kt];
@@ -904,6 +926,10 @@ k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, co
 
   // ================= consumer warps (CW * 32 threads, tid = consumer thread id)
   constexpr int NT = CW * 32;
+  if (VD) {   // the dictionary, once per launch (from L2 after the first CTAs), while the producers fill the first stages
+    for (int i = tid; i < 9 * nvd; i += NT) sdict[i] = __ldg(vdict + i);
+    named_bar_sync(1, NT);
+  }
   double dsum = 0.0;
   for (int it = 0;; ++it) {
     const int tile = blockIdx.x + it * gridDim.x;
@@ -925,6 +951,7 @@ k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, co
     const int k0l = (int)(k0 & kAlignMask);
     const int NN = R / 3, NB = cnt / 9;
     const uint16_t *sbt = sb + meta[6];
+    const uint16_t *svdt = reinterpret_cast<const uint16_t *>(base + off_sv) + meta[6];   // VD only
     const double *svt = sval + k0l;
     // uniform tile (all nodes have the same number of blocks - the interior of a structured mesh): node = b / Lb, no look-ups
     const bool uni = (mode & 1) != 0 && meta[7] != 0 && NN > 0 && NB >= 2 * NN;   // (>= 2 blocks per node: the reciprocal fits 32 bits)
@@ -934,23 +961,31 @@ k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, co
     for (int i = tid; i <= NN; i += NT) nbo[i] = uni ? i * Lbu : (int)((int64_t)snp[i] - k0) / 9;
     // ---- phase 1: one 3x3 block per thread and pass
     for (int b = tid; b < NB; b += NT) {
-      int noff, L, t3;
-      if (uni) {
-        const int i = (int)__umulhi((unsigned)b, magic);
-        noff = i * 9 * Lbu; L = 3 * Lbu; t3 = 3 * (b - i * Lbu);
+      const double *pv;
+      int L;
+      if (VD) {
+        // dictionary entry: rows 3 values apart (ids of the tile's blocks at the same offset as sbt)
+        pv = sdict + 9 * (int)svdt[b];
+        L = 3;
       } else {
-        int lo = 0, hi = NN - 1;                     // node of block b: last i with (snp[i] - k0) <= 9 b
-        const int kb = 9 * b;
-        while (lo < hi) {
-          const int mid = (lo + hi + 1) >> 1;
-          if ((int)((int64_t)snp[mid] - k0) <= kb) lo = mid; else hi = mid - 1;
+        int noff, t3;
+        if (uni) {
+          const int i = (int)__umulhi((unsigned)b, magic);
+          noff = i * 9 * Lbu; L = 3 * Lbu; t3 = 3 * (b - i * Lbu);
+        } else {
+          int lo = 0, hi = NN - 1;                     // node of block b: last i with (snp[i] - k0) <= 9 b
+          const int kb = 9 * b;
+          while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if ((int)((int64_t)snp[mid] - k0) <= kb) lo = mid; else hi = mid - 1;
+          }
+          noff = (int)((int64_t)snp[lo] - k0);
+          L = ((int)((int64_t)snp[lo + 1] - k0) - noff) / 3;   // non-zeros per row of this node
+          t3 = (kb - noff) / 3;                                  // 3 t, t = b - noff / 9
         }
-        noff = (int)((int64_t)snp[lo] - k0);
-        L = ((int)((int64_t)snp[lo + 1] - k0) - noff) / 3;   // non-zeros per row of this node
-        t3 = (kb - noff) / 3;                                  // 3 t, t = b - noff / 9
+        pv = svt + noff + t3;
       }
       const int ii = sbt[b];
-      const double *pv = svt + noff + t3;
       const double x0 = sx[ii], x1 = sx[ii + 1], x2 = sx[ii + 2];
       const double a0 = pv[0], a1 = pv[1], a2 = pv[2];
       const double b0 = pv[L], b1 = pv[L + 1], b2 = pv[L + 2];
@@ -1046,6 +1081,71 @@ __global__ void k_build_bidx(const RP *__restrict__ rowptr, const uint16_t *__re
   }
 }
 
+// ---- value dictionary plan helpers
+// A block is keyed by its nine values as uint64 bit patterns (-0.0 and 0.0, or two NaN payloads, are different blocks).  A
+// table slot holds the smallest (first-row position k << 24 | row length L) of the blocks with that value, so that the
+// representative is the first occurrence whatever the order the threads arrive in: slots only go EMPTY -> key (CAS) and then
+// down (atomicMin among equal blocks), so a stale non-empty read still names the right value.
+constexpr unsigned long long kVdEmpty = ~0ull;
+__device__ __forceinline__ void vd_block_bits(const double *__restrict__ val, int64_t k, int64_t L, unsigned long long w[9]) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+#pragma unroll
+    for (int c = 0; c < 3; ++c) w[3 * r + c] = (unsigned long long)__double_as_longlong(__ldg(val + k + r * L + c));
+}
+template <typename RP>
+__global__ void k_vdict_insert(const RP *__restrict__ rowptr, const double *__restrict__ val, int64_t nnodes,
+                               unsigned long long *__restrict__ table, uint16_t *__restrict__ bvid, int *__restrict__ count,
+                               int *__restrict__ fail) {
+  for (int64_t n = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; n < nnodes; n += (int64_t)gridDim.x * blockDim.x) {
+    if (*(volatile int *)fail) return;
+    const int64_t a0 = rowptr[3 * n], L = (int64_t)rowptr[3 * n + 1] - a0;
+    for (int64_t t3 = 0; t3 < L; t3 += 3) {
+      unsigned long long w[9];
+      vd_block_bits(val, a0 + t3, L, w);
+      unsigned long long h = 0x9e3779b97f4a7c15ull;
+#pragma unroll
+      for (int j = 0; j < 9; ++j) { h ^= w[j]; h *= 0xff51afd7ed558ccdull; h ^= h >> 32; }
+      const unsigned long long key = ((unsigned long long)(a0 + t3) << 24) | (unsigned long long)L;
+      int probe = 0, slot = (int)(h & (kVdictSlots - 1));
+      for (;; ++probe, slot = (slot + 1) & (kVdictSlots - 1)) {
+        if (probe == kVdictSlots) { atomicExch(fail, 2); return; }
+        unsigned long long v = *(volatile unsigned long long *)(table + slot);
+        if (v == kVdEmpty) {
+          v = atomicCAS(table + slot, kVdEmpty, key);
+          if (v == kVdEmpty) {
+            if (atomicAdd(count, 1) >= kVdictMax) { atomicExch(fail, 1); return; }
+            break;
+          }
+        }
+        unsigned long long u[9];
+        vd_block_bits(val, (int64_t)(v >> 24), (int64_t)(v & 0xffffff), u);
+        bool eq = true;
+#pragma unroll
+        for (int j = 0; j < 9; ++j) eq = eq && u[j] == w[j];
+        if (eq) {
+          if (key < v) atomicMin(table + slot, key);
+          break;
+        }
+      }
+      bvid[a0 / 9 + t3 / 3] = (uint16_t)slot;   // slot for now; k_vdict_finish maps it to the id
+    }
+  }
+}
+// slot -> id over all blocks, and the dictionary itself from the representatives (keys in id order)
+__global__ void k_vdict_finish(uint16_t *__restrict__ bvid, int64_t nblk, const uint16_t *__restrict__ slot_id,
+                               const double *__restrict__ val, const unsigned long long *__restrict__ rep, int nd,
+                               double *__restrict__ vdict) {
+  for (int64_t g = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; g < nblk; g += (int64_t)gridDim.x * blockDim.x)
+    bvid[g] = slot_id[bvid[g]];
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < 9 * nd) {
+    const unsigned long long v = rep[i / 9];
+    const int r = (i % 9) / 3, c = i % 3;
+    vdict[i] = val[(int64_t)(v >> 24) + r * (int64_t)(v & 0xffffff) + c];
+  }
+}
+
 // ---- T3 plan helpers
 // every row offset a multiple of 3  <=>  every row length a multiple of 3 (rowptr[0] = 0)
 template <typename RP>
@@ -1121,6 +1221,58 @@ struct DevTmp {
   ~DevTmp() { if (p) cudaFree(p); }
   template <typename T> T *as() const { return static_cast<T *>(p); }
 };
+
+// Value dictionary of a node-block matrix (P.vd = D distinct blocks, P.bvid, P.vdict), or P.vd = 0 when it has more than
+// kVdictMax distinct blocks.  Ids follow the first occurrence of each value, so the plan is deterministic.  mode 1 also
+// refuses a dictionary that the grid's CTAs would load (once each per launch) in more bytes than half the values it replaces.
+constexpr int kVdStages = 4;   // default ring of a dictionary plan (its stages are small)
+template <typename RP>
+inline int build_vdict(CsrPlan &P, cudaStream_t st, int mode, int grid) {
+  P.vd = 0;
+  const int64_t nblk = P.nnz / 9, nnodes = P.nrows / 3;
+  if (nblk == 0 || P.nnz >= (int64_t(1) << 40) || P.max_row >= (1 << 24)) return PCGB_OK;   // key = k << 24 | L
+  DevTmp t_table, t_ctl, t_map;
+  PCGB_CUDA(cudaMalloc(&t_table.p, kVdictSlots * sizeof(unsigned long long)));
+  PCGB_CUDA(cudaMalloc(&t_ctl.p, 2 * sizeof(int)));
+  PCGB_CUDA(cudaMemsetAsync(t_table.p, 0xff, kVdictSlots * sizeof(unsigned long long), st));
+  PCGB_CUDA(cudaMemsetAsync(t_ctl.p, 0, 2 * sizeof(int), st));
+  PCGB_CUDA(cudaMalloc(&P.bvid, ((size_t)nblk + 16) * sizeof(uint16_t)));
+  PCGB_CUDA(cudaMemsetAsync(P.bvid + nblk, 0, 16 * sizeof(uint16_t), st));
+  k_vdict_insert<RP><<<(int)std::min<int64_t>((nnodes + 127) / 128, (int64_t)num_sms() * 16), 128, 0, st>>>(
+      static_cast<const RP *>(P.rowptr), P.val, nnodes, t_table.as<unsigned long long>(), P.bvid, t_ctl.as<int>(), t_ctl.as<int>() + 1);
+  PCGB_CHECK_LAUNCH();
+  int h_ctl[2] = {0, 0};
+  std::vector<unsigned long long> table(kVdictSlots);
+  PCGB_CUDA(cudaMemcpyAsync(h_ctl, t_ctl.p, sizeof(h_ctl), cudaMemcpyDeviceToHost, st));
+  PCGB_CUDA(cudaMemcpyAsync(table.data(), t_table.p, kVdictSlots * sizeof(unsigned long long), cudaMemcpyDeviceToHost, st));
+  PCGB_CUDA(cudaStreamSynchronize(st));
+  const int nd = h_ctl[0];
+  if (h_ctl[1] != 0 || nd < 1 || nd > kVdictMax || (mode == 1 && nblk < 2 * (int64_t)nd * grid)) {
+    cudaFree(P.bvid); P.bvid = nullptr;
+    return PCGB_OK;
+  }
+  std::vector<std::pair<unsigned long long, int>> occ;   // (representative key, slot)
+  for (int s = 0; s < kVdictSlots; ++s) if (table[(size_t)s] != kVdEmpty) occ.emplace_back(table[(size_t)s], s);
+  std::sort(occ.begin(), occ.end());
+  if ((int)occ.size() != nd) return fail(PCGB_ERR_CUDA, "value dictionary: %d slots for %d blocks", (int)occ.size(), nd);
+  // one upload: slot -> id (u16 [kVdictSlots]) then the representatives in id order (u64 [nd])
+  std::vector<unsigned char> buf((size_t)kVdictSlots * 2 + (size_t)nd * 8);
+  uint16_t *slot_id = reinterpret_cast<uint16_t *>(buf.data());
+  unsigned long long *rep = reinterpret_cast<unsigned long long *>(buf.data() + (size_t)kVdictSlots * 2);
+  for (int s = 0; s < kVdictSlots; ++s) slot_id[s] = 0;
+  for (int i = 0; i < nd; ++i) { slot_id[occ[(size_t)i].second] = (uint16_t)i; rep[i] = occ[(size_t)i].first; }
+  PCGB_CUDA(cudaMalloc(&t_map.p, buf.size()));
+  PCGB_CUDA(cudaMemcpyAsync(t_map.p, buf.data(), buf.size(), cudaMemcpyHostToDevice, st));
+  PCGB_CUDA(cudaMalloc(&P.vdict, (size_t)nd * 9 * sizeof(double)));
+  const int64_t work = std::max<int64_t>(nblk, 9 * (int64_t)nd);
+  k_vdict_finish<<<(int)std::min<int64_t>((work + 255) / 256, (int64_t)num_sms() * 16), 256, 0, st>>>(
+      P.bvid, nblk, t_map.as<uint16_t>(), P.val, reinterpret_cast<const unsigned long long *>(t_map.as<unsigned char>() + (size_t)kVdictSlots * 2),
+      nd, P.vdict);
+  PCGB_CHECK_LAUNCH();
+  PCGB_CUDA(cudaStreamSynchronize(st));   // t_map is freed on return
+  P.vd = nd;
+  return PCGB_OK;
+}
 
 template <typename RP>
 inline int build_plan_t(CsrPlan &P, cudaStream_t st, int bsr_tile = 0, int attempt = 0) {
@@ -1356,7 +1508,8 @@ inline int build_plan_t(CsrPlan &P, cudaStream_t st, int bsr_tile = 0, int attem
             PCGB_CUDA(cudaStreamSynchronize(st));
             P.cap_blocks = (P.cap_nnz / 9 + 2 + 7) & ~7;
             P.cap_nodes = (P.cap_rows / 3 + 2 + 1) & ~1;
-            P.bsr_stage_bytes = P.cap_nnz * 8 + P.cap_x * 8 + (P.cap_nodes + 2) * 8 + (((P.cap_blocks + 16) * 2 + 15) & ~15) + 32;
+            const int sb_bytes = ((P.cap_blocks + 16) * 2 + 15) & ~15;
+            P.bsr_stage_bytes = P.cap_nnz * 8 + P.cap_x * 8 + (P.cap_nodes + 2) * 8 + sb_bytes + 32;
             P.bsr_stage_bytes = (P.bsr_stage_bytes + 127) & ~127;
             const bool inplace = env_int("PCGB_BSR_INPLACE", 1) != 0;
             P.bsr_mode = (env_int("PCGB_BSR_UNI", 1) ? 1 : 0) | (inplace ? 2 : 0);
@@ -1398,6 +1551,25 @@ inline int build_plan_t(CsrPlan &P, cudaStream_t st, int bsr_tile = 0, int attem
               P.persist = true;
               P.ctas_per_sm = std::min(bct > 0 ? bct : 1, bfit);
               P.grid_bsr = std::min(P.ntiles, num_sms() * P.ctas_per_sm);
+              // value dictionary (PCGB_SPMV_VDICT: 0 off, 1 when it pays, 2 whenever the blocks fit it).  The tiles, the grid and
+              // the consumer warps stay those of the plan without one - they fix the order in which x.y is summed, so y and
+              // x.y are the same bits either way; only the ring changes: a stage holds no values (sx | snp | bidx | bvid |
+              // meta), the row partials go to the scratch, and the dictionary sits behind it.
+              const int vd_mode = env_int("PCGB_SPMV_VDICT", 1);
+              if (vd_mode != 0) PCGB_TRY(build_vdict<RP>(P, st, vd_mode, P.grid_bsr));
+              if (P.vd) {
+                int vst = std::min(std::max(env_int("PCGB_SPMV_STAGES", kVdStages), 1), 8);
+                const int vprod = vst >= 4 ? 4 : vst;
+                vst -= vst % vprod;
+                const int vstage = (P.cap_x * 8 + (P.cap_nodes + 2) * 8 + 2 * sb_bytes + 32 + 127) & ~127;
+                const int vsmem = vst * vstage + 6 * P.cap_blocks * 8 + 2 * (P.cap_nodes + 2) * 4 + 64 + 72 * P.vd;
+                if (vsmem <= 226 * 1024 && (227 * 1024) / (vsmem + 2048) >= P.ctas_per_sm) {
+                  P.bsr_stages = vst; P.bsr_prod = vprod; P.bsr_stage_bytes = vstage; P.smem_bsr = vsmem; P.bsr_mode &= ~2;
+                } else {
+                  cudaFree(P.bvid); cudaFree(P.vdict);
+                  P.bvid = nullptr; P.vdict = nullptr; P.vd = 0;
+                }
+              }
               P.grid_persist = P.grid_bsr; P.smem_persist = P.smem_bsr; P.stages = P.bsr_stages; P.stage_bytes = P.bsr_stage_bytes;
               cudaFree(P.lidx); P.lidx = nullptr;           // the node-block kernel is the only consumer of the index stream now
               if (P.t3) { cudaFree(P.lidx3); P.lidx3 = nullptr; P.t3 = false; }
@@ -1508,10 +1680,10 @@ inline int launch_persist_lanes(const CsrPlan &P, const double *x, double *y, cu
   }
 }
 
-template <bool DOT, int CW, typename RP>
+template <bool DOT, int CW, typename RP, bool VD>
 inline int launch_bsr_cw(const CsrPlan &P, const double *x, double *y, cudaStream_t st, const int *skip, const TileDesc *desc,
                          int ntiles, int grid, double *dotp) {
-  auto kern = k_spmv_bsr3<DOT, CW, RP>;
+  auto kern = k_spmv_bsr3<DOT, CW, RP, VD>;
   if (skip == reinterpret_cast<const int *>(1)) {
     PCGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
     return PCGB_OK;
@@ -1519,19 +1691,27 @@ inline int launch_bsr_cw(const CsrPlan &P, const double *x, double *y, cudaStrea
   if (ntiles == 0) return PCGB_OK;
   kern<<<grid, (CW + P.bsr_prod) * 32, P.smem_bsr, st>>>(static_cast<const RP *>(P.rowptr), P.bidx, P.val, x, y, desc, P.win_start,
                                                                   P.win_off, ntiles, P.nnz, P.cap_nnz, P.cap_nodes, P.cap_x, P.cap_blocks,
-                                                                  P.bsr_stages, P.bsr_stage_bytes, P.bsr_mode, dotp, skip);
+                                                                  P.bsr_stages, P.bsr_stage_bytes, P.bsr_mode, dotp, skip, P.bvid,
+                                                                  P.vdict, P.vd);
   PCGB_CHECK_LAUNCH();
   return PCGB_OK;
+}
+
+template <bool DOT, typename RP, bool VD>
+inline int launch_bsr_vd(const CsrPlan &P, const double *x, double *y, cudaStream_t st, const int *skip, const TileDesc *desc,
+                         int ntiles, int grid, double *dotp) {
+  // consumer warps per CTA: 6 by default; 8 and 12 are selectable with PCGB_BSR_CW.  On H100 (hex 128^3) the three are equal
+  // within noise: 1.450-1.452 ms stand-alone (tools/spmv_sweep.py), 604-606 PCG it/s in bench.py.
+  if (P.bsr_cw == 8) return launch_bsr_cw<DOT, 8, RP, VD>(P, x, y, st, skip, desc, ntiles, grid, dotp);
+  if (P.bsr_cw == 12) return launch_bsr_cw<DOT, 12, RP, VD>(P, x, y, st, skip, desc, ntiles, grid, dotp);
+  return launch_bsr_cw<DOT, 6, RP, VD>(P, x, y, st, skip, desc, ntiles, grid, dotp);
 }
 
 template <bool DOT, typename RP>
 inline int launch_bsr_inst(const CsrPlan &P, const double *x, double *y, cudaStream_t st, const int *skip, const TileDesc *desc,
                            int ntiles, int grid, double *dotp) {
-  // consumer warps per CTA: 6 by default; 8 and 12 are selectable with PCGB_BSR_CW.  On H100 (hex 128^3) the three are equal
-  // within noise: 1.450-1.452 ms stand-alone (tools/spmv_sweep.py), 604-606 PCG it/s in bench.py.
-  if (P.bsr_cw == 8) return launch_bsr_cw<DOT, 8, RP>(P, x, y, st, skip, desc, ntiles, grid, dotp);
-  if (P.bsr_cw == 12) return launch_bsr_cw<DOT, 12, RP>(P, x, y, st, skip, desc, ntiles, grid, dotp);
-  return launch_bsr_cw<DOT, 6, RP>(P, x, y, st, skip, desc, ntiles, grid, dotp);
+  if (P.vd) return launch_bsr_vd<DOT, RP, true>(P, x, y, st, skip, desc, ntiles, grid, dotp);
+  return launch_bsr_vd<DOT, RP, false>(P, x, y, st, skip, desc, ntiles, grid, dotp);
 }
 
 inline int launch_persist_any(const CsrPlan &P, const double *x, double *y, bool with_dot, cudaStream_t st, const int *skip,
@@ -1652,6 +1832,7 @@ inline void free_plan(CsrPlan &P) {
   cudaFree(P.fix_row); cudaFree(P.fix_first); cudaFree(P.fix_cnt);
   cudaFree(P.tile_xlen); cudaFree(P.tile_win); cudaFree(P.win_start); cudaFree(P.win_off); cudaFree(P.lidx);
   cudaFree(P.tile_desc); cudaFree(P.lidx3); cudaFree(P.bidx); cudaFree(P.desc_split); cudaFree(P.dot_partials_split); cudaFree(P.diag_cache);
+  cudaFree(P.bvid); cudaFree(P.vdict);
 }
 
 }  // namespace pcgb

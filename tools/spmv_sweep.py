@@ -49,5 +49,6 @@ for cfg in configs:
     torch.cuda.synchronize()
     ms = e0.elapsed_time(e1) / reps
     print(json.dumps({**cfg, "ms": round(ms, 4), "GBps": round(M.spmv_bytes() / ms / 1e6, 1), "smem": M.plan_info()["smem_bytes"], "staged": M.plan_info()["staged"], "xcap": M.plan_info()["x_cap"], "maxw": M.plan_info()["max_windows_per_tile"], "mode": M.plan_info()["index_mode"], "lanes": M.plan_info()["lanes"],
-                      "streamGBps": round(M.stream_bytes() / ms / 1e6, 1), "ctas": M.plan_info()["resident_ctas"]}), flush=True)
+                      "streamGBps": round(M.stream_bytes() / ms / 1e6, 1), "ctas": M.plan_info()["resident_ctas"],
+                      "tile": M.plan_info()["tile_items"], "vdict": M.value_dict_blocks()}), flush=True)
     del M
