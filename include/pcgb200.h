@@ -316,14 +316,17 @@ int pcgb_hex_fill(const pcgb_hex_box *box, const double *ke_host, double ck, con
  * d_minv_fine (n doubles); the coarse levels use their own diagonals.
  * PCGB_ERR_ARG before anything is allocated: a solver with a halo plan or communicator, a box with e0 != 0 or ng != ne, a
  * box that does not coarsen at least once, a coarsest level above 1536 dofs, degree < 1, lo outside (0, 1.1), E or h <= 0,
- * or an operator whose size is not the box's.  The solver must outlive the handle; destroying the handle also drops the
+ * or an operator whose size is not the box's.  PCGB_ERR_ARG after allocation, with every allocation given back: a coarsest
+ * matrix whose Cholesky factorisation meets a pivot that is not positive (e.g. nu >= 0.5).  The solver must outlive the handle; destroying the handle also drops the
  * solver's cached graph of MG iterations.  Create synchronises the device first (d_minv_fine may come from any stream)
  * and again before it returns.                                                                                          */
 #define PCGB_MG_MAX_LEVELS 32
 int pcgb_mg_create(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, const double *d_minv_fine,
                    int degree, double lo, pcgb_mg_t *out);
 int pcgb_mg_destroy(pcgb_mg_t mg);
-int pcgb_mg_apply(pcgb_mg_t mg, const double *d_r, double *d_z, void *stream); /* z = M r (one V-cycle) */
+/* z = M r (one V-cycle).  PCGB_ERR_ARG, before any launch, when [d_r, d_r + n) and [d_z, d_z + n) overlap (z = r included):
+ * the pre-smoother writes z while the post-smoother still reads r. */
+int pcgb_mg_apply(pcgb_mg_t mg, const double *d_r, double *d_z, void *stream);
 /* levels; n per level, lambda per level (0 for the coarsest) into arrays of PCGB_MG_MAX_LEVELS entries; device bytes the
  * hierarchy allocated (vectors, coarse CSR, dense factor; the coarse SpMV plans' tile tables are not counted).  Any may be NULL. */
 int pcgb_mg_info(pcgb_mg_t mg, int32_t *nlevels, int64_t *n_level, double *lambda, int64_t *bytes);

@@ -1901,6 +1901,9 @@ int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked,
 int pcgb_mg_apply(pcgb_mg_t mg, const double *d_r, double *d_z, void *stream) {
   PCGB_TRY(require_device());
   if (!mg || !d_r || !d_z) return fail(PCGB_ERR_ARG, "pcgb_mg_apply: null argument");
+  // the pre-smoother writes z while the post-smoother still reads r as the fine right-hand side
+  const uintptr_t r0 = (uintptr_t)d_r, z0 = (uintptr_t)d_z, nb = (uintptr_t)mg->lv[0].n * sizeof(double);
+  if (r0 < z0 + nb && z0 < r0 + nb) return fail(PCGB_ERR_ARG, "pcgb_mg_apply: r and z overlap");
   int nl = 0;
   return mg_vcycle(mg, d_r, d_z, (cudaStream_t)stream, &nl, nullptr);
 }

@@ -32,11 +32,12 @@ def start_vector(n):
 
 
 class HexOp:
-    """y = A x of the clamped box ne (spacing h, E = 1, nu = 0.3) in the free-dof numbering, matrix-free."""
+    """y = A x of the clamped box ne (spacing h, Young's modulus E, Poisson ratio nu) in the free-dof numbering, matrix-free.
+    The element matrix is that of R.hex_box_csr: hex_ke(1, nu) * (E h)."""
 
-    def __init__(self, ne, h, nu=0.3):
+    def __init__(self, ne, h, nu=0.3, E=1.0):
         self.ne = tuple(ne)
-        self.ke = R.hex_ke(1.0, nu) * h
+        self.ke = R.hex_ke(1.0, nu) * (E * h)
         self.n = 3 * nfree(ne)
         nx, ny, nz = ne
         d = np.zeros((nz + 1, ny + 1, nx + 1, 3))
@@ -164,12 +165,13 @@ def lanczos_lambda(A, dinv, steps=LANCZOS_STEPS):
 
 
 class HostMultigrid:
-    """The V-cycle of pcgb_mg_apply on the host.  lambdas: use these estimates (e.g. the device's) instead of computing them."""
+    """The V-cycle of pcgb_mg_apply on the host.  lambdas: use these estimates (e.g. the device's) instead of computing them.
+    E, nu: the material of every level (the coarse matrices are rediscretised with the fine level's E and nu)."""
 
-    def __init__(self, ne, h, degree=2, lo=0.25, lambdas=None, minv=None):
+    def __init__(self, ne, h, degree=2, lo=0.25, lambdas=None, minv=None, E=1.0, nu=0.3):
         self.ne = levels_of(ne)
         self.degree, self.lo = degree, lo
-        self.A = [HexOp(n_, h * 2 ** l) for l, n_ in enumerate(self.ne)]
+        self.A = [HexOp(n_, h * 2 ** l, nu=nu, E=E) for l, n_ in enumerate(self.ne)]
         self.dinv = [1.0 / A.diag for A in self.A]
         if minv is not None:
             self.dinv[0] = minv
@@ -177,7 +179,7 @@ class HostMultigrid:
         self.lam = list(lambdas[:L - 1]) if lambdas is not None else [lanczos_lambda(self.A[l], self.dinv[l]) for l in range(L - 1)]
         self.coef = [cheb_coeffs(lam, degree, lo) for lam in self.lam]
         nec = self.ne[-1]
-        Ac = R.hex_box_csr(nec, (0, 0, 0), nec, h=h * 2 ** (L - 1)).toarray()
+        Ac = R.hex_box_csr(nec, (0, 0, 0), nec, E=E, nu=nu, h=h * 2 ** (L - 1)).toarray()
         self.chol = np.linalg.cholesky(Ac)
 
     def coarse_solve(self, r):
@@ -211,6 +213,29 @@ class HostMultigrid:
             x[l] = prolong_add(x[l + 1], x[l], self.ne[l])[0]
             x[l], _ = self.smooth(l, b[l], x[l], False)
         return x[0]
+
+
+# fine box -> dofs of its coarsest level: both sides of one 1024-thread pass of the one-CTA Cholesky kernels (1020 | 1026,
+# and n - k - 1 = 1024 inside 1026 and 1029), the smallest level and the largest one allowed
+COARSE_SIZES = {(4, 4, 4): 54, (6, 6, 6): 144, (14, 14, 10): 1008, (10, 6, 32): 1020, (4, 16, 36): 1026, (14, 12, 12): 1029,
+                (16, 14, 14): 1536}
+# materials and spacings of the material tests: (E, nu, h)
+MATERIALS = [(E, nu, h) for E in (7.5, 210.0) for nu in (0.2, 0.45) for h in (0.125, 2.0)]
+# a Poisson ratio above 1/2: negative bulk modulus, indefinite stiffness matrices
+BAD_NU_BOX, BAD_NU = (8, 8, 8), 0.6
+
+
+def coarsest_matrix(ne, h, E=1.0, nu=0.3):
+    """Dense matrix of the coarsest level of the fine box ne (spacing h), as pcgb_mg_create factors it."""
+    lv = levels_of(ne)
+    return R.hex_box_csr(lv[-1], (0, 0, 0), lv[-1], E=E, nu=nu, h=h * 2 ** (len(lv) - 1)).toarray()
+
+
+def refined_solve(A, r):
+    """A^-1 r by numpy, refined once with the residual r - A z summed in long double: the reference of the coarse solve."""
+    z = np.linalg.solve(A, r)
+    res = r.astype(np.longdouble) - A.astype(np.longdouble) @ z.astype(np.longdouble)
+    return z + np.linalg.solve(A, res.astype(np.float64))
 
 
 def pcg(A, b, M, tol, maxiter):

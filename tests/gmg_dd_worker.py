@@ -1,5 +1,5 @@
 """Multi-rank worker for the multigrid preconditioner across ranks (launched by tests/test_gpu_gmg_dd.py through
-torch.distributed.run; argv: out.json pgrid per kind).
+torch.distributed.run; argv: out.json pgrid per kind [degree lo E nu], the last four 2 0.25 1 0.3 when omitted).
 
 Every rank builds its box of partition_blocks(ng, pgrid) (per^3 elements), its operator (csr / ebe_ordered / ebe) with the
 interface lists of hexmesh, and HexMultigrid(op, block, blocks=...).  It also builds the one-rank HexMultigrid of the global
@@ -40,6 +40,7 @@ def _sha(a):
 
 def main():
     out_path, pgrid, per, kind = sys.argv[1], tuple(int(v) for v in sys.argv[2].split(",")), int(sys.argv[3]), sys.argv[4]
+    degree, lo, E, nu = (int(sys.argv[5]), float(sys.argv[6]), float(sys.argv[7]), float(sys.argv[8])) if len(sys.argv) > 5 else (2, 0.25, 1.0, 0.3)
     rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
     local = int(os.environ.get("LOCAL_RANK", rank))
     shared = os.environ.get("PCGB_SHARED_GPU", "0") == "1"
@@ -77,7 +78,7 @@ def main():
 
     ng = tuple(pgrid[a] * per for a in range(3))
     h = 1.0 / ng[0]
-    blocks = [HexBlock(b.ng, b.e0, b.ne, h=h) for b in partition_blocks(ng, pgrid)]
+    blocks = [HexBlock(b.ng, b.e0, b.ne, h=h, E=E, nu=nu) for b in partition_blocks(ng, pgrid)]
     blk = blocks[rank]
 
     def operator(b):
@@ -86,13 +87,13 @@ def main():
     nbr, lists, w = interface_lists(blocks, rank)
     n_global = 3 * G.nfree(ng)
     op = SubdomainOperator(operator(blk), comm, nbr, lists, w, n_global=n_global)
-    mg = HexMultigrid(op, blk, blocks=blocks)
+    mg = HexMultigrid(op, blk, degree=degree, lo=lo, blocks=blocks)
     info = mg.info()
     la = info["gather_level"]
     # the one-rank hierarchy of the global mesh, built by every rank on its own
-    gblk = HexBlock(ng, (0, 0, 0), ng, h=h)
+    gblk = HexBlock(ng, (0, 0, 0), ng, h=h, E=E, nu=nu)
     op1 = SubdomainOperator(operator(gblk))
-    mg1 = HexMultigrid(op1, gblk)
+    mg1 = HexMultigrid(op1, gblk, degree=degree, lo=lo)
     info1 = mg1.info()
     allinfo = allg((info["n"][la + 1:], [float(v).hex() for v in info["lambda"]], info["levels"]))
     note(all(a[1:] == allinfo[0][1:] and a[0] == allinfo[0][0] for a in allinfo), "lambda / level sizes differ across ranks")
@@ -139,7 +140,7 @@ def main():
     note(all(s == shas[0] for s in shas), "gathered vector / coarse solve differ across ranks")
 
     # the whole V-cycle
-    host = G.HostMultigrid(ng, h, lambdas=glam)
+    host = G.HostMultigrid(ng, h, degree=degree, lo=lo, lambdas=glam, E=E, nu=nu)
     r = rng.standard_normal(n_global)
     zt = mg.apply(t(r[maps[0]]))
     z = zt.cpu().numpy()
@@ -180,7 +181,7 @@ def main():
     minv = op.jacobi()
     if rank == 0:
         minv[5] = float("nan")
-    bad = HexMultigrid(op, blk, minv=minv, blocks=blocks)
+    bad = HexMultigrid(op, blk, degree=degree, lo=lo, minv=minv, blocks=blocks)
     _, ib = op.solve(b, bad, 1e-8, 50)
     note(ib.flag == 2, f"NaN in rank 0's Minv: flag {ib.flag}")
     del bad
@@ -219,13 +220,13 @@ def main():
     note(status == 0, f"communicator status {status}")
     xs = allg((maps[0], base.cpu().numpy(), {"trace": i0.trace, "trace_total": i0.trace_total}, fails, stats, time.time() - t0))
     if rank == 0:
-        res = {"world": world, "pgrid": list(pgrid), "per": per, "kind": kind, "transport": transport,
+        res = {"world": world, "pgrid": list(pgrid), "per": per, "kind": kind, "degree": degree, "lo": lo, "E": E, "nu": nu, "transport": transport,
                "fails": [f for g in xs for f in g[3]], "stats": [g[4] for g in xs], "seconds": max(g[5] for g in xs)}
         res.update(trace_checks([g[2] for g in xs], transport, 1e-12, 200, n_global))
         xg = np.zeros(n_global)
         for m, v, *_ in xs:
             xg[m] = v
-        A = R.hex_box_csr(ng, (0, 0, 0), ng, h=h)
+        A = R.hex_box_csr(ng, (0, 0, 0), ng, E=E, nu=nu, h=h)
         bh = bg.cpu().numpy()
         ref = R.ref_pcg([R.CsrPart(A, bh)], [1.0 / A.diagonal()], 1e-11, 20000)
         res["x_vs_ref"] = float(np.linalg.norm(xg - ref["X"][0]) / np.linalg.norm(ref["X"][0]))

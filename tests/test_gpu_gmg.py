@@ -78,8 +78,8 @@ def test_coarse_solve(cuda):
 
 def test_coarse_limit_and_refusals_leak_nothing(cuda):
     """A coarsest level of 1536 dofs is built and solves, and destroying it gives back all device memory it took; the next
-    possible size (1539: dofs come in threes) is refused, as are a multi-rank solver, an odd ne, e0 != 0 and degree < 1 -
-    all before anything is allocated."""
+    possible size (1539: dofs come in threes) is refused, as are a multi-rank solver, an odd ne, e0 != 0, degree < 1 and lo
+    outside (0, 1.1) or NaN - all before anything is allocated."""
     import gc
     import torch
     from pcg_mpi_solver_b200 import _lib
@@ -122,6 +122,8 @@ def test_coarse_limit_and_refusals_leak_nothing(cuda):
     off = HexBlock((32, 16, 16), (16, 0, 0), (16, 16, 16), h=1.0 / 32)
     refused(off, SubdomainOperator(generate_matrix(off, device=cuda)))
     refused(blk, op, degree=0)
+    for lo in (0.0, 1.1, float("nan")):     # the Chebyshev interval [lo, 1.1] lambda must be non-empty and positive
+        refused(blk, op, lo=lo)
     # a solver with a communicator (one peer-only rank stands for a multi-rank solver)
     from pcg_mpi_solver_b200.solver import Communicator
     comm = Communicator(0, 1, None, device=cuda)

@@ -18,11 +18,12 @@ CASES = [((2, 1, 1), 8, "csr"), ((3, 1, 1), 8, "csr"), ((2, 2, 1), 8, "csr"), ((
          ((2, 1, 1), 16, "ebe_ordered"), ((2, 1, 1), 8, "ebe")]
 
 
-def _run(pgrid, per, kind, tmp_path, port, env):
+def _run(pgrid, per, kind, tmp_path, port, env, extra=()):
     world = pgrid[0] * pgrid[1] * pgrid[2]
     out = tmp_path / f"gmg_dd_{world}_{per}_{kind}.json"
     cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={world}", "--master-addr", "127.0.0.1",
-           "--master-port", str(port), os.path.join(HERE, "gmg_dd_worker.py"), str(out), ",".join(map(str, pgrid)), str(per), kind]
+           "--master-port", str(port), os.path.join(HERE, "gmg_dd_worker.py"), str(out), ",".join(map(str, pgrid)), str(per), kind,
+           *map(str, extra)]
     r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True, timeout=1200, env=dict(os.environ, **env))
     assert r.returncode == 0, r.stdout[-4000:]
     return json.loads(out.read_text())
@@ -44,6 +45,13 @@ def _check(res, transport):
 def test_ranks_sharing_one_gpu(cuda, tmp_path, pgrid, per, kind):
     port = 29711 + CASES.index((pgrid, per, kind))
     _check(_run(pgrid, per, kind, tmp_path, port, {"PCGB_SHARED_GPU": "1", "PCGB_EXPECT_TRANSPORT": "peer"}), "peer")
+
+
+def test_ranks_sharing_one_gpu_degree_3_and_a_stiff_nearly_incompressible_material(cuda, tmp_path):
+    """Degree 3 (two recurrence steps), lo = 0.1, E = 210, nu = 0.45 through every ranked and replicated level."""
+    res = _run((2, 1, 1), 8, "csr", tmp_path, 29721, {"PCGB_SHARED_GPU": "1", "PCGB_EXPECT_TRANSPORT": "peer"}, (3, 0.1, 210.0, 0.45))
+    assert (res["degree"], res["lo"], res["E"], res["nu"]) == (3, 0.1, 210.0, 0.45)
+    _check(res, "peer")
 
 
 @pytest.mark.parametrize("transport", ["peer", "nccl"])
