@@ -301,6 +301,16 @@ int64_t pcgb_hex_nrows(const pcgb_hex_box *box);
 int pcgb_hex_count(const pcgb_hex_box *box, int64_t *d_rowcount, void *stream);
 int pcgb_hex_fill(const pcgb_hex_box *box, const double *ke_host, double ck, const int64_t *d_rowptr,
                   int32_t *d_col, double *d_val, void *stream);
+/* The same rows and columns for a voxel model: element e of the box (e = (z * ne[1] + y) * ne[0] + x, x fastest, the
+ * element order of hexmesh.hex_type_group) has its own scale d_ck[e] (device, ne[0]*ne[1]*ne[2] doubles; Ck = E_e h),
+ * as every element of the reference's concrete model carries its own ElemList_Ck (partition_mesh.py:437-479).  Each
+ * 3x3 block is sum_e d_ck[e] Ke[la, lb] over the elements of pcgb_hex_fill, in the same order, summed from 0.0.
+ * PCGB_ERR_ARG (before the fill; the check synchronises `stream`): an entry of d_ck that is not finite and positive. */
+int pcgb_hex_fill_field(const pcgb_hex_box *box, const double *ke_host, const double *d_ck, const int64_t *d_rowptr,
+                        int32_t *d_col, double *d_val, void *stream);
+/* The same check of d_ck on its own (PCGB_ERR_ARG for an entry that is not finite and positive; synchronises `stream`), so
+ * a caller can refuse a field before it allocates the CSR arrays. */
+int pcgb_hex_field_check(const pcgb_hex_box *box, const double *d_ck, void *stream);
 
 /* ---------------------------------------------------------------- opt-in: geometric multigrid preconditioner (hex boxes)
  * z = M r is one symmetric V-cycle over nested hex boxes (across ranks: pcgb_mg_create_ranks below), for a one-rank solver whose operator (CSR, EBE or ordered EBE) is
@@ -363,6 +373,30 @@ int pcgb_solve_mg(pcgb_solver_t s, pcgb_mg_t mg, const double *d_b, const double
 int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos, pcgb_halo_t gather,
                          const double *const *d_own, const double *ke_host, double E, double h, const double *d_minv_fine,
                          int degree, double lo, pcgb_mg_t *out);
+/* The one-rank preconditioner for a voxel model (pcgb_hex_fill_field; the reference's per-element ElemList_Ck,
+ * partition_mesh.py:437-479): d_ck_fine holds the fine box's Ck per element in the order of pcgb_hex_fill_field, and
+ * the coarse matrices are Galerkin products instead of rediscretisations, which equal P^T A P only for a constant Ck.
+ * Coarse element (X,Y,Z) has children (2X+cx, 2Y+cy, 2Z+cz), c in {0,1}^3; Q_c is the 24x24 trilinear interpolation
+ * from its 8 corners onto child c's nodes (child node l at p = c + (l&1, l>>1&1, l>>2&1), weight from corner k
+ * prod_a phi_{k_a}(p_a), phi_0(p) = (2-p)/2, phi_1(p) = p/2, exact in binary).  Level 1: K_E = sum_c Q_c^T (Ck_c Ke) Q_c;
+ * level l+1: K_E = sum_c Q_c^T K_child(c) Q_c; each level is assembled from its element matrices like pcgb_hex_fill
+ * (same rows, columns and element order), clamped nodes dropped, which is P_free^T A P_free with the P of
+ * pcgb_mg_restrict / pcgb_mg_prolong_add.  Fixed summation order, no atomics: a repeated create is bit-identical.  The
+ * element matrices take 4608 bytes per coarse element and live on the device only while the next level is built
+ * (pcgb_mg_setup_info).  Smoothers, lambda, D^-1, the coarse Cholesky factor, pcgb_mg_apply and pcgb_solve_mg are
+ * those of pcgb_mg_create.  Refusals: those of pcgb_mg_create, and PCGB_ERR_ARG, before anything is allocated, for an
+ * entry of d_ck_fine that is not finite and positive (a device check, after a device synchronise, so d_ck_fine may come
+ * from any stream).  d_ck_fine is not read after create returns. */
+int pcgb_mg_create_field(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine,
+                         const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out);
+/* For tests: level `level`'s CSR (1 <= level < nlevels - 1, the smoothed coarse levels) into caller buffers: int64 row
+ * offsets (n + 1), int32 columns and values (nnz each).  With all three buffers NULL only *nnz is written.  Synchronises
+ * `stream`.  PCGB_ERR_ARG for level 0 (the solver's operator), the coarsest level (held as a dense factor) and the
+ * gathered level of a multi-rank handle. */
+int pcgb_mg_level_csr(pcgb_mg_t mg, int level, int64_t *d_rowptr, int32_t *d_col, double *d_val, int64_t *nnz, void *stream);
+/* Set-up costs of a field hierarchy (0 for the others): device time of the Galerkin kernels in ms, and the peak device
+ * bytes of element matrices held at once during create.  Either may be NULL. */
+int pcgb_mg_setup_info(pcgb_mg_t mg, double *galerkin_ms, int64_t *element_matrix_peak_bytes);
 /* la (-1 for a one-rank handle) and the dofs of its gathered global box; pcgb_mg_info lists levels 0 .. la, then the
  * replicated levels (lambda 0 for level la and the coarsest) */
 int pcgb_mg_info_ranks(pcgb_mg_t mg, int32_t *gather_level, int64_t *n_gathered);

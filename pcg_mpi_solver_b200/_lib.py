@@ -114,6 +114,9 @@ SIGNATURES = {
     "pcgb_mg_coarse_solve": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcgb_mg_create_ranks": (c_int, [c_void_p, POINTER(HexBox), c_int, POINTER(c_void_p), c_void_p, POINTER(c_void_p), POINTER(c_double),
                                      c_double, c_double, c_void_p, c_int, c_double, POINTER(c_void_p)]),
+    "pcgb_mg_create_field": (c_int, [c_void_p, POINTER(HexBox), POINTER(c_double), c_void_p, c_void_p, c_int, c_double, POINTER(c_void_p)]),
+    "pcgb_mg_level_csr": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
+    "pcgb_mg_setup_info": (c_int, [c_void_p, POINTER(c_double), POINTER(c_int64)]),
     "pcgb_mg_info_ranks": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int64)]),
     "pcgb_mg_gather": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcgb_mg_scatter": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
@@ -121,6 +124,8 @@ SIGNATURES = {
     "pcgb_hex_nrows": (c_int64, [POINTER(HexBox)]),
     "pcgb_hex_count": (c_int, [POINTER(HexBox), c_void_p, c_void_p]),
     "pcgb_hex_fill": (c_int, [POINTER(HexBox), POINTER(c_double), c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcgb_hex_field_check": (c_int, [POINTER(HexBox), c_void_p, c_void_p]),
+    "pcgb_hex_fill_field": (c_int, [POINTER(HexBox), POINTER(c_double), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -222,6 +222,53 @@ k_mg_rz(const int *__restrict__ skip, int64_t n, const double *__restrict__ r, c
   }
 }
 
+// Weight of coarse corner k in the trilinear interpolation onto local node l of child c of a coarse element: child-c
+// node l sits at p = c + (l&1, l>>1&1, l>>2&1) in {0,1,2}^3 (units of the fine spacing), and the weight is
+// prod_a phi_{k_a}(p_a) with phi_0(p) = (2 - p) / 2, phi_1(p) = p / 2: one of 0, 1/8, 1/4, 1/2, 1, exact in binary.
+__device__ __forceinline__ double mg_child_weight(int c, int l, int k) {
+  double w = 1.0;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const int p = ((c >> a) & 1) + ((l >> a) & 1);
+    w *= ((k >> a) & 1) ? 0.5 * p : 0.5 * (2 - p);
+  }
+  return w;
+}
+
+// Galerkin element matrices of a coarse level: K_E = sum_c Q_c^T K_c Q_c over the 8 children c = cx + 2 cy + 4 cz of
+// coarse element E = (X, Y, Z) (fine element (2X + cx, 2Y + cy, 2Z + cz)), Q_c the 24x24 interpolation of mg_child_weight
+// (block-diagonal over the 3 directions).  K_c = ck[child] * Ke (Ke in c_hex_ke) when kf is NULL (the first coarse
+// level, built from the fine field), else kf[576 child ..] (the level below's Galerkin matrices).  One CTA per coarse
+// element, one thread per entry (i, j): T = K_c Q_c in shared memory (l ascending), then (Q_c^T T)[i][j] (l ascending),
+// added to the entry in ascending c.  No atomics: a repeated set-up is bit-identical.  The result is written mirrored
+// from its upper triangle, so every element matrix, and every CSR assembled from them, is exactly symmetric.
+constexpr int kMgGalerkinThreads = 576;
+__global__ void __launch_bounds__(kMgGalerkinThreads)
+k_mg_galerkin(int cnx, int cny, int fnx, int fny, const double *__restrict__ ck, const double *__restrict__ kf, double *__restrict__ kc) {
+  __shared__ double K[576], T[576];
+  const int t = threadIdx.x, i = t / 24, j = t % 24;
+  const int64_t E = blockIdx.x;
+  const int X = (int)(E % cnx), Y = (int)((E / cnx) % cny), Z = (int)(E / ((int64_t)cnx * cny));
+  double acc = 0.0;
+  for (int c = 0; c < 8; ++c) {
+    const int64_t child = ((int64_t)(2 * Z + (c >> 2)) * fny + (2 * Y + ((c >> 1) & 1))) * fnx + (2 * X + (c & 1));
+    K[t] = kf ? kf[576 * child + t] : ck[child] * c_hex_ke[t];
+    __syncthreads();
+    double s = 0.0;
+#pragma unroll
+    for (int l = 0; l < 8; ++l) s += mg_child_weight(c, l, j / 3) * K[i * 24 + 3 * l + j % 3];
+    T[t] = s;
+    __syncthreads();
+    s = 0.0;
+#pragma unroll
+    for (int l = 0; l < 8; ++l) s += mg_child_weight(c, l, i / 3) * T[(3 * l + i % 3) * 24 + j];
+    acc += s;
+  }
+  K[t] = acc;   // every thread is past its last read of K (the second barrier of c = 7)
+  __syncthreads();
+  kc[576 * E + t] = i <= j ? K[t] : K[j * 24 + i];
+}
+
 // dense[i][col] = val of the coarsest level's CSR (dense zero-filled before)
 __global__ void k_mg_densify(int64_t n, const int64_t *__restrict__ rowptr, const int *__restrict__ col, const double *__restrict__ val,
                              double *__restrict__ dense) {

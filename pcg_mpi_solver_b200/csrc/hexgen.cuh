@@ -96,4 +96,69 @@ k_hex_fill(HexGeom g, double ck, const int64_t *__restrict__ rowptr, int *__rest
   }
 }
 
+// k_hex_fill for a heterogeneous box: the same rows, columns and element loop, but every element brings its own matrix.
+// kElemMat = false: element e = (oz * ny + oy) * nx + ox of the box contributes ck[e] * Ke (Ke in c_hex_ke; a voxel model
+// with one Young's modulus per element).  kElemMat = true: it contributes kel[576 e ..] (one row-major 24x24 matrix per
+// element; the Galerkin coarse levels of the multigrid).  Each block entry is summed from 0.0 over the elements in
+// (oz, oy, ox) ascending order.
+template <bool kElemMat>
+__global__ void __launch_bounds__(256)
+k_hex_fill_var(HexGeom g, const double *__restrict__ ck, const double *__restrict__ kel, const int64_t *__restrict__ rowptr,
+               int *__restrict__ col, double *__restrict__ val) {
+  const int64_t t = (blockIdx.x * (int64_t)blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (t >= g.nfree_nodes) return;
+  const int fx = (int)(t % g.nxf);
+  const int ly = (int)((t / g.nxf) % (g.ny + 1));
+  const int lz = (int)(t / ((int64_t)g.nxf * (g.ny + 1)));
+  const int lx = fx + g.x_lo;
+  const int dx = lane % 3 - 1, dy = (lane / 3) % 3 - 1, dz = lane / 9 - 1;
+  const int bx = lx + dx, by = ly + dy, bz = lz + dz;
+  const bool valid = lane < 27 && !(bx < g.x_lo || bx > g.nx || by < 0 || by > g.ny || bz < 0 || bz > g.nz);
+  const unsigned mask = __ballot_sync(0xffffffffu, valid);
+  if (!valid) return;
+  const int slot = __popc(mask & ((1u << lane) - 1u));
+  double blk[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+  const int ox0 = max(max(lx, bx) - 1, 0), ox1 = min(min(lx, bx), g.nx - 1);
+  const int oy0 = max(max(ly, by) - 1, 0), oy1 = min(min(ly, by), g.ny - 1);
+  const int oz0 = max(max(lz, bz) - 1, 0), oz1 = min(min(lz, bz), g.nz - 1);
+  for (int oz = oz0; oz <= oz1; ++oz)
+    for (int oy = oy0; oy <= oy1; ++oy)
+      for (int ox = ox0; ox <= ox1; ++ox) {
+        const int la = (lx - ox) + 2 * (ly - oy) + 4 * (lz - oz);
+        const int lb = (bx - ox) + 2 * (by - oy) + 4 * (bz - oz);
+        const int64_t e = ((int64_t)oz * g.ny + oy) * g.nx + ox;
+        if (kElemMat) {
+          const double *k = kel + 576 * e;
+#pragma unroll
+          for (int d = 0; d < 3; ++d)
+#pragma unroll
+            for (int c = 0; c < 3; ++c) blk[d * 3 + c] += k[(la * 3 + d) * 24 + lb * 3 + c];
+        } else {
+          const double s = ck[e];
+#pragma unroll
+          for (int d = 0; d < 3; ++d)
+#pragma unroll
+            for (int c = 0; c < 3; ++c) blk[d * 3 + c] += s * c_hex_ke[(la * 3 + d) * 24 + lb * 3 + c];
+        }
+      }
+  const int64_t bnode = ((int64_t)bz * (g.ny + 1) + by) * g.nxf + (bx - g.x_lo);
+#pragma unroll
+  for (int d = 0; d < 3; ++d) {
+    const int64_t base = rowptr[3 * t + d] + 3 * slot;
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      col[base + c] = (int)(3 * bnode + c);
+      val[base + c] = blk[d * 3 + c];
+    }
+  }
+}
+
+// *bad = 1 when some v[i] is not a finite positive number (a per-element Ck field)
+__global__ void k_field_check(int64_t n, const double *__restrict__ v, int *__restrict__ bad) {
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride)
+    if (!(v[i] > 0.0) || !isfinite(v[i])) *bad = 1;
+}
+
 }  // namespace pcgb

@@ -1022,6 +1022,12 @@ struct pcgb_mg_s {
   double *partials = nullptr, *red = nullptr, *h_red = nullptr;
   int *d_bad = nullptr;
   int64_t bytes = 0;
+  // field hierarchies (pcgb_mg_create_field): the fine per-element Ck, the Galerkin element matrices of the level being
+  // built (freed once the next level's exist), their peak device bytes and the device time of k_mg_galerkin
+  const double *ck_fine = nullptr;
+  double *kel = nullptr;
+  int64_t kel_peak = 0;
+  double galerkin_ms = 0.0;
 };
 
 namespace {
@@ -1577,7 +1583,7 @@ int pcgb_mg_destroy(pcgb_mg_t mg) {
     if (l > 0) { cudaFree(L.b); cudaFree(L.x); }
     cudaFree(L.r); cudaFree(L.d); cudaFree(L.q);
   }
-  cudaFree(mg->chol); cudaFree(mg->z); cudaFree(mg->partials); cudaFree(mg->red); cudaFree(mg->d_bad);
+  cudaFree(mg->chol); cudaFree(mg->z); cudaFree(mg->partials); cudaFree(mg->red); cudaFree(mg->d_bad); cudaFree(mg->kel);
   if (mg->h_red) cudaFreeHost(mg->h_red);
   delete mg;
   return PCGB_OK;
@@ -1585,8 +1591,9 @@ int pcgb_mg_destroy(pcgb_mg_t mg) {
 
 namespace {
 // Stiffness matrix of level L's box as device CSR (int64 row offsets; the caller frees them): k_hex_count, a host scan,
-// k_hex_fill with Ck = ck
-int mg_hex_csr(const HexGeom &g, const double *ke_host, double ck, int64_t **rp, int **col, double **val, int64_t *nnz) {
+// k_hex_fill with Ck = ck, or (kel != NULL) k_hex_fill_var from the level's per-element matrices
+int mg_hex_csr(const HexGeom &g, const double *ke_host, double ck, int64_t **rp, int **col, double **val, int64_t *nnz,
+               const double *kel = nullptr) {
   const int64_t n = 3 * g.nfree_nodes;
   std::vector<int64_t> cnt((size_t)n + 1);
   PCGB_CUDA(cudaMalloc(rp, (size_t)(n + 1) * sizeof(int64_t)));
@@ -1598,9 +1605,43 @@ int mg_hex_csr(const HexGeom &g, const double *ke_host, double ck, int64_t **rp,
   PCGB_CUDA(cudaMemcpy(*rp, cnt.data(), cnt.size() * sizeof(int64_t), cudaMemcpyHostToDevice));
   PCGB_CUDA(cudaMalloc(col, (size_t)*nnz * sizeof(int)));
   PCGB_CUDA(cudaMalloc(val, (size_t)*nnz * sizeof(double)));
-  PCGB_CUDA(cudaMemcpyToSymbol(c_hex_ke, ke_host, 24 * 24 * sizeof(double)));
-  k_hex_fill<<<(unsigned)((g.nfree_nodes * 32 + 255) / 256), 256>>>(g, ck, *rp, *col, *val);
+  if (kel) {
+    k_hex_fill_var<true><<<(unsigned)((g.nfree_nodes * 32 + 255) / 256), 256>>>(g, nullptr, kel, *rp, *col, *val);
+  } else {
+    PCGB_CUDA(cudaMemcpyToSymbol(c_hex_ke, ke_host, 24 * 24 * sizeof(double)));
+    k_hex_fill<<<(unsigned)((g.nfree_nodes * 32 + 255) / 256), 256>>>(g, ck, *rp, *col, *val);
+  }
   PCGB_CHECK_LAUNCH();
+  return PCGB_OK;
+}
+
+// Field hierarchies: the Galerkin element matrices of level l (l >= 1) from those of level l - 1 (level 1: from the fine
+// Ck field and Ke), into mg->kel; the level below's matrices are freed once these exist, so at most two levels' are held.
+int mg_galerkin_level(pcgb_mg_t mg, int l, const double *ke_host) {
+  const HexGeom &F = mg->lv[(size_t)l - 1].g, &C = mg->lv[(size_t)l].g;
+  const int64_t nce = (int64_t)C.nx * C.ny * C.nz;
+  const int64_t prev = l > 1 ? 576 * sizeof(double) * (int64_t)F.nx * F.ny * F.nz : 0;
+  double *kc = nullptr;
+  PCGB_CUDA(cudaMalloc(&kc, (size_t)nce * 576 * sizeof(double)));
+  mg->kel_peak = std::max(mg->kel_peak, prev + nce * 576 * (int64_t)sizeof(double));
+  if (l == 1) PCGB_CUDA(cudaMemcpyToSymbol(c_hex_ke, ke_host, 24 * 24 * sizeof(double)));
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  cudaEventCreate(&e0);
+  cudaEventCreate(&e1);
+  cudaEventRecord(e0, 0);
+  k_mg_galerkin<<<(unsigned)nce, kMgGalerkinThreads>>>(C.nx, C.ny, F.nx, F.ny, mg->ck_fine, l > 1 ? mg->kel : nullptr, kc);
+  const cudaError_t le = cudaGetLastError();
+  cudaEventRecord(e1, 0);
+  const cudaError_t se = cudaEventSynchronize(e1);
+  float ms = 0.0f;
+  if (le == cudaSuccess && se == cudaSuccess) cudaEventElapsedTime(&ms, e0, e1);
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  cudaFree(mg->kel);
+  mg->kel = kc;
+  if (le != cudaSuccess || se != cudaSuccess) return fail(PCGB_ERR_CUDA, "pcgb_mg_create_field: Galerkin kernel failed: %s",
+                                                          cudaGetErrorString(le != cudaSuccess ? le : se));
+  mg->galerkin_ms += ms;
   return PCGB_OK;
 }
 
@@ -1740,11 +1781,12 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
       PCGB_CUDA(cudaMemcpy(L.own, own[l], (size_t)L.n * sizeof(double), cudaMemcpyDeviceToDevice));
       if (l == mg->la) continue;   // gathered: no operator, no smoother
     }
+    if (mg->ck_fine && l > 0) PCGB_TRY(mg_galerkin_level(mg, l, ke_host));   // field: the level's Galerkin element matrices
     if (l == nlev - 1) {   // coarsest: dense Cholesky factor of its matrix
       int64_t *rp = nullptr, nnz = 0;
       int *col = nullptr;
       double *val = nullptr;
-      int rc = mg_hex_csr(L.g, ke_host, ck, &rp, &col, &val, &nnz);
+      int rc = mg_hex_csr(L.g, ke_host, ck, &rp, &col, &val, &nnz, mg->kel);
       mg->nc = (int)L.n;
       if (rc == PCGB_OK && alloc(&mg->chol, L.n * L.n) == cudaSuccess && cudaMemset(mg->chol, 0, (size_t)(L.n * L.n) * sizeof(double)) == cudaSuccess) {
         k_mg_densify<<<(unsigned)((L.n + 255) / 256), 256>>>(L.n, rp, col, val, mg->chol);
@@ -1755,6 +1797,8 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
       }
       cudaDeviceSynchronize();
       cudaFree(rp); cudaFree(col); cudaFree(val);
+      cudaFree(mg->kel);
+      mg->kel = nullptr;
       PCGB_TRY(rc);
       int bad = 0;
       PCGB_CUDA(cudaMemcpy(&bad, mg->d_bad, sizeof(int), cudaMemcpyDeviceToHost));
@@ -1766,7 +1810,7 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
     PCGB_CUDA(alloc(&L.q, L.n));
     if (l > 0) {
       int64_t *rp = nullptr, nnz = 0;
-      const int rc = mg_hex_csr(L.g, ke_host, ck, &rp, &L.col, &L.val, &nnz);
+      const int rc = mg_hex_csr(L.g, ke_host, ck, &rp, &L.col, &L.val, &nnz, mg->kel);
       L.rowptr = rp;
       PCGB_TRY(rc);
       mg->bytes += 12 * nnz + 8 * (L.n + 1);
@@ -1796,34 +1840,106 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
 }
 }  // namespace
 
-int pcgb_mg_create(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, const double *d_minv_fine,
-                   int degree, double lo, pcgb_mg_t *out) {
+namespace {
+// *bad = whether some of the n entries of d_v is not a finite positive number (synchronises `st`)
+int field_bad(int64_t n, const double *d_v, cudaStream_t st, const char *who, int *bad) {
+  int *d_flag = nullptr;
+  PCGB_CUDA(cudaMalloc(&d_flag, sizeof(int)));
+  cudaMemsetAsync(d_flag, 0, sizeof(int), st);
+  k_field_check<<<(unsigned)std::max<int64_t>(1, std::min<int64_t>((n + 255) / 256, 4096)), 256, 0, st>>>(n, d_v, d_flag);
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaMemcpyAsync(bad, d_flag, sizeof(int), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+  cudaFree(d_flag);
+  return e == cudaSuccess ? PCGB_OK : fail(PCGB_ERR_CUDA, "%s: field check failed: %s", who, cudaGetErrorString(e));
+}
+
+// pcgb_mg_create (d_ck_fine NULL: Ck = E 2^l h on level l) and pcgb_mg_create_field (Galerkin levels from d_ck_fine)
+int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, const double *d_ck_fine,
+                  const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out, const char *who) {
   PCGB_TRY(require_device());
-  if (!s || !box || !ke_host || !d_minv_fine || !out) return fail(PCGB_ERR_ARG, "pcgb_mg_create: null argument");
-  if (s->halo || s->comm) return fail(PCGB_ERR_ARG, "pcgb_mg_create: one rank only (the solver has a halo plan or a communicator)");
+  if (!s || !box || !ke_host || !d_minv_fine || !out) return fail(PCGB_ERR_ARG, "%s: null argument", who);
+  if (s->halo || s->comm) return fail(PCGB_ERR_ARG, "%s: one rank only (the solver has a halo plan or a communicator)", who);
   if (degree < 1 || !(lo > 0.0 && lo < 1.1) || !(E > 0.0) || !(h > 0.0))
-    return fail(PCGB_ERR_ARG, "pcgb_mg_create: degree >= 1, 0 < lo < 1.1, E > 0 and h > 0 required");
+    return fail(PCGB_ERR_ARG, "%s: degree >= 1, 0 < lo < 1.1, E > 0 and h > 0 required", who);
   for (int a = 0; a < 3; ++a)
     if (box->e0[a] != 0 || box->ng[a] != box->ne[a] || box->ne[a] <= 0)
-      return fail(PCGB_ERR_ARG, "pcgb_mg_create: the box must be the whole mesh (e0 = 0, ng = ne)");
+      return fail(PCGB_ERR_ARG, "%s: the box must be the whole mesh (e0 = 0, ng = ne)", who);
   std::vector<HexGeom> geo{hex_geom(box)};
-  if (3 * geo[0].nfree_nodes != s->n) return fail(PCGB_ERR_ARG, "pcgb_mg_create: the solver's operator has %lld rows, the box %lld",
-                                                  (long long)s->n, (long long)(3 * geo[0].nfree_nodes));
+  if (3 * geo[0].nfree_nodes != s->n) return fail(PCGB_ERR_ARG, "%s: the solver's operator has %lld rows, the box %lld",
+                                                  who, (long long)s->n, (long long)(3 * geo[0].nfree_nodes));
   mg_whole_box_levels(geo);
-  if (geo.size() < 2) return fail(PCGB_ERR_ARG, "pcgb_mg_create: the box does not coarsen (every ne must be even and >= 4)");
+  if (geo.size() < 2) return fail(PCGB_ERR_ARG, "%s: the box does not coarsen (every ne must be even and >= 4)", who);
   if (3 * geo.back().nfree_nodes > kMgMaxCoarse)
-    return fail(PCGB_ERR_ARG, "pcgb_mg_create: the coarsest level has %lld dofs (at most %d)", (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
-  if (geo.size() > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "pcgb_mg_create: more than %d levels", PCGB_MG_MAX_LEVELS);
+    return fail(PCGB_ERR_ARG, "%s: the coarsest level has %lld dofs (at most %d)", who, (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
+  if (geo.size() > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "%s: more than %d levels", who, PCGB_MG_MAX_LEVELS);
+  if (d_ck_fine) {
+    // the check runs on the legacy stream, which does not wait for non-blocking streams: finish whatever work of the caller
+    // may still be writing d_ck_fine first
+    PCGB_CUDA(cudaDeviceSynchronize());
+    int bad = 0;
+    PCGB_TRY(field_bad((int64_t)geo[0].nx * geo[0].ny * geo[0].nz, d_ck_fine, 0, who, &bad));
+    if (bad) return fail(PCGB_ERR_ARG, "%s: every Ck of the field must be finite and positive", who);
+  }
   pcgb_mg_t mg = new pcgb_mg_s();
-  mg->s = s; mg->degree = degree; mg->lo = lo;
+  mg->s = s; mg->degree = degree; mg->lo = lo; mg->ck_fine = d_ck_fine;
   mg->lv.resize(geo.size());
   for (size_t l = 0; l < geo.size(); ++l) {
     MgLevel &L = mg->lv[l];
     L.g = geo[l]; L.glev = (int)l; L.place = MgPlace{geo[l], 0, 0, 0};
   }
   const int rc = mg_build(mg, ke_host, E, h, d_minv_fine, nullptr);
+  mg->ck_fine = nullptr;   // the caller's array: not read after create
   if (rc != PCGB_OK) { pcgb_mg_destroy(mg); return rc; }
   *out = mg;
+  return PCGB_OK;
+}
+}  // namespace
+
+int pcgb_mg_create(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, const double *d_minv_fine,
+                   int degree, double lo, pcgb_mg_t *out) {
+  return mg_create_one(s, box, ke_host, E, h, nullptr, d_minv_fine, degree, lo, out, "pcgb_mg_create");
+}
+
+int pcgb_mg_create_field(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine,
+                         const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
+  if (!d_ck_fine) {
+    PCGB_TRY(require_device());
+    return fail(PCGB_ERR_ARG, "pcgb_mg_create_field: null argument");
+  }
+  return mg_create_one(s, box, ke_host, 1.0, 1.0, d_ck_fine, d_minv_fine, degree, lo, out, "pcgb_mg_create_field");
+}
+
+int pcgb_mg_level_csr(pcgb_mg_t mg, int level, int64_t *d_rowptr, int32_t *d_col, double *d_val, int64_t *nnz, void *stream) {
+  PCGB_TRY(require_device());
+  if (!mg || !nnz) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: null argument");
+  if (level <= 0 || level + 1 >= (int)mg->lv.size() || level == mg->la)
+    return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: level %d has no coarse CSR (levels 1 .. %d, not the gathered one)", level,
+                (int)mg->lv.size() - 2);
+  const MgLevel &L = mg->lv[(size_t)level];
+  *nnz = L.P.nnz;
+  if (!d_rowptr && !d_col && !d_val) return PCGB_OK;
+  if (!d_rowptr || !d_col || !d_val) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: give all three buffers or none");
+  const cudaStream_t st = (cudaStream_t)stream;
+  std::vector<int64_t> r64((size_t)L.n + 1);
+  if (L.P.rp64) {
+    PCGB_CUDA(cudaMemcpy(r64.data(), L.rowptr, r64.size() * sizeof(int64_t), cudaMemcpyDeviceToHost));
+  } else {
+    std::vector<int32_t> r32(r64.size());
+    PCGB_CUDA(cudaMemcpy(r32.data(), L.rowptr, r32.size() * sizeof(int32_t), cudaMemcpyDeviceToHost));
+    std::copy(r32.begin(), r32.end(), r64.begin());
+  }
+  PCGB_CUDA(cudaMemcpyAsync(d_rowptr, r64.data(), r64.size() * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  PCGB_CUDA(cudaMemcpyAsync(d_col, L.col, (size_t)L.P.nnz * sizeof(int32_t), cudaMemcpyDeviceToDevice, st));
+  PCGB_CUDA(cudaMemcpyAsync(d_val, L.val, (size_t)L.P.nnz * sizeof(double), cudaMemcpyDeviceToDevice, st));
+  PCGB_CUDA(cudaStreamSynchronize(st));
+  return PCGB_OK;
+}
+
+int pcgb_mg_setup_info(pcgb_mg_t mg, double *galerkin_ms, int64_t *element_matrix_peak_bytes) {
+  if (!mg) return fail(PCGB_ERR_ARG, "pcgb_mg_setup_info: null argument");
+  if (galerkin_ms) *galerkin_ms = mg->galerkin_ms;
+  if (element_matrix_peak_bytes) *element_matrix_peak_bytes = mg->kel_peak;
   return PCGB_OK;
 }
 
@@ -2007,6 +2123,33 @@ int pcgb_hex_fill(const pcgb_hex_box *box, const double *ke_host, double ck, con
   PCGB_CUDA(cudaMemcpyToSymbolAsync(c_hex_ke, ke_host, 24 * 24 * sizeof(double), 0, cudaMemcpyHostToDevice, (cudaStream_t)stream));
   const int64_t threads = g.nfree_nodes * 32;
   k_hex_fill<<<(unsigned)((threads + 255) / 256), 256, 0, (cudaStream_t)stream>>>(g, ck, d_rowptr, d_col, d_val);
+  PCGB_CHECK_LAUNCH();
+  return PCGB_OK;
+}
+
+int pcgb_hex_field_check(const pcgb_hex_box *box, const double *d_ck, void *stream) {
+  if (!box || !d_ck) return fail(PCGB_ERR_ARG, "pcgb_hex_field_check: null argument");
+  PCGB_TRY(require_device());
+  HexGeom g = hex_geom(box);
+  if (g.nx <= 0 || g.ny <= 0 || g.nz <= 0) return fail(PCGB_ERR_ARG, "pcgb_hex_field_check: empty box");
+  int bad = 0;
+  PCGB_TRY(field_bad((int64_t)g.nx * g.ny * g.nz, d_ck, (cudaStream_t)stream, "pcgb_hex_field_check", &bad));
+  return bad ? fail(PCGB_ERR_ARG, "pcgb_hex_field_check: every Ck of the field must be finite and positive") : PCGB_OK;
+}
+
+int pcgb_hex_fill_field(const pcgb_hex_box *box, const double *ke_host, const double *d_ck, const int64_t *d_rowptr, int32_t *d_col,
+                        double *d_val, void *stream) {
+  if (!box || !ke_host || !d_ck || !d_rowptr || !d_col || !d_val) return fail(PCGB_ERR_ARG, "pcgb_hex_fill_field: null argument");
+  PCGB_TRY(require_device());
+  HexGeom g = hex_geom(box);
+  if (g.nx <= 0 || g.ny <= 0 || g.nz <= 0 || g.nfree_nodes <= 0) return fail(PCGB_ERR_ARG, "pcgb_hex_fill_field: empty box");
+  const cudaStream_t st = (cudaStream_t)stream;
+  int bad = 0;
+  PCGB_TRY(field_bad((int64_t)g.nx * g.ny * g.nz, d_ck, st, "pcgb_hex_fill_field", &bad));
+  if (bad) return fail(PCGB_ERR_ARG, "pcgb_hex_fill_field: every Ck of the field must be finite and positive");
+  PCGB_CUDA(cudaMemcpyToSymbolAsync(c_hex_ke, ke_host, 24 * 24 * sizeof(double), 0, cudaMemcpyHostToDevice, st));
+  const int64_t threads = g.nfree_nodes * 32;
+  k_hex_fill_var<false><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(g, d_ck, nullptr, d_rowptr, d_col, d_val);
   PCGB_CHECK_LAUNCH();
   return PCGB_OK;
 }

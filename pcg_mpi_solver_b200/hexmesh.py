@@ -105,13 +105,54 @@ class HexBlock:
         return [(self.e0[a], self.e0[a] + self.ne[a]) for a in range(3)]
 
 
-def generate_matrix(block: HexBlock, device="cuda") -> CsrMatrix:
-    """Sub-assembled K_i[Eff,Eff] of the box, generated on the device."""
+def _same_device(a, b) -> bool:
+    """torch devices a and b are one device ('cuda' stands for the current CUDA device)."""
+    a, b = torch.device(a), torch.device(b)
+    if a.type == "cuda" and a.index is None:
+        a = torch.device("cuda", torch.cuda.current_device())
+    if b.type == "cuda" and b.index is None:
+        b = torch.device("cuda", torch.cuda.current_device())
+    return a == b
+
+
+def check_field(E_field, block: HexBlock, device=None) -> np.ndarray | torch.Tensor:
+    """A per-element Young's modulus of `block`: float64, shape (ne[2], ne[1], ne[0]) (x fastest in memory), a numpy array,
+    a CPU tensor or a tensor on `device` (device None: a tensor on any device).  Raises ValueError otherwise.  Its values
+    (finite, positive) are checked on the device by the kernels that read it."""
+    shape = tuple(int(v) for v in reversed(block.ne))
+    if isinstance(E_field, torch.Tensor):
+        if E_field.dtype != torch.float64:
+            raise ValueError(f"E_field: float64 required, got {E_field.dtype}")
+        if device is not None and E_field.device.type != "cpu" and not _same_device(E_field.device, device):
+            raise ValueError(f"E_field: on {E_field.device}, expected the CPU or {device}")
+    elif isinstance(E_field, np.ndarray):
+        if E_field.dtype != np.float64:
+            raise ValueError(f"E_field: float64 required, got {E_field.dtype}")
+    else:
+        raise ValueError("E_field: a numpy array or a torch tensor required")
+    if tuple(E_field.shape) != shape:
+        raise ValueError(f"E_field: shape {tuple(E_field.shape)}, the box has {shape} elements (ne[2], ne[1], ne[0])")
+    return E_field
+
+
+def field_ck(E_field, block: HexBlock, device) -> torch.Tensor:
+    """Ck = E_e * h per element of the box, as a contiguous float64 device vector in element order."""
+    check_field(E_field, block, device)
+    t = torch.from_numpy(E_field) if isinstance(E_field, np.ndarray) else E_field
+    return (t.reshape(-1).to(device, torch.float64) * float(block.h)).contiguous()
+
+
+def generate_matrix(block: HexBlock, device="cuda", E_field=None) -> CsrMatrix:
+    """Sub-assembled K_i[Eff,Eff] of the box, generated on the device.  E_field: one Young's modulus per element of the box
+    (shape (ne[2], ne[1], ne[0]), float64; see block_field), replacing block.E: a voxel model (pcgb_hex_fill_field)."""
     lib = _lib.load()
     box = block.cbox()
     n = int(lib.pcgb_hex_nrows(ctypes.byref(box)))
     assert n == block.n
+    ck = None if E_field is None else field_ck(E_field, block, device)
     with torch.cuda.device(device):
+        if ck is not None:   # refuse a bad field before the CSR arrays are allocated
+            _lib.check(lib.pcgb_hex_field_check(ctypes.byref(box), _lib.ptr(ck), _lib.stream_ptr()), "pcgb_hex_field_check")
         counts = torch.empty(n + 1, dtype=torch.int64, device=device)
         _lib.check(lib.pcgb_hex_count(ctypes.byref(box), _lib.ptr(counts), _lib.stream_ptr()), "pcgb_hex_count")
         rowptr = torch.cumsum(counts, 0)  # plumbing: inclusive scan of the per-row counts
@@ -120,18 +161,25 @@ def generate_matrix(block: HexBlock, device="cuda") -> CsrMatrix:
         col = torch.empty(nnz, dtype=torch.int32, device=device)
         val = torch.empty(nnz, dtype=torch.float64, device=device)
         ke = np.ascontiguousarray(hex_element_stiffness(1.0, block.nu))
-        _lib.check(lib.pcgb_hex_fill(ctypes.byref(box), ke.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
-                                     float(block.E * block.h), _lib.ptr(rowptr), _lib.ptr(col), _lib.ptr(val),
-                                     _lib.stream_ptr()), "pcgb_hex_fill")
+        if ck is None:
+            _lib.check(lib.pcgb_hex_fill(ctypes.byref(box), ke.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
+                                         float(block.E * block.h), _lib.ptr(rowptr), _lib.ptr(col), _lib.ptr(val),
+                                         _lib.stream_ptr()), "pcgb_hex_fill")
+        else:
+            _lib.check(lib.pcgb_hex_fill_field(ctypes.byref(box), ke.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
+                                               _lib.ptr(ck), _lib.ptr(rowptr), _lib.ptr(col), _lib.ptr(val),
+                                               _lib.stream_ptr()), "pcgb_hex_fill_field")
         torch.cuda.current_stream().synchronize()
         if nnz < 2**31:
             rowptr = rowptr.to(torch.int32)
     return CsrMatrix(rowptr, col, val, (n, n))
 
 
-def hex_type_group(block: HexBlock):
+def hex_type_group(block: HexBlock, E_field=None, device=None):
     """The box as the reference would hold it: ONE pattern type group (the Q1 hexahedron, no sign flips,
     Ck = E*h; partition_mesh.py:443-491) in the local all-dof numbering 3*node + dir (x fastest), plus LocDofEff.
+    E_field (shape (ne[2], ne[1], ne[0])): Ck = E_field * h per element instead (a tensor on the CPU or on `device`; any
+    device when `device` is None).
     Returns (TypeGroup, loc_dof_eff, ndof)."""
     from .partition import TypeGroup
     nx, ny, nz = block.ne
@@ -145,27 +193,42 @@ def hex_type_group(block: HexBlock):
     lz, ly, lx = np.meshgrid(np.arange(nz + 1), np.arange(ny + 1), np.arange(nx + 1), indexing="ij")
     free_nodes = np.nonzero(lx.ravel() >= block.x_lo)[0]     # ascending -> the free numbering of generate_matrix
     eff = (3 * free_nodes[:, None] + np.arange(3)[None, :]).ravel()
-    grp = TypeGroup(0, dofs, np.zeros(dofs.shape, dtype=bool), np.full(ex.size, block.E * block.h), hex_element_stiffness(1.0, block.nu), None)
+    if E_field is None:
+        ck = np.full(ex.size, block.E * block.h)
+    else:
+        check_field(E_field, block, device)
+        f = E_field.detach().cpu().numpy() if isinstance(E_field, torch.Tensor) else E_field
+        ck = np.ascontiguousarray(f, dtype=np.float64).reshape(-1) * block.h
+    grp = TypeGroup(0, dofs, np.zeros(dofs.shape, dtype=bool), ck, hex_element_stiffness(1.0, block.nu), None)
     return grp, eff, 3 * (nx + 1) * (ny + 1) * (nz + 1)
 
 
-def generate_ebe(block: HexBlock, device="cuda", ordered: bool = False):
+def generate_ebe(block: HexBlock, device="cuda", ordered: bool = False, E_field=None):
     """The same box as a matrix-free EBE operator (ebe.EbeMatrix); opt-in companion of generate_matrix (SURVEY 8(f1)).
-    ordered=True builds ebe.EbeMatrixOrdered, the bit-reproducible variant with a fixed summation order."""
+    ordered=True builds ebe.EbeMatrixOrdered, the bit-reproducible variant with a fixed summation order.  E_field: as in
+    generate_matrix."""
     from .ebe import EbeMatrix, EbeMatrixOrdered
-    grp, eff, ndof = hex_type_group(block)
+    grp, eff, ndof = hex_type_group(block, E_field, device)
     return (EbeMatrixOrdered if ordered else EbeMatrix)([grp], eff, ndof, device=device)
 
 
-def hex_mdf_model(ng, E: float = 1.0, nu: float = 0.3, h: float | None = None, traction: float = 1.0):
+def hex_mdf_model(ng, E: float = 1.0, nu: float = 0.3, h: float | None = None, traction: float = 1.0, E_field=None):
     """The structured hex problem as an in-memory `MdfModel` (the reference's model-definition schema, SURVEY
     Appendix A) so that the general pipeline - `partition_mesh(model, nparts)` with METIS, the subdomain builder,
     device assembly / EBE - can run on it (config C3: the 128^3 mesh partitioned 8-way by METIS).
-    Global numbering: node = (gz*(ny+1)+gy)*(nx+1)+gx, dof = 3*node+dir; one pattern type (the Q1 hexahedron)."""
+    Global numbering: node = (gz*(ny+1)+gy)*(nx+1)+gx, dof = 3*node+dir; one pattern type (the Q1 hexahedron).
+    E_field (shape (ng[2], ng[1], ng[0])): one Young's modulus per element, Ck = E_field * h in element order, as the
+    reference's concrete model carries one ElemList_Ck per element."""
     from .model import MdfModel
     nx, ny, nz = ng
     h = 1.0 / nx if h is None else h
     ne = nx * ny * nz
+    if E_field is None:
+        ck = np.full(ne, E * h)
+    else:
+        check_field(E_field, HexBlock(tuple(ng), (0, 0, 0), tuple(ng)))
+        f = E_field.detach().cpu().numpy() if isinstance(E_field, torch.Tensor) else E_field
+        ck = np.ascontiguousarray(f, dtype=np.float64).reshape(-1) * h
     ez, ey, ex = np.meshgrid(np.arange(nz), np.arange(ny), np.arange(nx), indexing="ij")
     ex, ey, ez = ex.ravel(), ey.ravel(), ez.ravel()
     nodes = np.empty((ne, 8), dtype=np.int64)
@@ -191,7 +254,7 @@ def hex_mdf_model(ng, E: float = 1.0, nu: float = 0.3, h: float | None = None, t
                     node_flat=nodes.ravel().astype(np.int32), node_offset=offsets(8),
                     dof_flat=dofs.ravel().astype(np.int32), dof_offset=offsets(24),
                     sign_flat=np.zeros(ne * 24, dtype=bool), sign_offset=offsets(24),
-                    etype=np.zeros(ne, dtype=np.int32), ck=np.full(ne, E * h), F=F, Ud=np.zeros(ndof),
+                    etype=np.zeros(ne, dtype=np.int32), ck=ck, F=F, Ud=np.zeros(ndof),
                     dof_eff=eff.astype(np.int64), fixed_dof=fixed.astype(np.int64), ke=[hex_element_stiffness(1.0, nu)], dt=0.0)
 
 
@@ -210,6 +273,46 @@ def load_vector(block: HexBlock, traction: float = 1.0, device="cuda") -> torch.
     node = block.free_index_of_global_nodes(torch.full_like(GY, x1), GY, GZ)
     b[3 * node.reshape(-1) + 2] = (-traction * block.h * block.h * (cz[:, None] * cy[None, :])).reshape(-1)
     return b
+
+
+def block_field(global_field, block: HexBlock):
+    """The box's slice of a field of the whole mesh (shape (ng[2], ng[1], ng[0])): what generate_matrix / generate_ebe take
+    as E_field for that box, so every rank builds its own operator without communication."""
+    ng = tuple(int(v) for v in reversed(block.ng))
+    if tuple(global_field.shape) != ng:
+        raise ValueError(f"block_field: the field has shape {tuple(global_field.shape)}, the mesh {ng}")
+    (x0, x1), (y0, y1), (z0, z1) = block.node_ranges()
+    out = global_field[z0:z1, y0:y1, x0:x1]
+    return out.contiguous() if isinstance(out, torch.Tensor) else np.ascontiguousarray(out)
+
+
+def inclusion_field(ng, fraction: float = 0.4, radii=(2.0, 6.0), E_matrix: float = 1.0, E_inclusion: float = 10.0,
+                    seed: int = 0) -> np.ndarray:
+    """A two-phase voxel field of spherical inclusions in a matrix (a synthetic stand-in for aggregate in mortar), shape
+    (ng[2], ng[1], ng[0]), float64, values E_matrix and E_inclusion only.  Spheres with centres uniform in the box and
+    radii uniform in `radii` (element edges) are drawn from numpy's default_rng(seed) one by one; an element (centre at
+    i + 1/2) inside one becomes inclusion; drawing stops once the inclusion fraction reaches `fraction`, so it overshoots
+    by at most one sphere.  Deterministic: equal arguments give identical bytes."""
+    nx, ny, nz = (int(v) for v in ng)
+    if not 0.0 <= fraction < 1.0 or not (0 < radii[0] <= radii[1]):
+        raise ValueError("inclusion_field: 0 <= fraction < 1 and 0 < radii[0] <= radii[1] required")
+    rng = np.random.default_rng(seed)
+    inc = np.zeros((nz, ny, nx), dtype=bool)
+    target = fraction * inc.size
+    count = 0
+    while count < target:
+        c = rng.uniform(0.0, 1.0, 3) * (nx, ny, nz)
+        r = rng.uniform(radii[0], radii[1])
+        lo = [max(int(np.floor(c[a] - r)), 0) for a in range(3)]
+        hi = [min(int(np.ceil(c[a] + r)) + 1, (nx, ny, nz)[a]) for a in range(3)]
+        if any(lo[a] >= hi[a] for a in range(3)):
+            continue
+        z, y, x = np.meshgrid(np.arange(lo[2], hi[2]) + 0.5, np.arange(lo[1], hi[1]) + 0.5, np.arange(lo[0], hi[0]) + 0.5, indexing="ij")
+        inside = (x - c[0]) ** 2 + (y - c[1]) ** 2 + (z - c[2]) ** 2 <= r * r
+        sub = inc[lo[2]:hi[2], lo[1]:hi[1], lo[0]:hi[0]]
+        count += int(np.count_nonzero(inside & ~sub))
+        sub |= inside
+    return np.where(inc, float(E_inclusion), float(E_matrix))
 
 
 def block_grid(nranks: int):

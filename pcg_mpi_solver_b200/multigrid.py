@@ -20,7 +20,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .hexmesh import HexBlock, hex_element_stiffness, interface_lists
+from .hexmesh import HexBlock, field_ck, hex_element_stiffness, interface_lists
 
 MAX_GATHERED = 1 << 17    # dofs of the largest global box gathered onto every rank (kMgMaxGathered)
 MAX_COARSE = 1536         # dofs of the largest coarsest level (kMgMaxCoarse)
@@ -73,9 +73,14 @@ class HexMultigrid:
 
     One rank: block is the whole mesh (e0 = 0, ng = ne, every ne even).  Across ranks (op.comm with 2 or more ranks):
     blocks lists every rank's box and block is blocks[op.comm.rank]; construction is collective and refuses (ValueError,
-    on every rank alike, before anything is allocated) what `rank_levels` refuses."""
+    on every rank alike, before anything is allocated) what `rank_levels` refuses.
 
-    def __init__(self, op, block: HexBlock, degree: int = 2, lo: float = 0.25, minv: torch.Tensor | None = None, blocks=None):
+    E_field (one rank only): the per-element Young's modulus `op` was generated with (hexmesh.generate_matrix / generate_ebe
+    with E_field; shape (ne[2], ne[1], ne[0]), float64).  The coarse levels are then Galerkin products of element matrices
+    (pcgb_mg_create_field) instead of rediscretisations with block.E.  With a multi-rank `op` it raises ValueError."""
+
+    def __init__(self, op, block: HexBlock, degree: int = 2, lo: float = 0.25, minv: torch.Tensor | None = None, blocks=None,
+                 E_field=None):
         self.op, self.block, self.degree, self.lo = op, block, int(degree), float(lo)
         self.n = op.n
         self.device = op.device
@@ -84,6 +89,19 @@ class HexMultigrid:
         self.levels = None
         comm = getattr(op, "comm", None)
         ranked = comm is not None and comm.nranks > 1
+        if E_field is not None:
+            if ranked:
+                raise ValueError("HexMultigrid: E_field is supported on one rank only")
+            ck = field_ck(E_field, block, self.device)
+            minv = op.jacobi() if minv is None else minv.to(self.device, torch.float64).contiguous()
+            ke = np.ascontiguousarray(hex_element_stiffness(1.0, block.nu))
+            box = block.cbox()
+            with torch.cuda.device(self.device):
+                torch.cuda.synchronize(self.device)
+                _lib.check(_lib.load().pcgb_mg_create_field(op._solver, ctypes.byref(box), ke.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
+                                                            _lib.ptr(ck), _lib.ptr(minv), self.degree, self.lo, ctypes.byref(self._h)),
+                           "pcgb_mg_create_field")
+            return
         if ranked:
             if blocks is None or len(blocks) != comm.nranks:
                 raise ValueError("HexMultigrid: a multi-rank operator needs `blocks`, one box per rank")
@@ -156,7 +174,28 @@ class HexMultigrid:
             out.update(gather_level=la.value, n_gathered=int(ng.value), global_lambda=lams[:la.value] + lams[la.value + 1:])
         return out
 
+    def setup_info(self) -> dict:
+        """galerkin_ms (device time of the Galerkin kernels) and element_matrix_peak_bytes (element matrices held at once
+        during the set-up); both 0 without E_field."""
+        ms, peak = ctypes.c_double(), ctypes.c_int64()
+        _lib.check(_lib.load().pcgb_mg_setup_info(self._h, ctypes.byref(ms), ctypes.byref(peak)), "pcgb_mg_setup_info")
+        return {"galerkin_ms": float(ms.value), "element_matrix_peak_bytes": int(peak.value)}
+
     # ---- the V-cycle's parts (tests; collective across ranks)
+    def level_matrix(self, level: int):
+        """The CSR of smoothed coarse level `level` (1 .. levels - 2) as (rowptr int64, col int32, val float64) device tensors."""
+        lib = _lib.load()
+        nnz = ctypes.c_int64()
+        _lib.check(lib.pcgb_mg_level_csr(self._h, level, None, None, None, ctypes.byref(nnz), None), "pcgb_mg_level_csr")
+        n = self.info()["n"][level]
+        rowptr = torch.empty(n + 1, dtype=torch.int64, device=self.device)
+        col = torch.empty(nnz.value, dtype=torch.int32, device=self.device)
+        val = torch.empty(nnz.value, dtype=torch.float64, device=self.device)
+        with torch.cuda.device(self.device):
+            _lib.check(lib.pcgb_mg_level_csr(self._h, level, _lib.ptr(rowptr), _lib.ptr(col), _lib.ptr(val), ctypes.byref(nnz),
+                                             _lib.stream_ptr()), "pcgb_mg_level_csr")
+        return rowptr, col, val
+
     def restrict(self, level: int, rf: torch.Tensor) -> torch.Tensor:
         rc = self._vec(self.info()["n"][level + 1])
         with torch.cuda.device(self.device):

@@ -1,0 +1,115 @@
+"""Time to solution of Jacobi-PCG against multigrid-preconditioned PCG on a voxel model: a hex box with one Young's modulus
+per element (hexmesh.inclusion_field: spherical inclusions of E_matrix * contrast in a matrix of E_matrix = 1).
+
+    python tools/voxel_bench.py --block 128 --contrast 10 [--fraction 0.4] [--operator csr|ebe_ordered|ebe] [--repeats 3]
+
+For each arm one JSON line: iterations, flag, the device time of the loop (CUDA events inside the solve) and the host wall
+time of the whole solve (ending in a device synchronise).  The multigrid arm adds its set-up wall time, the device time of
+its Galerkin kernels, the hierarchy's device bytes as the library counts them, the drop in free device memory across the
+set-up, the peak bytes of element matrices held during it, and the value-dictionary size of the fine matrix (CSR operator)
+and of every coarse level (0: more distinct 3x3 blocks than the dictionary holds, the plain node-block kernel).  Every line
+carries the card's name, power limit and SM clock.  Needs a GPU; there is no CPU path.
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+
+def card():
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader"],
+                             stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=30).stdout.strip().splitlines()
+        return out[0] if out else "unknown"
+    except Exception:
+        return "unknown"
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--block", type=int, default=128)
+    ap.add_argument("--contrast", type=float, default=10.0)
+    ap.add_argument("--fraction", type=float, default=0.4)
+    ap.add_argument("--radii", type=float, nargs=2, default=(2.0, 6.0))
+    ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--tol", type=float, default=1e-8)
+    ap.add_argument("--operator", choices=["csr", "ebe_ordered", "ebe"], default="csr")
+    ap.add_argument("--degree", type=int, default=2)
+    ap.add_argument("--repeats", type=int, default=3)
+    ap.add_argument("--jacobi-maxiter", type=int, default=50000)
+    a = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        sys.exit("voxel_bench: needs a CUDA device")
+    from pcg_mpi_solver_b200.csr import CsrMatrix
+    from pcg_mpi_solver_b200.hexmesh import HexBlock, generate_ebe, generate_matrix, inclusion_field, load_vector
+    from pcg_mpi_solver_b200.multigrid import HexMultigrid
+    from pcg_mpi_solver_b200.solver import SubdomainOperator
+    dev = torch.device("cuda:0")
+    B = a.block
+    blk = HexBlock((B, B, B), (0, 0, 0), (B, B, B), h=1.0 / B)
+    field = inclusion_field(blk.ng, a.fraction, tuple(a.radii), 1.0, a.contrast, a.seed)
+    if a.operator == "csr":
+        A = generate_matrix(blk, device=dev, E_field=field)
+        fine_dict = A.value_dict_blocks()
+    else:
+        A = generate_ebe(blk, device=dev, ordered=a.operator == "ebe_ordered", E_field=field)
+        fine_dict = None
+    op = SubdomainOperator(A)
+    b = load_vector(blk, device=dev)
+    minv = op.jacobi()
+    torch.cuda.synchronize()
+    torch.cuda.empty_cache()
+    free0, _ = torch.cuda.mem_get_info(dev)
+    t0 = time.perf_counter()
+    mg = HexMultigrid(op, blk, degree=a.degree, minv=minv, E_field=field)
+    torch.cuda.synchronize()
+    setup_s = time.perf_counter() - t0
+    free_drop = free0 - torch.cuda.mem_get_info(dev)[0]
+    info, sinfo = mg.info(), mg.setup_info()
+    level_dict = []
+    for l in range(1, info["levels"] - 1):
+        rp, col, val = mg.level_matrix(l)
+        M = CsrMatrix(rp, col, val, (info["n"][l], info["n"][l]))
+        level_dict.append(M.value_dict_blocks())
+        del M, rp, col, val
+    torch.cuda.empty_cache()
+
+    def run(M, maxiter):
+        op.solve(b, M, a.tol, maxiter)                          # warm-up (graph capture, module loads)
+        best = None
+        for _ in range(a.repeats):
+            torch.cuda.synchronize()
+            t = time.perf_counter()
+            x, si = op.solve(b, M, a.tol, maxiter)
+            torch.cuda.synchronize()
+            wall = time.perf_counter() - t
+            if best is None or wall < best[0]:
+                best = (wall, si, x)
+        return best
+
+    wj, ij, xj = run(minv, a.jacobi_maxiter)
+    wm, im, xm = run(mg, 1000)
+    common = {"block": B, "operator": a.operator, "contrast": a.contrast, "fraction": a.fraction,
+              "inclusion_fraction": round(float((field != 1.0).mean()), 4), "tol": a.tol, "card": card()}
+    print(json.dumps({**common, "arm": "jacobi", "flag": ij.flag, "iters": ij.iters, "loop_ms": round(ij.loop_ms, 3),
+                      "wall_s": round(wj, 4), "ms_per_iter": round(ij.loop_ms / max(ij.loop_iters, 1), 4),
+                      "fine_value_dict_blocks": fine_dict}))
+    print(json.dumps({**common, "arm": "multigrid", "flag": im.flag, "iters": im.iters, "loop_ms": round(im.loop_ms, 3),
+                      "wall_s": round(wm, 4), "ms_per_iter": round(im.loop_ms / max(im.loop_iters, 1), 4),
+                      "setup_s": round(setup_s, 3), "galerkin_ms": round(sinfo["galerkin_ms"], 3),
+                      "element_matrix_peak_bytes": sinfo["element_matrix_peak_bytes"], "degree": a.degree,
+                      "levels": info["levels"], "n_levels": info["n"], "lambda": [round(v, 4) for v in info["lambda"]],
+                      "hierarchy_bytes": info["bytes"], "device_free_drop_bytes": free_drop,
+                      "fine_value_dict_blocks": fine_dict, "level_value_dict_blocks": level_dict,
+                      "speedup_wall": round(wj / wm, 2), "speedup_wall_with_setup": round(wj / (wm + setup_s), 2),
+                      "x_rel_diff_vs_jacobi": float((xm - xj).norm() / xj.norm())}))
+
+
+if __name__ == "__main__":
+    main()
