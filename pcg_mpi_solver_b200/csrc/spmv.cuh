@@ -85,6 +85,7 @@ struct CsrPlan {
   int vd = 0;                      // distinct blocks D (0: no dictionary, the kernel streams val)
   uint16_t *bvid = nullptr;        // [nnz/9 + 16]  dictionary id of the block at bidx's position
   double *vdict = nullptr;         // [vd * 9]      the blocks, row-major
+  int bsr_group = 0;               // tiles a CTA consumes between two barriers (k_spmv_bsr3_vd: one warp per tile)
   // interface-first split (multi-GPU overlap): tiles that own an interface row are listed first in desc_split
   struct TileDesc *desc_split = nullptr;  // [ntiles] permutation of tile_desc
   int nb_tiles = 0;                       // leading boundary tiles of desc_split
@@ -784,26 +785,155 @@ k_spmv_persist(const RP *__restrict__ rowptr, const uint16_t *__restrict__ lidx,
   }
 }
 
-// ------------------------------------------------------------------ node-block ("BSR-3") persistent kernel
-// Same tiles, x windows, TMA / mbarrier ring and producer warps as k_spmv_persist; the CONSUMER differs: the tile is a
-// whole number of nodes (3 rows with one column pattern of aligned triples) and is processed as a flat list of 3x3 blocks,
-// one block per consumer thread per pass:
+// ------------------------------------------------------------------ node-block ("BSR-3") persistent kernels
+// Same tiles, x windows, TMA / mbarrier ring and producer warps as k_spmv_persist; the tile is a whole number of nodes
+// (3 rows with one column pattern of aligned triples).  Two consumers, one per plan kind, share the producer and the
+// 3x3 block product, and sum every row in the same order - partials of the node's blocks in block order, from 0.0 - so
+// that y and x.y are the same bits whichever one runs:
+//   k_spmv_bsr3     streams the values; the tile is a flat list of 3x3 blocks, one block per consumer thread per pass:
 //     phase 1   thread b: node i by binary search in the node offsets, ONE 16-bit staged position -> x triple (3 LDS),
 //               9 values at stride 3 doubles across the lanes (conflict-free), 9 FMAs -> 3 row partials to shared memory;
 //     phase 2   (after one named barrier, scratch double-buffered by tile parity) thread r < R adds the partials of its
 //               row in block order -> y[r]: fixed summation order, bit-reproducible, no shuffles, no atomics.
-// Per 9 non-zeros: 13 shared-memory loads + 3 stores instead of 27 loads, and 8 + 2/9 bytes from HBM instead of 10.
-// VD (value dictionary): the producer copies the tile's 16-bit block ids where it copied val; every CTA holds the nvd
-// distinct blocks in shared memory and phase 1 reads the nine values of block b from vdict[bvid[b]] - the same bits in
-// the same FMA order, so y and x.y are bit-identical to the kernel that streams val.  4 + 2/9 bytes per block from HBM.
-template <bool DOT, int CW, typename RP, bool VD = false>
+//     Per 9 non-zeros: 13 shared-memory loads + 3 stores instead of 27 loads, and 8 + 2/9 bytes from HBM instead of 10.
+//   k_spmv_bsr3_vd  value dictionary: the stage holds the tile's 16-bit block ids where it held val, and every CTA keeps
+//     the nvd distinct blocks in shared memory; a warp owns a whole tile (see there).  4 + 2/9 bytes per block from HBM.
+constexpr int kBsrMaxStages = 16;   // ring of the dictionary kernel (mbarrier pairs)
+constexpr int kVdStride = 10;       // doubles per dictionary entry in shared memory: 9 values + 1 pad -> five 16-byte loads
+
+// the three row partials of a 3x3 block (rows L doubles apart) times an x triple
+__device__ __forceinline__ void block3_rows(const double *pv, int L, double x0, double x1, double x2, double &p0, double &p1,
+                                            double &p2) {
+  const double a0 = pv[0], a1 = pv[1], a2 = pv[2];
+  const double b0 = pv[L], b1 = pv[L + 1], b2 = pv[L + 2];
+  const double c0 = pv[2 * L], c1 = pv[2 * L + 1], c2 = pv[2 * L + 2];
+  p0 = fma(a2, x2, fma(a1, x1, a0 * x0));
+  p1 = fma(b2, x2, fma(b1, x1, b0 * x0));
+  p2 = fma(c2, x2, fma(c1, x1, c0 * x0));
+}
+
+// stage of the node-block ring: sval[cap_nnz] f64 | sx[cap_x] f64 | snp[cap_nodes+2] i64 | sbidx[cap_blocks+16] u16 | meta[8] i32
+//                         VD:                      sx[cap_x] f64 | snp[cap_nodes+2] i64 | sbidx[cap_blocks+16] u16 | svid[cap_blocks+16] u16 | meta
+struct Bsr3Stage {
+  size_t off_sx, off_snp, off_sb, off_sv, off_meta;
+};
+template <bool VD>
+__device__ __forceinline__ Bsr3Stage bsr3_stage(int cap_nnz, int cap_x, int cap_nodes, int cap_blocks) {
+  const size_t sb_bytes = ((size_t)(cap_blocks + 16) * 2 + 15) & ~(size_t)15;
+  Bsr3Stage L;
+  L.off_sx = VD ? 0 : (size_t)cap_nnz * 8;
+  L.off_snp = L.off_sx + (size_t)cap_x * 8;
+  L.off_sb = L.off_snp + (size_t)(cap_nodes + 2) * 8;
+  L.off_sv = L.off_sb + sb_bytes;
+  L.off_meta = L.off_sb + (VD ? 2 : 1) * sb_bytes;
+  return L;
+}
+
+// producer warp p of nprod (tiles it = p, p + nprod, ...; stage it % stages, stages % nprod == 0): TMA val (VD: the block
+// ids) + block indices, cp.async node offsets + x windows.  The descriptor and the window descriptors of the NEXT tile
+// are fetched while the current one is being issued.
+template <bool VD, typename RP>
+__device__ __forceinline__ void bsr3_produce(int p, int nprod, unsigned char *smem_raw, const Bsr3Stage &SL, int stages,
+                                             int stage_bytes, uint64_t *full_bar, uint64_t *empty_bar,
+                                             const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx,
+                                             const double *__restrict__ val, const uint16_t *__restrict__ bvid,
+                                             const double *__restrict__ x, const TileDesc *__restrict__ desc,
+                                             const int *__restrict__ win_start, const int *__restrict__ win_off, int ntiles,
+                                             int64_t nnz) {
+  const int lane = threadIdx.x & 31;
+  const uint64_t pol = l2_evict_first_policy();
+  int it = p;
+  int tile = blockIdx.x + it * gridDim.x;
+  bool have = tile < ntiles;
+  int4 d0 = make_int4(0, 0, 0, 0), d1 = make_int4(0, 0, 0, 0);
+  int ws = 0, wo = 0;
+  if (have) {
+    const int4 *dp = reinterpret_cast<const int4 *>(desc + tile);
+    d0 = __ldg(dp); d1 = __ldg(dp + 1);
+    if (lane < d1.z) { ws = __ldg(win_start + d1.y + lane); wo = __ldg(win_off + d1.y + lane); }
+  }
+  while (have) {
+    const int s = it % stages;
+    const uint32_t ph = (uint32_t)((it / stages) & 1);
+    const int nit = it + nprod;
+    const int ntile = blockIdx.x + nit * gridDim.x;
+    const bool nhave = ntile < ntiles;
+    int4 nd0 = make_int4(0, 0, 0, 0), nd1 = make_int4(0, 0, 0, 0);
+    if (nhave) {
+      const int4 *dp = reinterpret_cast<const int4 *>(desc + ntile);
+      nd0 = __ldg(dp); nd1 = __ldg(dp + 1);
+    }
+    const int64_t k0 = ((int64_t)(uint32_t)d0.x) | ((int64_t)d0.y << 32);
+    const int cnt = d0.z, r0 = d0.w, R = d1.x & 0x3fffffff, uni = (d1.x >> 30) & 1, wb = d1.y, nw = d1.z, xlen = d1.w;
+    unsigned char *base = smem_raw + (size_t)s * stage_bytes;
+    double *sval = reinterpret_cast<double *>(base);
+    double *sx = reinterpret_cast<double *>(base + SL.off_sx);
+    RP *snp = reinterpret_cast<RP *>(base + SL.off_snp);
+    uint16_t *sb = reinterpret_cast<uint16_t *>(base + SL.off_sb);
+    int *meta = reinterpret_cast<int *>(base + SL.off_meta);
+    const int64_t k1 = k0 + cnt;
+    const int64_t ka = k0 & ~(int64_t)kAlignMask;
+    mbar_wait(&empty_bar[s], ph ^ 1u);
+    if (lane == 0) {
+      // bidx (and bvid) are padded by 16 entries: the aligned window [ba, bend) never leaves the array
+      const int64_t b0 = k0 / 9, ba = b0 & ~(int64_t)kAlignMask;
+      const int64_t bend = (b0 + cnt / 9 + kAlignMask) & ~(int64_t)kAlignMask;
+      const uint32_t ib = (uint32_t)(bend - ba) * 2u;
+      if (VD) {
+        mbar_expect_tx(&full_bar[s], 2u * ib);
+        if (ib > 0) {
+          bulk_g2s(sb, bidx + ba, ib, &full_bar[s], pol);
+          bulk_g2s(base + SL.off_sv, bvid + ba, ib, &full_bar[s], pol);
+        }
+      } else {
+        int64_t kend = (k1 + kAlignMask) & ~(int64_t)kAlignMask;
+        const int64_t lim = nnz & ~(int64_t)kAlignMask;
+        if (kend > lim) kend = lim;
+        const int nb = (int)(kend - ka);
+        mbar_expect_tx(&full_bar[s], (nb > 0 ? (uint32_t)nb * 8u : 0u) + ib);
+        if (nb > 0) bulk_g2s(sval, val + ka, (uint32_t)nb * 8u, &full_bar[s], pol);
+        if (ib > 0) bulk_g2s(sb, bidx + ba, ib, &full_bar[s], pol);
+      }
+      meta[0] = r0; meta[1] = R; meta[2] = tile; meta[3] = cnt;
+      meta[4] = (int)(k0 & 0xffffffff); meta[5] = (int)(k0 >> 32); meta[6] = (int)(b0 - ba); meta[7] = uni;
+    }
+    if (!VD) {
+      const int64_t lim = nnz & ~(int64_t)kAlignMask;
+      const int64_t kt = (lim > ka ? lim : ka) + lane;
+      if (lane <= kAlignMask && kt >= lim && kt < k1) sval[kt - ka] = val[kt];
+    }
+    // offsets of the first row of every node of the tile (+ the end): asynchronous copies
+    for (int i = lane; i <= R / 3; i += 32) cp_async<sizeof(RP)>(snp + i, rowptr + r0 + 3 * i);
+    for (int w0 = 0; w0 < nw; w0 += 32) {
+      if (w0 > 0) {
+        ws = 0; wo = 0;
+        if (w0 + lane < nw) { ws = __ldg(win_start + wb + w0 + lane); wo = __ldg(win_off + wb + w0 + lane); }
+      }
+      const int nwc = min(32, nw - w0);
+      const int wo_next = (w0 + nwc < nw) ? __ldg(win_off + wb + w0 + nwc) : xlen;
+      for (int w = 0; w < nwc; ++w) {
+        const int s0 = __shfl_sync(0xffffffffu, ws, w), o0 = __shfl_sync(0xffffffffu, wo, w);
+        const int o1n = __shfl_sync(0xffffffffu, wo, (w + 1) & 31);
+        const int len = ((w + 1 < nwc) ? o1n : wo_next) - o0;
+        for (int t = lane; t < len; t += 32) cp_async<8>(sx + o0 + t, x + s0 + t);
+      }
+    }
+    int nws = 0, nwo = 0;
+    if (nhave && lane < nd1.z) { nws = __ldg(win_start + nd1.y + lane); nwo = __ldg(win_off + nd1.y + lane); }
+    cp_async_arrive_noinc(&full_bar[s]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&full_bar[s]);
+    d0 = nd0; d1 = nd1; ws = nws; wo = nwo; it = nit; tile = ntile; have = nhave;
+  }
+}
+
+template <bool DOT, int CW, typename RP>
 __global__ void __launch_bounds__((CW + 4) * 32)
 k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, const double *__restrict__ val,
             const double *__restrict__ x, double *__restrict__ y, const TileDesc *__restrict__ desc,
             const int *__restrict__ win_start, const int *__restrict__ win_off, int ntiles, int64_t nnz, int cap_nnz,
             int cap_nodes, int cap_x, int cap_blocks, int stages, int stage_bytes, int mode, double *__restrict__ dot_partials,
-            const int *__restrict__ skip, const uint16_t *__restrict__ bvid = nullptr, const double *__restrict__ vdict = nullptr,
-            int nvd = 0) {
+            const int *__restrict__ skip) {
   if (skip != nullptr && *skip != 0) return;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   __shared__ uint64_t full_bar[8], empty_bar[8];
@@ -817,119 +947,26 @@ k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, co
   }
   __syncthreads();
 
-  // stage layout: sval[cap_nnz] f64 | sx[cap_x] f64 | snp[cap_nodes+2] i64 | sbidx[cap_blocks+16] u16 | meta[8] i32
-  //          VD:                      sx[cap_x] f64 | snp[cap_nodes+2] i64 | sbidx[cap_blocks+16] u16 | svid[cap_blocks+16] u16 | meta
-  const size_t sb_bytes = ((size_t)(cap_blocks + 16) * 2 + 15) & ~(size_t)15;
-  const size_t off_sx = VD ? 0 : (size_t)cap_nnz * 8, off_snp = off_sx + (size_t)cap_x * 8;
-  const size_t off_sb = off_snp + (size_t)(cap_nodes + 2) * 8, off_sv = off_sb + sb_bytes, off_meta = off_sb + (VD ? 2 : 1) * sb_bytes;
+  const Bsr3Stage SL = bsr3_stage<false>(cap_nnz, cap_x, cap_nodes, cap_blocks);
   // scratch behind the stages: row partials [2][3*cap_blocks] f64, node block offsets [2][cap_nodes+2] i32
   // (tried and rejected: a warp-segmented scan that leaves only a few partials per tile - no 25 KB scratch, larger stages - but
   //  35 shuffles per pass; 8 lanes per row in phase 2 serialises the two phases)
   // mode bit 1 (default): the row partials of a block OVERWRITE the block's own first-row values in the stage (the thread has all
   // nine values in registers by then) - no separate scratch, which buys a third stage per CTA; the stage is handed back to
-  // the producer only after phase 2 has read the partials.  A VD stage holds no values: the scratch is always used.
-  const bool inplace = !VD && (mode & 2) != 0;
+  // the producer only after phase 2 has read the partials.
+  const bool inplace = (mode & 2) != 0;
   const int part_len = inplace ? 0 : 3 * cap_blocks;
   double *spart = reinterpret_cast<double *>(smem_raw + (size_t)stages * stage_bytes);
   int *snbo = reinterpret_cast<int *>(spart + (size_t)2 * part_len);
-  double *sdict = reinterpret_cast<double *>(snbo + 2 * (cap_nodes + 2));   // VD: nvd blocks behind the scratch (16 B aligned)
 
   if (warp >= CW) {
-    // ================= producer warp p (see k_spmv_persist): TMA val + block indices, cp.async node offsets + x windows
-    const int p = warp - CW;
-    const uint64_t pol = l2_evict_first_policy();
-    int it = p;
-    int tile = blockIdx.x + it * gridDim.x;
-    bool have = tile < ntiles;
-    int4 d0 = make_int4(0, 0, 0, 0), d1 = make_int4(0, 0, 0, 0);
-    int ws = 0, wo = 0;
-    if (have) {
-      const int4 *dp = reinterpret_cast<const int4 *>(desc + tile);
-      d0 = __ldg(dp); d1 = __ldg(dp + 1);
-      if (lane < d1.z) { ws = __ldg(win_start + d1.y + lane); wo = __ldg(win_off + d1.y + lane); }
-    }
-    while (have) {
-      const int s = it % stages;
-      const uint32_t ph = (uint32_t)((it / stages) & 1);
-      const int nit = it + nprod;
-      const int ntile = blockIdx.x + nit * gridDim.x;
-      const bool nhave = ntile < ntiles;
-      int4 nd0 = make_int4(0, 0, 0, 0), nd1 = make_int4(0, 0, 0, 0);
-      if (nhave) {
-        const int4 *dp = reinterpret_cast<const int4 *>(desc + ntile);
-        nd0 = __ldg(dp); nd1 = __ldg(dp + 1);
-      }
-      const int64_t k0 = ((int64_t)(uint32_t)d0.x) | ((int64_t)d0.y << 32);
-      const int cnt = d0.z, r0 = d0.w, R = d1.x & 0x3fffffff, uni = (d1.x >> 30) & 1, wb = d1.y, nw = d1.z, xlen = d1.w;
-      unsigned char *base = smem_raw + (size_t)s * stage_bytes;
-      double *sval = reinterpret_cast<double *>(base);
-      double *sx = reinterpret_cast<double *>(base + off_sx);
-      RP *snp = reinterpret_cast<RP *>(base + off_snp);
-      uint16_t *sb = reinterpret_cast<uint16_t *>(base + off_sb);
-      int *meta = reinterpret_cast<int *>(base + off_meta);
-      const int64_t k1 = k0 + cnt;
-      const int64_t ka = k0 & ~(int64_t)kAlignMask;
-      mbar_wait(&empty_bar[s], ph ^ 1u);
-      if (lane == 0) {
-        // bidx (and bvid) are padded by 16 entries: the aligned window [ba, bend) never leaves the array
-        const int64_t b0 = k0 / 9, ba = b0 & ~(int64_t)kAlignMask;
-        const int64_t bend = (b0 + cnt / 9 + kAlignMask) & ~(int64_t)kAlignMask;
-        const uint32_t ib = (uint32_t)(bend - ba) * 2u;
-        if (VD) {
-          mbar_expect_tx(&full_bar[s], 2u * ib);
-          if (ib > 0) {
-            bulk_g2s(sb, bidx + ba, ib, &full_bar[s], pol);
-            bulk_g2s(base + off_sv, bvid + ba, ib, &full_bar[s], pol);
-          }
-        } else {
-          int64_t kend = (k1 + kAlignMask) & ~(int64_t)kAlignMask;
-          const int64_t lim = nnz & ~(int64_t)kAlignMask;
-          if (kend > lim) kend = lim;
-          const int nb = (int)(kend - ka);
-          mbar_expect_tx(&full_bar[s], (nb > 0 ? (uint32_t)nb * 8u : 0u) + ib);
-          if (nb > 0) bulk_g2s(sval, val + ka, (uint32_t)nb * 8u, &full_bar[s], pol);
-          if (ib > 0) bulk_g2s(sb, bidx + ba, ib, &full_bar[s], pol);
-        }
-        meta[0] = r0; meta[1] = R; meta[2] = tile; meta[3] = cnt;
-        meta[4] = (int)(k0 & 0xffffffff); meta[5] = (int)(k0 >> 32); meta[6] = (int)(b0 - ba); meta[7] = uni;
-      }
-      if (!VD) {
-        const int64_t lim = nnz & ~(int64_t)kAlignMask;
-        const int64_t kt = (lim > ka ? lim : ka) + lane;
-        if (lane <= kAlignMask && kt >= lim && kt < k1) sval[kt - ka] = val[kt];
-      }
-      // offsets of the first row of every node of the tile (+ the end): asynchronous copies
-      for (int i = lane; i <= R / 3; i += 32) cp_async<sizeof(RP)>(snp + i, rowptr + r0 + 3 * i);
-      for (int w0 = 0; w0 < nw; w0 += 32) {
-        if (w0 > 0) {
-          ws = 0; wo = 0;
-          if (w0 + lane < nw) { ws = __ldg(win_start + wb + w0 + lane); wo = __ldg(win_off + wb + w0 + lane); }
-        }
-        const int nwc = min(32, nw - w0);
-        const int wo_next = (w0 + nwc < nw) ? __ldg(win_off + wb + w0 + nwc) : xlen;
-        for (int w = 0; w < nwc; ++w) {
-          const int s0 = __shfl_sync(0xffffffffu, ws, w), o0 = __shfl_sync(0xffffffffu, wo, w);
-          const int o1n = __shfl_sync(0xffffffffu, wo, (w + 1) & 31);
-          const int len = ((w + 1 < nwc) ? o1n : wo_next) - o0;
-          for (int t = lane; t < len; t += 32) cp_async<8>(sx + o0 + t, x + s0 + t);
-        }
-      }
-      int nws = 0, nwo = 0;
-      if (nhave && lane < nd1.z) { nws = __ldg(win_start + nd1.y + lane); nwo = __ldg(win_off + nd1.y + lane); }
-      cp_async_arrive_noinc(&full_bar[s]);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&full_bar[s]);
-      d0 = nd0; d1 = nd1; ws = nws; wo = nwo; it = nit; tile = ntile; have = nhave;
-    }
+    bsr3_produce<false, RP>(warp - CW, nprod, smem_raw, SL, stages, stage_bytes, full_bar, empty_bar, rowptr, bidx, val, nullptr,
+                            x, desc, win_start, win_off, ntiles, nnz);
     return;
   }
 
   // ================= consumer warps (CW * 32 threads, tid = consumer thread id)
   constexpr int NT = CW * 32;
-  if (VD) {   // the dictionary, once per launch (from L2 after the first CTAs), while the producers fill the first stages
-    for (int i = tid; i < 9 * nvd; i += NT) sdict[i] = __ldg(vdict + i);
-    named_bar_sync(1, NT);
-  }
   double dsum = 0.0;
   for (int it = 0;; ++it) {
     const int tile = blockIdx.x + it * gridDim.x;
@@ -939,10 +976,10 @@ k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, co
     const int par = it & 1;
     const unsigned char *base = smem_raw + (size_t)s * stage_bytes;
     const double *sval = reinterpret_cast<const double *>(base);
-    const double *sx = reinterpret_cast<const double *>(base + off_sx);
-    const RP *snp = reinterpret_cast<const RP *>(base + off_snp);
-    const uint16_t *sb = reinterpret_cast<const uint16_t *>(base + off_sb);
-    const int *meta = reinterpret_cast<const int *>(base + off_meta);
+    const double *sx = reinterpret_cast<const double *>(base + SL.off_sx);
+    const RP *snp = reinterpret_cast<const RP *>(base + SL.off_snp);
+    const uint16_t *sb = reinterpret_cast<const uint16_t *>(base + SL.off_sb);
+    const int *meta = reinterpret_cast<const int *>(base + SL.off_meta);
     double *part = spart + (size_t)par * part_len;
     int *nbo = snbo + par * (cap_nodes + 2);
     mbar_wait(&full_bar[s], ph);
@@ -951,7 +988,6 @@ k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, co
     const int k0l = (int)(k0 & kAlignMask);
     const int NN = R / 3, NB = cnt / 9;
     const uint16_t *sbt = sb + meta[6];
-    const uint16_t *svdt = reinterpret_cast<const uint16_t *>(base + off_sv) + meta[6];   // VD only
     const double *svt = sval + k0l;
     // uniform tile (all nodes have the same number of blocks - the interior of a structured mesh): node = b / Lb, no look-ups
     const bool uni = (mode & 1) != 0 && meta[7] != 0 && NN > 0 && NB >= 2 * NN;   // (>= 2 blocks per node: the reciprocal fits 32 bits)
@@ -961,39 +997,27 @@ k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, co
     for (int i = tid; i <= NN; i += NT) nbo[i] = uni ? i * Lbu : (int)((int64_t)snp[i] - k0) / 9;
     // ---- phase 1: one 3x3 block per thread and pass
     for (int b = tid; b < NB; b += NT) {
-      const double *pv;
-      int L;
-      if (VD) {
-        // dictionary entry: rows 3 values apart (ids of the tile's blocks at the same offset as sbt)
-        pv = sdict + 9 * (int)svdt[b];
-        L = 3;
+      int noff, t3, L;
+      if (uni) {
+        const int i = (int)__umulhi((unsigned)b, magic);
+        noff = i * 9 * Lbu; L = 3 * Lbu; t3 = 3 * (b - i * Lbu);
       } else {
-        int noff, t3;
-        if (uni) {
-          const int i = (int)__umulhi((unsigned)b, magic);
-          noff = i * 9 * Lbu; L = 3 * Lbu; t3 = 3 * (b - i * Lbu);
-        } else {
-          int lo = 0, hi = NN - 1;                     // node of block b: last i with (snp[i] - k0) <= 9 b
-          const int kb = 9 * b;
-          while (lo < hi) {
-            const int mid = (lo + hi + 1) >> 1;
-            if ((int)((int64_t)snp[mid] - k0) <= kb) lo = mid; else hi = mid - 1;
-          }
-          noff = (int)((int64_t)snp[lo] - k0);
-          L = ((int)((int64_t)snp[lo + 1] - k0) - noff) / 3;   // non-zeros per row of this node
-          t3 = (kb - noff) / 3;                                  // 3 t, t = b - noff / 9
+        int lo = 0, hi = NN - 1;                     // node of block b: last i with (snp[i] - k0) <= 9 b
+        const int kb = 9 * b;
+        while (lo < hi) {
+          const int mid = (lo + hi + 1) >> 1;
+          if ((int)((int64_t)snp[mid] - k0) <= kb) lo = mid; else hi = mid - 1;
         }
-        pv = svt + noff + t3;
+        noff = (int)((int64_t)snp[lo] - k0);
+        L = ((int)((int64_t)snp[lo + 1] - k0) - noff) / 3;   // non-zeros per row of this node
+        t3 = (kb - noff) / 3;                                  // 3 t, t = b - noff / 9
       }
+      const double *pv = svt + noff + t3;
       const int ii = sbt[b];
-      const double x0 = sx[ii], x1 = sx[ii + 1], x2 = sx[ii + 2];
-      const double a0 = pv[0], a1 = pv[1], a2 = pv[2];
-      const double b0 = pv[L], b1 = pv[L + 1], b2 = pv[L + 2];
-      const double c0 = pv[2 * L], c1 = pv[2 * L + 1], c2 = pv[2 * L + 2];
+      double p0, p1, p2;
+      block3_rows(pv, L, sx[ii], sx[ii + 1], sx[ii + 2], p0, p1, p2);
       double *pp = inplace ? const_cast<double *>(pv) : part + 3 * b;   // in place: positions 3t..3t+2 of the node's first row
-      pp[0] = fma(a2, x2, fma(a1, x1, a0 * x0));
-      pp[1] = fma(b2, x2, fma(b1, x1, b0 * x0));
-      pp[2] = fma(c2, x2, fma(c1, x1, c0 * x0));
+      pp[0] = p0; pp[1] = p1; pp[2] = p2;
     }
     const bool has_rows = warp * 32 < R;            // this warp owns rows in phase 2
     if (!inplace || !has_rows) {
@@ -1020,6 +1044,122 @@ k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, co
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic writes to the stage before the next TMA fill
       __syncwarp();
       if (lane == 0) mbar_arrive(&empty_bar[s]);
+    }
+  }
+  if (DOT) {
+    double v = warp_sum(dsum);
+    if (lane == 0) red[warp] = v;
+    named_bar_sync(1, NT);
+    if (warp == 0) {
+      double t = lane < CW ? red[lane] : 0.0;
+      t = warp_sum(t);
+      if (lane == 0) dot_partials[blockIdx.x] = t;
+    }
+  }
+}
+
+// Value-dictionary consumer.  The CTA takes its tiles (it = 0, 1, ... -> tile blockIdx.x + it * gridDim.x, as above) in
+// groups of G consecutive ones:
+//     phase A   warp g < G owns tile g of the group, with no CTA barrier: lane <-> node, the lane walks the node's blocks
+//               in block order and keeps the three row sums in registers (acc += the block's row partial, from 0.0 - the
+//               partial and the sum of k_spmv_bsr3 exactly), writes them to the group's y buffer and hands the stage back;
+//     phase B   after ONE named barrier per group, the tiles of the group in tile order, thread r < R of the NT = CW * 32
+//               consumer threads storing row r and adding x.y as k_spmv_bsr3's phase 2 does.
+// So every consumer thread sees the same rows in the same order as there: y and every per-CTA x.y partial are the same
+// bits, and G only sets how many stages are in flight.  Per 32 blocks (one warp step): 2 x 1 index loads, 3 x loads at
+// stride 3 doubles and five 16-byte dictionary loads that are broadcasts where the nodes share the block (the interior).
+// The y buffers are double-buffered by group parity: the barrier of group n + 1 orders phase B of group n before phase A
+// of group n + 2.
+template <bool DOT, int CW, typename RP>
+__global__ void __launch_bounds__((CW + 4) * 32)
+k_spmv_bsr3_vd(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, const uint16_t *__restrict__ bvid,
+               const double *__restrict__ vdict, int nvd, const double *__restrict__ x, double *__restrict__ y,
+               const TileDesc *__restrict__ desc, const int *__restrict__ win_start, const int *__restrict__ win_off,
+               int ntiles, int cap_nodes, int cap_x, int cap_blocks, int stages, int stage_bytes, int group,
+               double *__restrict__ dot_partials, const int *__restrict__ skip) {
+  if (skip != nullptr && *skip != 0) return;
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  __shared__ uint64_t full_bar[kBsrMaxStages], empty_bar[kBsrMaxStages];
+  __shared__ int2 grows[2][kBsrMaxStages];   // (r0, R) of the tiles of a group, by group parity
+  __shared__ double red[32];
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int nprod = (int)(blockDim.x >> 5) - CW;   // producer warps; stages % nprod == 0, group <= stages
+
+  if (tid == 0) {
+    for (int s = 0; s < stages; ++s) { mbar_init(&full_bar[s], 34); mbar_init(&empty_bar[s], 1); }
+    mbar_fence_init();
+  }
+  __syncthreads();
+
+  const Bsr3Stage SL = bsr3_stage<true>(0, cap_x, cap_nodes, cap_blocks);
+  // behind the stages: y buffers [2][group][3 * cap_nodes] f64, then the dictionary [nvd][kVdStride] f64 (16 B aligned)
+  const int ylen = 3 * cap_nodes;
+  double *sy = reinterpret_cast<double *>(smem_raw + (size_t)stages * stage_bytes);
+  double *sdict = sy + (size_t)2 * group * ylen;
+
+  if (warp >= CW) {
+    bsr3_produce<true, RP>(warp - CW, nprod, smem_raw, SL, stages, stage_bytes, full_bar, empty_bar, rowptr, bidx, nullptr, bvid,
+                           x, desc, win_start, win_off, ntiles, 0);
+    return;
+  }
+
+  constexpr int NT = CW * 32;
+  // the dictionary, once per launch (from L2 after the first CTAs), while the producers fill the first stages
+  for (int i = tid; i < kVdStride * nvd; i += NT) {
+    const int e = i / kVdStride, c = i - kVdStride * e;
+    sdict[i] = c < 9 ? __ldg(vdict + 9 * e + c) : 0.0;
+  }
+  named_bar_sync(1, NT);
+  double dsum = 0.0;
+  for (int g0 = 0; blockIdx.x + g0 * gridDim.x < ntiles; g0 += group) {
+    const int par = (g0 / group) & 1;
+    double *yg = sy + (size_t)par * group * ylen;
+    // ---- phase A: warp g takes tile g0 + g of the group
+    if (warp < group) {
+      const int it = g0 + warp;
+      const int tile = blockIdx.x + it * gridDim.x;
+      if (tile < ntiles) {
+        const int s = it % stages;
+        const unsigned char *base = smem_raw + (size_t)s * stage_bytes;
+        const double *sx = reinterpret_cast<const double *>(base + SL.off_sx);
+        const RP *snp = reinterpret_cast<const RP *>(base + SL.off_snp);
+        const int *meta = reinterpret_cast<const int *>(base + SL.off_meta);
+        mbar_wait(&full_bar[s], (uint32_t)((it / stages) & 1));
+        const int r0 = meta[0], R = meta[1];
+        const int64_t k0 = ((int64_t)(uint32_t)meta[4]) | ((int64_t)meta[5] << 32);
+        const uint16_t *sbt = reinterpret_cast<const uint16_t *>(base + SL.off_sb) + meta[6];
+        const uint16_t *svdt = reinterpret_cast<const uint16_t *>(base + SL.off_sv) + meta[6];
+        double *yt = yg + warp * ylen;
+        for (int i = lane; i < R / 3; i += 32) {
+          const int b0 = (int)((int64_t)snp[i] - k0) / 9, b1 = (int)((int64_t)snp[i + 1] - k0) / 9;
+          double acc0 = 0.0, acc1 = 0.0, acc2 = 0.0;
+#pragma unroll 2
+          for (int b = b0; b < b1; ++b) {
+            const int ii = sbt[b];
+            const double2 *pv = reinterpret_cast<const double2 *>(sdict + kVdStride * (int)svdt[b]);
+            const double2 v01 = pv[0], v23 = pv[1], v45 = pv[2], v67 = pv[3], v8 = pv[4];
+            const double x0 = sx[ii], x1 = sx[ii + 1], x2 = sx[ii + 2];
+            acc0 += fma(v23.x, x2, fma(v01.y, x1, v01.x * x0));
+            acc1 += fma(v45.y, x2, fma(v45.x, x1, v23.y * x0));
+            acc2 += fma(v8.x, x2, fma(v67.y, x1, v67.x * x0));
+          }
+          yt[3 * i] = acc0; yt[3 * i + 1] = acc1; yt[3 * i + 2] = acc2;
+        }
+        if (lane == 0) grows[par][warp] = make_int2(r0, R);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty_bar[s]);
+      }
+    }
+    named_bar_sync(1, NT);
+    // ---- phase B: the tiles of the group in order, one row per consumer thread
+    for (int g = 0; g < group && blockIdx.x + (g0 + g) * gridDim.x < ntiles; ++g) {
+      const int2 rr = grows[par][g];
+      const double *yt = yg + g * ylen;
+      for (int r = tid; r < rr.y; r += NT) {
+        const double acc = yt[r];
+        y[rr.x + r] = acc;
+        if (DOT) dsum = fma(acc, __ldg(x + rr.x + r), dsum);
+      }
     }
   }
   if (DOT) {
@@ -1225,7 +1365,6 @@ struct DevTmp {
 // Value dictionary of a node-block matrix (P.vd = D distinct blocks, P.bvid, P.vdict), or P.vd = 0 when it has more than
 // kVdictMax distinct blocks.  Ids follow the first occurrence of each value, so the plan is deterministic.  mode 1 also
 // refuses a dictionary that the grid's CTAs would load (once each per launch) in more bytes than half the values it replaces.
-constexpr int kVdStages = 4;   // default ring of a dictionary plan (its stages are small)
 template <typename RP>
 inline int build_vdict(CsrPlan &P, cudaStream_t st, int mode, int grid) {
   P.vd = 0;
@@ -1554,17 +1693,31 @@ inline int build_plan_t(CsrPlan &P, cudaStream_t st, int bsr_tile = 0, int attem
               // value dictionary (PCGB_SPMV_VDICT: 0 off, 1 when it pays, 2 whenever the blocks fit it).  The tiles, the grid and
               // the consumer warps stay those of the plan without one - they fix the order in which x.y is summed, so y and
               // x.y are the same bits either way; only the ring changes: a stage holds no values (sx | snp | bidx | bvid |
-              // meta), the row partials go to the scratch, and the dictionary sits behind it.
+              // meta), and behind the ring sit the y buffers of two groups of tiles and the dictionary (k_spmv_bsr3_vd).
               const int vd_mode = env_int("PCGB_SPMV_VDICT", 1);
               if (vd_mode != 0) PCGB_TRY(build_vdict<RP>(P, st, vd_mode, P.grid_bsr));
               if (P.vd) {
-                int vst = std::min(std::max(env_int("PCGB_SPMV_STAGES", kVdStages), 1), 8);
-                const int vprod = vst >= 4 ? 4 : vst;
-                vst -= vst % vprod;
+                // G warps consume G tiles at once, so the ring holds the G stages of a group plus two that the producers
+                // fill for the next one: G = CW where that still fits the CTAs per SM of the plan (hex 128^3: CW 6 and 8),
+                // else the largest G that does.  PCGB_SPMV_STAGES sets the ring instead, G = min(CW, stages).
                 const int vstage = (P.cap_x * 8 + (P.cap_nodes + 2) * 8 + 2 * sb_bytes + 32 + 127) & ~127;
-                const int vsmem = vst * vstage + 6 * P.cap_blocks * 8 + 2 * (P.cap_nodes + 2) * 4 + 64 + 72 * P.vd;
-                if (vsmem <= 226 * 1024 && (227 * 1024) / (vsmem + 2048) >= P.ctas_per_sm) {
-                  P.bsr_stages = vst; P.bsr_prod = vprod; P.bsr_stage_bytes = vstage; P.smem_bsr = vsmem; P.bsr_mode &= ~2;
+                auto ring_smem = [&](int g, int s) { return s * vstage + 2 * g * 3 * P.cap_nodes * 8 + kVdStride * 8 * P.vd; };
+                auto ring_fits = [&](int smem) { return smem <= 226 * 1024 && (227 * 1024) / (smem + 2048) >= P.ctas_per_sm; };
+                int vst = 0, vg = 0;
+                const int env_st = env_int("PCGB_SPMV_STAGES", 0);
+                if (env_st > 0) {
+                  vst = std::min(env_st, kBsrMaxStages);
+                  vg = std::min(P.bsr_cw, vst);
+                  if (!ring_fits(ring_smem(vg, vst))) vst = 0;
+                } else {
+                  for (int g = P.bsr_cw; g >= 1 && vst == 0; --g) {
+                    const int s = std::min((g + 3) & ~1, kBsrMaxStages);   // g + 2, even (producer warps: see below)
+                    if (ring_fits(ring_smem(g, s))) { vst = s; vg = g; }
+                  }
+                }
+                if (vst > 0) {
+                  P.bsr_stages = vst; P.bsr_group = vg; P.bsr_stage_bytes = vstage; P.smem_bsr = ring_smem(vg, vst);
+                  P.bsr_prod = vst < 4 ? vst : vst % 4 == 0 ? 4 : vst % 2 == 0 ? 2 : 1;   // stages % producers == 0
                 } else {
                   cudaFree(P.bvid); cudaFree(P.vdict);
                   P.bvid = nullptr; P.vdict = nullptr; P.vd = 0;
@@ -1683,16 +1836,27 @@ inline int launch_persist_lanes(const CsrPlan &P, const double *x, double *y, cu
 template <bool DOT, int CW, typename RP, bool VD>
 inline int launch_bsr_cw(const CsrPlan &P, const double *x, double *y, cudaStream_t st, const int *skip, const TileDesc *desc,
                          int ntiles, int grid, double *dotp) {
-  auto kern = k_spmv_bsr3<DOT, CW, RP, VD>;
-  if (skip == reinterpret_cast<const int *>(1)) {
-    PCGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
-    return PCGB_OK;
+  if constexpr (VD) {
+    auto kern = k_spmv_bsr3_vd<DOT, CW, RP>;
+    if (skip == reinterpret_cast<const int *>(1)) {
+      PCGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+      return PCGB_OK;
+    }
+    if (ntiles == 0) return PCGB_OK;
+    kern<<<grid, (CW + P.bsr_prod) * 32, P.smem_bsr, st>>>(static_cast<const RP *>(P.rowptr), P.bidx, P.bvid, P.vdict, P.vd, x, y,
+                                                           desc, P.win_start, P.win_off, ntiles, P.cap_nodes, P.cap_x, P.cap_blocks,
+                                                           P.bsr_stages, P.bsr_stage_bytes, P.bsr_group, dotp, skip);
+  } else {
+    auto kern = k_spmv_bsr3<DOT, CW, RP>;
+    if (skip == reinterpret_cast<const int *>(1)) {
+      PCGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 226 * 1024));
+      return PCGB_OK;
+    }
+    if (ntiles == 0) return PCGB_OK;
+    kern<<<grid, (CW + P.bsr_prod) * 32, P.smem_bsr, st>>>(static_cast<const RP *>(P.rowptr), P.bidx, P.val, x, y, desc, P.win_start,
+                                                           P.win_off, ntiles, P.nnz, P.cap_nnz, P.cap_nodes, P.cap_x, P.cap_blocks,
+                                                           P.bsr_stages, P.bsr_stage_bytes, P.bsr_mode, dotp, skip);
   }
-  if (ntiles == 0) return PCGB_OK;
-  kern<<<grid, (CW + P.bsr_prod) * 32, P.smem_bsr, st>>>(static_cast<const RP *>(P.rowptr), P.bidx, P.val, x, y, desc, P.win_start,
-                                                                  P.win_off, ntiles, P.nnz, P.cap_nnz, P.cap_nodes, P.cap_x, P.cap_blocks,
-                                                                  P.bsr_stages, P.bsr_stage_bytes, P.bsr_mode, dotp, skip, P.bvid,
-                                                                  P.vdict, P.vd);
   PCGB_CHECK_LAUNCH();
   return PCGB_OK;
 }
