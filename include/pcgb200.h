@@ -389,6 +389,24 @@ int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked,
  * from any stream).  d_ck_fine is not read after create returns. */
 int pcgb_mg_create_field(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine,
                          const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out);
+/* The one-rank preconditioner for a box of any size, uniform or a voxel model; like pcgb_mg_create and
+ * pcgb_mg_create_field it replaces the diagonal preconditioner of pcg_solver.py:346-352 and 446-454.  Every axis of a
+ * level is coarsened on its own while some axis has ne >= 3: an axis with ne >= 3 is halved to (ne + 1) / 2 elements,
+ * coarse node j at fine node s(j) = min(2j, ne), so an odd axis ends in a coarse element one fine element wide at its high
+ * end; an axis with ne <= 2 is kept (s(j) = j).  The coarsest level has at most 2x2x2 elements (54 dofs).  Fine node i
+ * between s(j) and s(j+1) takes weight (s(j+1) - i) / (s(j+1) - s(j)) from coarse node j and the rest from j + 1 (0, 1/2
+ * or 1); P is the tensor product of the three 1-D maps, clamped nodes dropped.  The coarse levels are Galerkin products of
+ * element matrices as in pcgb_mg_create_field, a coarse element having 1 or 2 children per axis, phi_0(p) = (w - p) / w,
+ * phi_1(p) = p / w with w its width in fine elements; the fine elements carry d_ck_fine (as in pcgb_mg_create_field) or,
+ * d_ck_fine NULL, Ck = E h.  A level whose axes are all halved from even ne uses exactly the kernels of
+ * pcgb_mg_create_field (so an all-even box gives its hierarchy bit for bit); only levels with an odd or kept axis use the
+ * transfers and Galerkin products for any widths.  Element matrices are always built: 4608 bytes per level-1 element at
+ * the peak (pcgb_mg_setup_info).  PCGB_ERR_ARG before anything is allocated: the refusals of pcgb_mg_create_field but the
+ * coarsening rule's (a box with every ne <= 2, more than PCGB_MG_MAX_LEVELS levels), and E or h <= 0. */
+int pcgb_mg_create_any(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine, double E, double h,
+                       const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out);
+/* The element counts of level `level` (0 .. nlevels - 1) of any handle into ne[3] (x, y, z); PCGB_ERR_ARG outside. */
+int pcgb_mg_level_box(pcgb_mg_t mg, int level, int32_t *ne);
 /* For tests: level `level`'s CSR (1 <= level < nlevels - 1, the smoothed coarse levels) into caller buffers: int64 row
  * offsets (n + 1), int32 columns and values (nnz each).  With all three buffers NULL only *nnz is written.  Synchronises
  * `stream`.  PCGB_ERR_ARG for level 0 (the solver's operator), the coarsest level (held as a dense factor) and the

@@ -269,6 +269,137 @@ k_mg_galerkin(int cnx, int cny, int fnx, int fny, const double *__restrict__ ck,
   kc[576 * E + t] = i <= j ? K[t] : K[j * 24 + i];
 }
 
+// ---- boxes of any size (pcgb_mg_create_any).  Every axis of a level is coarsened on its own: halved (ne >= 3; coarse node
+// j sits at fine node s(j) = min(2j, ne), so an odd axis ends in a coarse element one fine element wide at its high end) or
+// kept (ne <= 2; s(j) = j).  `keep` holds one bit per axis (x = 1, y = 2, z = 4).  P is the tensor product of the three 1-D
+// interpolations between consecutive s(j), with weights 0, 1/2 and 1 (exact in binary); clamped nodes carry 0 as above.
+// A level with every axis halved and every ne even uses k_mg_restrict / k_mg_prolong_add / k_mg_galerkin themselves.
+
+// coarse position of coarse node j on an axis of nf fine elements
+__device__ __forceinline__ int mg_any_pos(int j, int nf, bool keep) { return keep ? j : min(2 * j, nf); }
+
+// r_c = P^T r_f for any axis modes: one thread per coarse free node; per axis the fine nodes s(j) + d, d in {-1, 0, 1}, that
+// lie strictly inside the coarse elements on either side (weight 1/2; only an element two fine elements wide has one) and
+// s(j) itself (weight 1), summed in (dz, dy, dx) ascending order from 0.0.  A kept axis contributes d = 0 only.
+__global__ void __launch_bounds__(256)
+k_mg_restrict_any(HexGeom gf, HexGeom gc, int keep, const double *__restrict__ rf, double *__restrict__ rc, const int *__restrict__ skip) {
+  if (skip != nullptr && *skip != 0) return;
+  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (t >= gc.nfree_nodes) return;
+  int c[3];
+  mg_node(gc, t, c[0], c[1], c[2]);
+  const int nf[3] = {gf.nx, gf.ny, gf.nz}, ncm[3] = {gc.nx, gc.ny, gc.nz};
+  int s[3], lo[3], hi[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const bool k = (keep >> a) & 1;
+    s[a] = mg_any_pos(c[a], nf[a], k);
+    lo[a] = c[a] > 0 && s[a] - mg_any_pos(c[a] - 1, nf[a], k) == 2 ? -1 : 0;
+    hi[a] = c[a] < ncm[a] && mg_any_pos(c[a] + 1, nf[a], k) - s[a] == 2 ? 1 : 0;
+  }
+  double s0 = 0.0, s1 = 0.0, s2 = 0.0;
+  for (int dz = lo[2]; dz <= hi[2]; ++dz) {
+    for (int dy = lo[1]; dy <= hi[1]; ++dy) {
+      for (int dx = lo[0]; dx <= hi[0]; ++dx) {
+        const int fx = s[0] + dx;
+        if (fx < gf.x_lo) continue;
+        const double w = (dx ? 0.5 : 1.0) * (dy ? 0.5 : 1.0) * (dz ? 0.5 : 1.0);
+        const double *src = rf + 3 * mg_index(gf, fx, s[1] + dy, s[2] + dz);
+        s0 += w * src[0]; s1 += w * src[1]; s2 += w * src[2];
+      }
+    }
+  }
+  rc[3 * t] = s0; rc[3 * t + 1] = s1; rc[3 * t + 2] = s2;
+}
+
+// x_f += P e_c for any axis modes: one thread per fine free node; per axis the coarse node at the fine node (weight 1) or
+// the two around it (an interior node of a two-wide coarse element, 1/2 each), summed in (z, y, x) ascending order from
+// 0.0, then added to x_f.
+__global__ void __launch_bounds__(256)
+k_mg_prolong_add_any(HexGeom gf, HexGeom gc, int keep, const double *__restrict__ ec, double *__restrict__ xf, const int *__restrict__ skip) {
+  if (skip != nullptr && *skip != 0) return;
+  const int64_t t = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (t >= gf.nfree_nodes) return;
+  int f[3];
+  mg_node(gf, t, f[0], f[1], f[2]);
+  const int nf[3] = {gf.nx, gf.ny, gf.nz};
+  int c0[3], m[3];
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    if ((keep >> a) & 1) { c0[a] = f[a]; m[a] = 1; }
+    else if ((f[a] & 1) == 0) { c0[a] = f[a] >> 1; m[a] = 1; }
+    else if (f[a] == nf[a]) { c0[a] = (f[a] + 1) >> 1; m[a] = 1; }   // the high end of an odd axis: a coarse node
+    else { c0[a] = f[a] >> 1; m[a] = 2; }
+  }
+  const double w = (m[0] == 2 ? 0.5 : 1.0) * (m[1] == 2 ? 0.5 : 1.0) * (m[2] == 2 ? 0.5 : 1.0);
+  double s0 = 0.0, s1 = 0.0, s2 = 0.0;
+  for (int kz = 0; kz < m[2]; ++kz) {
+    for (int ky = 0; ky < m[1]; ++ky) {
+      for (int kx = 0; kx < m[0]; ++kx) {
+        const int cx = c0[0] + kx;
+        if (cx < gc.x_lo) continue;   // clamped coarse node
+        const double *src = ec + 3 * mg_index(gc, cx, c0[1] + ky, c0[2] + kz);
+        s0 += w * src[0]; s1 += w * src[1]; s2 += w * src[2];
+      }
+    }
+  }
+  xf[3 * t] += s0; xf[3 * t + 1] += s1; xf[3 * t + 2] += s2;
+}
+
+// mg_child_weight for coarse elements of width w_a in {1, 2} fine elements per axis (bit a of `thin`: w_a = 1, so c_a = 0):
+// phi_0(p) = (w - p) / w, phi_1(p) = p / w.  A width-2 axis performs mg_child_weight's arithmetic.
+__device__ __forceinline__ double mg_child_weight_any(int c, int l, int k, int thin) {
+  double w = 1.0;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const int p = ((c >> a) & 1) + ((l >> a) & 1);
+    if ((thin >> a) & 1) w *= ((k >> a) & 1) ? (double)p : (double)(1 - p);
+    else w *= ((k >> a) & 1) ? 0.5 * p : 0.5 * (2 - p);
+  }
+  return w;
+}
+
+// k_mg_galerkin for any axis modes: coarse element (X, Y, Z) covers fine elements s(X) .. s(X+1) - 1 per axis (one or two),
+// and K_E = sum_c Q_c^T K_c Q_c over the children that exist, c = cx + 2 cy + 4 cz ascending, with mg_child_weight_any.
+// When every axis is two wide this is k_mg_galerkin's arithmetic in k_mg_galerkin's order.  Every thread of a CTA skips the
+// same children, so the barriers stay uniform.
+__global__ void __launch_bounds__(kMgGalerkinThreads)
+k_mg_galerkin_any(int cnx, int cny, int fnx, int fny, int fnz, int keep, const double *__restrict__ ck, const double *__restrict__ kf,
+                  double *__restrict__ kc) {
+  __shared__ double K[576], T[576];
+  const int t = threadIdx.x, i = t / 24, j = t % 24;
+  const int64_t E = blockIdx.x;
+  const int C[3] = {(int)(E % cnx), (int)((E / cnx) % cny), (int)(E / ((int64_t)cnx * cny))};
+  const int nf[3] = {fnx, fny, fnz};
+  int f0[3], m[3], thin = 0;
+#pragma unroll
+  for (int a = 0; a < 3; ++a) {
+    const bool k = (keep >> a) & 1;
+    f0[a] = mg_any_pos(C[a], nf[a], k);
+    m[a] = mg_any_pos(C[a] + 1, nf[a], k) - f0[a];
+    if (m[a] == 1) thin |= 1 << a;
+  }
+  double acc = 0.0;
+  for (int c = 0; c < 8; ++c) {
+    if ((c & 1) >= m[0] || ((c >> 1) & 1) >= m[1] || (c >> 2) >= m[2]) continue;
+    const int64_t child = ((int64_t)(f0[2] + (c >> 2)) * fny + (f0[1] + ((c >> 1) & 1))) * fnx + (f0[0] + (c & 1));
+    K[t] = kf ? kf[576 * child + t] : ck[child] * c_hex_ke[t];
+    __syncthreads();
+    double s = 0.0;
+#pragma unroll
+    for (int l = 0; l < 8; ++l) s += mg_child_weight_any(c, l, j / 3, thin) * K[i * 24 + 3 * l + j % 3];
+    T[t] = s;
+    __syncthreads();
+    s = 0.0;
+#pragma unroll
+    for (int l = 0; l < 8; ++l) s += mg_child_weight_any(c, l, i / 3, thin) * T[(3 * l + i % 3) * 24 + j];
+    acc += s;
+  }
+  K[t] = acc;   // every thread is past its last read of K (the second barrier of the last child)
+  __syncthreads();
+  kc[576 * E + t] = i <= j ? K[t] : K[j * 24 + i];
+}
+
 // dense[i][col] = val of the coarsest level's CSR (dense zero-filled before)
 __global__ void k_mg_densify(int64_t n, const int64_t *__restrict__ rowptr, const int *__restrict__ col, const double *__restrict__ val,
                              double *__restrict__ dense) {

@@ -100,7 +100,11 @@ struct pcgb_solver_s {
   long long trace_cap = 0;
   double *snapshot = nullptr;   // [5][n] + 3: r, p, q, x buffer 0, x buffer 1, then xcur, xmin, alias at the loop exit
   double *tr_local = nullptr;   // [8] device: this rank's sums before the all-reduce (multi-rank traces)
+  // multigrid handles built on this solver: destroying the solver first detaches them, so a later pcgb_mg_destroy (a
+  // garbage collector may finalise the two in either order) does not read the freed solver
+  std::vector<pcgb_mg_t> mgs;
 };
+void mg_detach(pcgb_mg_t mg);
 
 static int require_device() {
   int n = 0;
@@ -873,6 +877,7 @@ int pcgb_solver_create_ebe_ordered(pcgb_ebe_ordered_t O, pcgb_halo_t halo, pcgb_
 
 int pcgb_solver_destroy(pcgb_solver_t s) {
   if (!s) return PCGB_OK;
+  for (pcgb_mg_t mg : s->mgs) mg_detach(mg);
   if (s->gexec) cudaGraphExecDestroy(s->gexec);
   if (s->own) cudaStreamDestroy(s->own);
   if (s->side) cudaStreamDestroy(s->side);
@@ -1007,6 +1012,10 @@ struct MgLevel {
   double *r = nullptr, *d = nullptr, *q = nullptr;           // smoother residual, direction, operator product
   double lambda = 0.0, inv_theta = 0.0;
   std::vector<double> c1, c2;                                // Chebyshev recurrence of steps 1 .. degree-1
+  // the coarsening from this level to the next (pcgb_mg_create_any): any = some axis is kept or odd, so the transfers
+  // and the Galerkin products take the *_any kernels with `keep` (bit a: axis a kept); otherwise every ne is halved
+  bool any = false;
+  int keep = 0;
 };
 
 struct pcgb_mg_s {
@@ -1029,6 +1038,8 @@ struct pcgb_mg_s {
   int64_t kel_peak = 0;
   double galerkin_ms = 0.0;
 };
+
+void mg_detach(pcgb_mg_t mg) { mg->s = nullptr; }
 
 namespace {
 
@@ -1077,10 +1088,21 @@ int mg_coarse_solve(pcgb_mg_t mg, const double *r, double *z, cudaStream_t st, i
 // exchange-add completes the sum
 int mg_restrict(pcgb_mg_t mg, int l, const double *rf, double *rc, cudaStream_t st, int *nl, const int *skip) {
   const MgLevel &A = mg->lv[(size_t)l], &C = mg->lv[(size_t)l + 1];
-  k_mg_restrict<<<mg_node_grid(C.g), 256, 0, st>>>(A.g, C.g, rf, A.own, rc, skip);
+  if (A.any) k_mg_restrict_any<<<mg_node_grid(C.g), 256, 0, st>>>(A.g, C.g, A.keep, rf, rc, skip);
+  else k_mg_restrict<<<mg_node_grid(C.g), 256, 0, st>>>(A.g, C.g, rf, A.own, rc, skip);
   PCGB_CHECK_LAUNCH();
   *nl += 1;
   return C.halo ? halo_exchange_add(C.halo, rc, st, nl) : PCGB_OK;
+}
+
+// x_f += P e_c from level l+1 to l
+int mg_prolong_add(pcgb_mg_t mg, int l, const double *ec, double *xf, cudaStream_t st, int *nl, const int *skip) {
+  const MgLevel &A = mg->lv[(size_t)l], &C = mg->lv[(size_t)l + 1];
+  if (A.any) k_mg_prolong_add_any<<<mg_node_grid(A.g), 256, 0, st>>>(A.g, C.g, A.keep, ec, xf, skip);
+  else k_mg_prolong_add<<<mg_node_grid(A.g), 256, 0, st>>>(A.g, C.g, ec, xf, skip);
+  PCGB_CHECK_LAUNCH();
+  *nl += 1;
+  return PCGB_OK;
 }
 
 // level la's ranked vector -> the global box of level la (replicated on every rank), and back
@@ -1120,9 +1142,7 @@ int mg_vcycle(pcgb_mg_t mg, const double *rin, double *zout, cudaStream_t st, in
       continue;
     }
     double *x = l ? A.x : zout;
-    k_mg_prolong_add<<<mg_node_grid(A.g), 256, 0, st>>>(A.g, C.g, C.x, x, skip);
-    PCGB_CHECK_LAUNCH();
-    *nl += 1;
+    PCGB_TRY(mg_prolong_add(mg, l, C.x, x, st, nl, skip));
     PCGB_TRY(mg_smooth(mg, l, l ? A.b : rin, x, false, false, st, nl, skip));
   }
   return PCGB_OK;
@@ -1576,6 +1596,7 @@ int pcgb_mg_destroy(pcgb_mg_t mg) {
     s->gexec = nullptr;
     s->gkey = {};
   }
+  if (s) s->mgs.erase(std::remove(s->mgs.begin(), s->mgs.end(), mg), s->mgs.end());
   for (size_t l = 0; l < mg->lv.size(); ++l) {
     MgLevel &L = mg->lv[l];
     if (L.has_plan) free_plan(L.P);
@@ -1629,7 +1650,11 @@ int mg_galerkin_level(pcgb_mg_t mg, int l, const double *ke_host) {
   cudaEventCreate(&e0);
   cudaEventCreate(&e1);
   cudaEventRecord(e0, 0);
-  k_mg_galerkin<<<(unsigned)nce, kMgGalerkinThreads>>>(C.nx, C.ny, F.nx, F.ny, mg->ck_fine, l > 1 ? mg->kel : nullptr, kc);
+  const MgLevel &FL = mg->lv[(size_t)l - 1];
+  if (FL.any)
+    k_mg_galerkin_any<<<(unsigned)nce, kMgGalerkinThreads>>>(C.nx, C.ny, F.nx, F.ny, F.nz, FL.keep, mg->ck_fine, l > 1 ? mg->kel : nullptr, kc);
+  else
+    k_mg_galerkin<<<(unsigned)nce, kMgGalerkinThreads>>>(C.nx, C.ny, F.nx, F.ny, mg->ck_fine, l > 1 ? mg->kel : nullptr, kc);
   const cudaError_t le = cudaGetLastError();
   cudaEventRecord(e1, 0);
   const cudaError_t se = cudaEventSynchronize(e1);
@@ -1745,6 +1770,30 @@ void mg_whole_box_levels(std::vector<HexGeom> &geo) {
   }
 }
 
+// whole boxes below geo.back() under the rule of pcgb_mg_create_any: every axis with ne >= 3 becomes (ne + 1) / 2 elements,
+// the others are kept, while some axis has ne >= 3.  keep[l] is the kept-axis mask from level l to l + 1 and any[l] whether
+// that coarsening leaves the even rule (an axis kept or odd).  Stops past max_levels (the caller refuses that depth).
+void mg_any_box_levels(std::vector<HexGeom> &geo, std::vector<int> &keep, std::vector<char> &any, size_t max_levels) {
+  while (geo.size() <= max_levels) {
+    const HexGeom g = geo.back();
+    const int ne[3] = {g.nx, g.ny, g.nz};
+    if (ne[0] <= 2 && ne[1] <= 2 && ne[2] <= 2) break;
+    pcgb_hex_box cb{};
+    int k = 0;
+    bool odd = false;
+    for (int a = 0; a < 3; ++a) {
+      if (ne[a] <= 2) k |= 1 << a;
+      odd = odd || (ne[a] > 2 && ne[a] % 2);
+      cb.ne[a] = ne[a] <= 2 ? ne[a] : (ne[a] + 1) / 2;
+      cb.ng[a] = cb.ne[a];
+      cb.e0[a] = 0;
+    }
+    keep.push_back(k);
+    any.push_back(k != 0 || odd);
+    geo.push_back(hex_geom(&cb));
+  }
+}
+
 // largest global box a multi-rank hierarchy gathers onto every rank
 constexpr int64_t kMgMaxGathered = 1 << 17;
 
@@ -1854,9 +1903,10 @@ int field_bad(int64_t n, const double *d_v, cudaStream_t st, const char *who, in
   return e == cudaSuccess ? PCGB_OK : fail(PCGB_ERR_CUDA, "%s: field check failed: %s", who, cudaGetErrorString(e));
 }
 
-// pcgb_mg_create (d_ck_fine NULL: Ck = E 2^l h on level l) and pcgb_mg_create_field (Galerkin levels from d_ck_fine)
+// pcgb_mg_create (d_ck_fine NULL: Ck = E 2^l h on level l), pcgb_mg_create_field (Galerkin levels from d_ck_fine) and
+// pcgb_mg_create_any (any_rule: the coarsening of mg_any_box_levels, Galerkin levels from d_ck_fine or, NULL, Ck = E h)
 int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, const double *d_ck_fine,
-                  const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out, const char *who) {
+                  const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out, const char *who, bool any_rule = false) {
   PCGB_TRY(require_device());
   if (!s || !box || !ke_host || !d_minv_fine || !out) return fail(PCGB_ERR_ARG, "%s: null argument", who);
   if (s->halo || s->comm) return fail(PCGB_ERR_ARG, "%s: one rank only (the solver has a halo plan or a communicator)", who);
@@ -1868,8 +1918,15 @@ int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_hos
   std::vector<HexGeom> geo{hex_geom(box)};
   if (3 * geo[0].nfree_nodes != s->n) return fail(PCGB_ERR_ARG, "%s: the solver's operator has %lld rows, the box %lld",
                                                   who, (long long)s->n, (long long)(3 * geo[0].nfree_nodes));
-  mg_whole_box_levels(geo);
-  if (geo.size() < 2) return fail(PCGB_ERR_ARG, "%s: the box does not coarsen (every ne must be even and >= 4)", who);
+  std::vector<int> keep;
+  std::vector<char> any;
+  if (any_rule) {
+    mg_any_box_levels(geo, keep, any, PCGB_MG_MAX_LEVELS);
+    if (geo.size() < 2) return fail(PCGB_ERR_ARG, "%s: the box does not coarsen (some ne must be >= 3)", who);
+  } else {
+    mg_whole_box_levels(geo);
+    if (geo.size() < 2) return fail(PCGB_ERR_ARG, "%s: the box does not coarsen (every ne must be even and >= 4)", who);
+  }
   if (3 * geo.back().nfree_nodes > kMgMaxCoarse)
     return fail(PCGB_ERR_ARG, "%s: the coarsest level has %lld dofs (at most %d)", who, (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
   if (geo.size() > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "%s: more than %d levels", who, PCGB_MG_MAX_LEVELS);
@@ -1881,16 +1938,27 @@ int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_hos
     PCGB_TRY(field_bad((int64_t)geo[0].nx * geo[0].ny * geo[0].nz, d_ck_fine, 0, who, &bad));
     if (bad) return fail(PCGB_ERR_ARG, "%s: every Ck of the field must be finite and positive", who);
   }
+  // a uniform box under the any rule: Galerkin levels from Ck = E h on every fine element (freed once the levels exist)
+  double *ck_uniform = nullptr;
+  if (any_rule && !d_ck_fine) {
+    PCGB_CUDA(cudaDeviceSynchronize());
+    const std::vector<double> ckh((size_t)geo[0].nx * geo[0].ny * geo[0].nz, E * h);
+    PCGB_CUDA(upload(&ck_uniform, ckh));
+    d_ck_fine = ck_uniform;
+  }
   pcgb_mg_t mg = new pcgb_mg_s();
   mg->s = s; mg->degree = degree; mg->lo = lo; mg->ck_fine = d_ck_fine;
   mg->lv.resize(geo.size());
   for (size_t l = 0; l < geo.size(); ++l) {
     MgLevel &L = mg->lv[l];
     L.g = geo[l]; L.glev = (int)l; L.place = MgPlace{geo[l], 0, 0, 0};
+    if (l < any.size()) { L.any = any[l] != 0; L.keep = keep[l]; }
   }
   const int rc = mg_build(mg, ke_host, E, h, d_minv_fine, nullptr);
   mg->ck_fine = nullptr;   // the caller's array: not read after create
+  cudaFree(ck_uniform);
   if (rc != PCGB_OK) { pcgb_mg_destroy(mg); return rc; }
+  s->mgs.push_back(mg);
   *out = mg;
   return PCGB_OK;
 }
@@ -1908,6 +1976,20 @@ int pcgb_mg_create_field(pcgb_solver_t s, const pcgb_hex_box *box, const double 
     return fail(PCGB_ERR_ARG, "pcgb_mg_create_field: null argument");
   }
   return mg_create_one(s, box, ke_host, 1.0, 1.0, d_ck_fine, d_minv_fine, degree, lo, out, "pcgb_mg_create_field");
+}
+
+int pcgb_mg_create_any(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine, double E, double h,
+                       const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
+  return mg_create_one(s, box, ke_host, E, h, d_ck_fine, d_minv_fine, degree, lo, out, "pcgb_mg_create_any", true);
+}
+
+int pcgb_mg_level_box(pcgb_mg_t mg, int level, int32_t *ne) {
+  if (!mg || !ne) return fail(PCGB_ERR_ARG, "pcgb_mg_level_box: null argument");
+  if (level < 0 || level >= (int)mg->lv.size())
+    return fail(PCGB_ERR_ARG, "pcgb_mg_level_box: level %d outside 0 .. %d", level, (int)mg->lv.size() - 1);
+  const HexGeom &g = mg->lv[(size_t)level].g;
+  ne[0] = g.nx; ne[1] = g.ny; ne[2] = g.nz;
+  return PCGB_OK;
 }
 
 int pcgb_mg_level_csr(pcgb_mg_t mg, int level, int64_t *d_rowptr, int32_t *d_col, double *d_val, int64_t *nnz, void *stream) {
@@ -2010,6 +2092,7 @@ int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked,
   }
   const int rc = mg_build(mg, ke_host, E, h, d_minv_fine, d_own);
   if (rc != PCGB_OK) { pcgb_mg_destroy(mg); return rc; }
+  s->mgs.push_back(mg);
   *out = mg;
   return PCGB_OK;
 }
@@ -2048,10 +2131,8 @@ int pcgb_mg_prolong_add(pcgb_mg_t mg, int level, const double *d_coarse, double 
   PCGB_TRY(require_device());
   if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || level == mg->la || !d_fine || !d_coarse)
     return fail(PCGB_ERR_ARG, "pcgb_mg_prolong_add: bad argument");
-  const MgLevel &F = mg->lv[(size_t)level], &C = mg->lv[(size_t)level + 1];
-  k_mg_prolong_add<<<mg_node_grid(F.g), 256, 0, (cudaStream_t)stream>>>(F.g, C.g, d_coarse, d_fine, nullptr);
-  PCGB_CHECK_LAUNCH();
-  return PCGB_OK;
+  int nl = 0;
+  return mg_prolong_add(mg, level, d_coarse, d_fine, (cudaStream_t)stream, &nl, nullptr);
 }
 
 int pcgb_mg_smooth(pcgb_mg_t mg, int level, const double *d_b, double *d_x, void *stream) {

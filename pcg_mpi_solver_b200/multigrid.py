@@ -11,6 +11,10 @@ them): every rank halves its own box while all ranks can (`rank_levels`), with o
 level from `hexmesh.interface_lists`; the first level where some rank cannot halve is gathered onto every rank and continues
 as the one-rank hierarchy of its global box.  The global boxes are those of the one-rank preconditioner on the global mesh,
 so it is the same operator up to rounding.
+
+`coarsening="any"` (one rank) accepts a box of any size: every axis is coarsened on its own (`any_levels`), halved to
+(ne + 1) / 2 elements while ne >= 3 and kept once ne <= 2, down to at most 2x2x2 elements, and the coarse levels are always
+Galerkin products of element matrices (pcgb_mg_create_any), with or without `E_field`.
 """
 from __future__ import annotations
 
@@ -34,6 +38,20 @@ def _whole_levels(ne):
     out = [tuple(int(v) for v in ne)]
     while all(v % 2 == 0 and v // 2 >= 2 for v in out[-1]):
         out.append(tuple(v // 2 for v in out[-1]))
+    return out
+
+
+def any_levels(ne, max_levels: int = _lib.MG_MAX_LEVELS) -> list:
+    """Element counts of every level under coarsening="any": an axis with ne >= 3 becomes (ne + 1) / 2 (coarse node j at
+    fine node min(2j, ne)), one with ne <= 2 is kept, while some axis has ne >= 3.  Raises ValueError, as pcgb_mg_create_any
+    refuses, for a box with nothing to coarsen or a hierarchy of more than `max_levels` levels."""
+    out = [tuple(int(v) for v in ne)]
+    while any(v >= 3 for v in out[-1]):
+        out.append(tuple((v + 1) // 2 if v >= 3 else v for v in out[-1]))
+        if len(out) > max_levels:
+            raise ValueError(f"HexMultigrid: the box {tuple(ne)} needs more than {max_levels} levels")
+    if len(out) < 2:
+        raise ValueError(f"HexMultigrid: the box {tuple(ne)} does not coarsen (some ne must be >= 3)")
     return out
 
 
@@ -71,16 +89,22 @@ class HexMultigrid:
     of its interval as a fraction of the estimated largest eigenvalue of D^-1 A (the upper end is 1.1 times it).  minv: the
     fine level's inverse diagonal (op.jacobi() if omitted).
 
-    One rank: block is the whole mesh (e0 = 0, ng = ne, every ne even).  Across ranks (op.comm with 2 or more ranks):
+    One rank: block is the whole mesh (e0 = 0, ng = ne; under the default coarsening="even" every level halves every ne
+    while all are even and the halves stay >= 2, and the coarsest level must have at most 1536 dofs).  Across ranks (op.comm with 2 or more ranks):
     blocks lists every rank's box and block is blocks[op.comm.rank]; construction is collective and refuses (ValueError,
     on every rank alike, before anything is allocated) what `rank_levels` refuses.
 
     E_field (one rank only): the per-element Young's modulus `op` was generated with (hexmesh.generate_matrix / generate_ebe
     with E_field; shape (ne[2], ne[1], ne[0]), float64).  The coarse levels are then Galerkin products of element matrices
-    (pcgb_mg_create_field) instead of rediscretisations with block.E.  With a multi-rank `op` it raises ValueError."""
+    (pcgb_mg_create_field) instead of rediscretisations with block.E.  With a multi-rank `op` it raises ValueError.
+
+    coarsening (one rank only): "even" (the default, above) or "any": a box of any size, each axis halved or kept on its own
+    (`any_levels`), Galerkin levels from E_field or, without it, from Ck = block.E * block.h on every element
+    (pcgb_mg_create_any).  "any" builds 4608 bytes of element matrices per level-1 element during the set-up and sets up
+    slower than the rediscretised default.  Any other string, or "any" with a multi-rank `op`, raises ValueError."""
 
     def __init__(self, op, block: HexBlock, degree: int = 2, lo: float = 0.25, minv: torch.Tensor | None = None, blocks=None,
-                 E_field=None):
+                 E_field=None, coarsening: str = "even"):
         self.op, self.block, self.degree, self.lo = op, block, int(degree), float(lo)
         self.n = op.n
         self.device = op.device
@@ -89,6 +113,22 @@ class HexMultigrid:
         self.levels = None
         comm = getattr(op, "comm", None)
         ranked = comm is not None and comm.nranks > 1
+        if coarsening not in ("even", "any"):
+            raise ValueError(f"HexMultigrid: coarsening must be 'even' or 'any', not {coarsening!r}")
+        self.coarsening = coarsening
+        if coarsening == "any":
+            if ranked:
+                raise ValueError("HexMultigrid: coarsening='any' is supported on one rank only")
+            ck = None if E_field is None else field_ck(E_field, block, self.device)
+            minv = op.jacobi() if minv is None else minv.to(self.device, torch.float64).contiguous()
+            ke = np.ascontiguousarray(hex_element_stiffness(1.0, block.nu))
+            box = block.cbox()
+            with torch.cuda.device(self.device):
+                torch.cuda.synchronize(self.device)
+                _lib.check(_lib.load().pcgb_mg_create_any(op._solver, ctypes.byref(box), ke.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
+                                                          _lib.ptr(ck), float(block.E), float(block.h), _lib.ptr(minv), self.degree,
+                                                          self.lo, ctypes.byref(self._h)), "pcgb_mg_create_any")
+            return
         if E_field is not None:
             if ranked:
                 raise ValueError("HexMultigrid: E_field is supported on one rank only")
@@ -176,10 +216,21 @@ class HexMultigrid:
 
     def setup_info(self) -> dict:
         """galerkin_ms (device time of the Galerkin kernels) and element_matrix_peak_bytes (element matrices held at once
-        during the set-up); both 0 without E_field."""
+        during the set-up); both 0 for the default coarsening without E_field."""
         ms, peak = ctypes.c_double(), ctypes.c_int64()
         _lib.check(_lib.load().pcgb_mg_setup_info(self._h, ctypes.byref(ms), ctypes.byref(peak)), "pcgb_mg_setup_info")
         return {"galerkin_ms": float(ms.value), "element_matrix_peak_bytes": int(peak.value)}
+
+    def level_shapes(self) -> list:
+        """Element counts (nx, ny, nz) of every level (pcgb_mg_level_box); across ranks the rank's boxes up to the gathered
+        level, then the global ones."""
+        lib = _lib.load()
+        ne = (ctypes.c_int32 * 3)()
+        out = []
+        for l in range(self.info()["levels"]):
+            _lib.check(lib.pcgb_mg_level_box(self._h, l, ne), "pcgb_mg_level_box")
+            out.append(tuple(int(v) for v in ne))
+        return out
 
     # ---- the V-cycle's parts (tests; collective across ranks)
     def level_matrix(self, level: int):

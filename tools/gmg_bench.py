@@ -1,6 +1,11 @@
 """Time to solution of Jacobi-PCG against multigrid-preconditioned PCG (HexMultigrid) on the bench's hex box.
 
     python tools/gmg_bench.py --block 128 --tol 1e-8 [--operator csr|ebe_ordered|ebe] [--repeats 3]
+    python tools/gmg_bench.py --shape 200,150,75 --coarsening any
+
+--shape NX,NY,NZ replaces the cubic --block box (h = 1 / NX); --coarsening any builds HexMultigrid(coarsening="any"), which
+accepts any box.  Either option adds the level boxes, the Galerkin kernels' device time and the element-matrix peak of
+`setup_info` to the multigrid line; without them the output is unchanged.
 
 For each arm: iterations, flag, the device time of the loop (CUDA events inside the solve), the host wall time of the whole
 solve (ending in a device synchronise), and for the multigrid arm its set-up time, the V-cycle time per application
@@ -37,7 +42,13 @@ def main():
     ap.add_argument("--degree", type=int, default=2)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--vcycles", type=int, default=50)
+    ap.add_argument("--coarsening", choices=["even", "any"], default="even")
+    ap.add_argument("--shape", type=str, default=None, help="NX,NY,NZ (instead of --block)")
     a = ap.parse_args()
+    shape = tuple(int(v) for v in a.shape.split(",")) if a.shape else (a.block,) * 3
+    if len(shape) != 3 or min(shape) < 1:
+        sys.exit("gmg_bench: --shape needs three positive element counts")
+    extra = a.shape is not None or a.coarsening != "even"
     import torch
     if not torch.cuda.is_available():
         sys.exit("gmg_bench: needs a CUDA device")
@@ -46,7 +57,7 @@ def main():
     from pcg_mpi_solver_b200.solver import SubdomainOperator
     dev = torch.device("cuda:0")
     B = a.block
-    blk = HexBlock((B, B, B), (0, 0, 0), (B, B, B), h=1.0 / B)
+    blk = HexBlock(shape, (0, 0, 0), shape, h=1.0 / shape[0])
     if a.operator == "csr":
         A = generate_matrix(blk, device=dev)
         op_bytes = A.val.numel() * 12 + A.rowptr.numel() * A.rowptr.element_size()
@@ -60,7 +71,7 @@ def main():
     torch.cuda.empty_cache()
     free0, _ = torch.cuda.mem_get_info(dev)
     t0 = time.perf_counter()
-    mg = HexMultigrid(op, blk, degree=a.degree, minv=minv)
+    mg = HexMultigrid(op, blk, degree=a.degree, minv=minv, coarsening=a.coarsening)
     torch.cuda.synchronize()
     setup_s = time.perf_counter() - t0
     free_drop = free0 - torch.cuda.mem_get_info(dev)[0]    # everything create took, the SpMV plans' tables included
@@ -94,6 +105,8 @@ def main():
     vc_ms = e0.elapsed_time(e1) / a.vcycles
     diff = float((xm - xj).norm() / xj.norm())
     common = {"block": B, "operator": a.operator, "tol": a.tol, "card": card()}
+    if extra:
+        common = {"shape": list(shape), "coarsening": a.coarsening, "operator": a.operator, "tol": a.tol, "card": card()}
     print(json.dumps({**common, "arm": "jacobi", "flag": ij.flag, "iters": ij.iters, "loop_ms": round(ij.loop_ms, 3),
                       "wall_s": round(wj, 4), "ms_per_iter": round(ij.loop_ms / max(ij.loop_iters, 1), 4)}))
     print(json.dumps({**common, "arm": "multigrid", "flag": im.flag, "iters": im.iters, "loop_ms": round(im.loop_ms, 3),
@@ -101,7 +114,8 @@ def main():
                       "vcycle_ms": round(vc_ms, 4), "setup_s": round(setup_s, 3), "degree": a.degree, "levels": info["levels"],
                       "n_levels": info["n"], "lambda": [round(v, 4) for v in info["lambda"]], "hierarchy_bytes": info["bytes"], "device_free_drop_bytes": free_drop,
                       "fine_operator_bytes": op_bytes, "speedup_wall": round(wj / wm, 2),
-                      "x_rel_diff_vs_jacobi": diff}))
+                      "x_rel_diff_vs_jacobi": diff,
+                      **({"level_shapes": [list(v) for v in mg.level_shapes()], **mg.setup_info()} if extra else {})}))
 
 
 if __name__ == "__main__":
