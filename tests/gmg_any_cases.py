@@ -170,6 +170,17 @@ class HostAnyMultigrid(G.HostMultigrid):
         return x[0]
 
 
+def uniform_field(ne, E=1.0):
+    """The field of a uniform box of modulus E: what pcgb_mg_create_any builds without one (Ck = E h per element)."""
+    return np.full((ne[2], ne[1], ne[0]), float(E))
+
+
+# boxes whose Galerkin coarsest matrix at gmg_cases.BAD_NU has a negative eigenvalue (pinned in test_gmg_galerkin_cpu.py):
+# the field path on a random field of BAD_NU_FIELD_BOX, the any rule on BAD_NU_ANY_BOX uniform and with a random field;
+# the fields are voxel_cases.random_field(box, seed=sum(box))
+BAD_NU_FIELD_BOX, BAD_NU_ANY_BOX = (8, 8, 8), (9, 7, 5)
+
+
 def field_of(ne, contrast, seed=0):
     """The test field of a box: uniform 1 at contrast 1, else V.two_phase (inclusions of modulus `contrast`)."""
     if contrast == 1:

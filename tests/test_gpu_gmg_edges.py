@@ -302,12 +302,15 @@ def _fma_close(got, a, b, c):
 
 
 def _check_mg_steps(cuda, kind, w, x0, K, seed):
+    """_check_mg_steps_on the 8^3 box's operator of `kind` and its default preconditioner."""
+    blk, op, mg = _setup(cuda, (8, 8, 8), kind)
+    _check_mg_steps_on(cuda, op, mg, kind != "ebe", w, x0, K, seed, kind)
+
+
+def _check_mg_steps_on(cuda, op, mg, exact, w, x0, K, seed, label):
     """Runs maxiter = k = 1..K with fixed_iters: p of iteration 0 is M b bit for bit (without x0), p of every later
-    iteration is fma(beta, p, M r) of the previous run's snapshot, each record's rz is sum z r w and its #inf exact.  The
-    atomic EBE operator (not bit-reproducible) gets the same identities to a tolerance."""
-    ne = (8, 8, 8)
-    blk, op, mg = _setup(cuda, ne, kind)
-    exact = kind != "ebe"
+    iteration is fma(beta, p, M r) of the previous run's snapshot, each record's rz is sum z r w and its #inf exact.  An
+    operator that is not bit-reproducible (exact False: the atomic EBE) gets the same identities to a tolerance."""
     rng = np.random.default_rng(seed)
     n = mg.n
     b = rng.standard_normal(n)
@@ -340,7 +343,7 @@ def _check_mg_steps(cuda, kind, w, x0, K, seed):
         t = z.astype(LD) * (r.astype(LD) * wn.astype(LD))
         mag = float(np.abs(t).sum())
         dev = abs(LD(rec["inp"][S.RZ]) - t.sum())
-        _stat(f"MG-PCG rz / sum|terms| {kind}", float(dev) / mag)
+        _stat(f"MG-PCG rz / sum|terms| {label}", float(dev) / mag)
         assert dev <= ((n + 2) * EPS if exact else 1e-12) * mag, (k, float(dev) / mag)
         assert float(rec["inp"][S.NINF]) == float((~np.isfinite(z)).sum())
         prev = {"p": p, "r": r}
