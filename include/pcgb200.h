@@ -35,6 +35,7 @@ typedef struct pcgb_ebe_s *pcgb_ebe_t;     /* opt-in matrix-free element-by-elem
 typedef struct pcgb_asm_s *pcgb_asm_t;     /* device assembly of K_i[Eff,Eff] from the pattern groups (symbolic phase state) */
 typedef struct pcgb_ebe2_s *pcgb_ebe2_t;   /* coloured (atomics-free, bit-reproducible) variant of the EBE operator */
 typedef struct pcgb_ebe_ordered_s *pcgb_ebe_ordered_t; /* EBE operator with a fixed summation order (bit-reproducible, solver-ready) */
+typedef struct pcgb_hexop_s *pcgb_hexop_t; /* index-free matrix-free operator of a hex box (the ordered operator's bits) */
 typedef struct pcgb_mg_s *pcgb_mg_t;       /* geometric multigrid preconditioner of a hex-box solver (one V-cycle) */
 
 /* error codes */
@@ -311,6 +312,31 @@ int pcgb_hex_fill_field(const pcgb_hex_box *box, const double *ke_host, const do
 /* The same check of d_ck on its own (PCGB_ERR_ARG for an entry that is not finite and positive; synchronises `stream`), so
  * a caller can refuse a field before it allocates the CSR arrays. */
 int pcgb_hex_field_check(const pcgb_hex_box *box, const double *d_ck, void *stream);
+
+/* ---------------------------------------------------------------- opt-in: index-free matrix-free operator of a hex box
+ * y = K_i x of `box` (the pcgb_hex_* numbering, no interface sum) with every index computed from the node's coordinates:
+ * no index list, slot buffer, position list or atomics.  Bit-identical to pcgb_ebe_ordered_create on the box's single
+ * pattern group (Ke, Ck per element in the order of pcgb_hex_fill_field): for free dof (node, d)
+ *   y = 0.0;  for la = 0..7 ascending with element e = node - (la&1, la>>1&1, la>>2&1) inside the box:
+ *             acc = 0.0;  for b = 0..23: acc = fma(Ke[3 la + d][b], Ck_e * x_b, acc)   (x_b = 0.0 for a clamped node);
+ *             y = y + acc
+ * (calcMatVecProd, pcg_solver.py:263-300, in np.bincount's order).  Ck_e = ck, or d_ck[e] when d_ck is not NULL (device,
+ * ne[0]*ne[1]*ne[2] doubles, caller-owned: it must outlive the handle).  ke_host (24x24, row-major) is copied into the
+ * handle and passed with every launch, so no other operator or generator can change it.
+ * pcgb_hexop_create refuses with PCGB_ERR_ARG, holding no device memory: a box with some ne <= 0 or outside its global
+ * mesh, a uniform ck that is not finite and positive, a field entry that is not (checked on the device after a device
+ * synchronise).  The handle itself holds no device memory.
+ * pcgb_hexop_apply refuses overlapping x and y (each y is computed from x around it).  pcgb_hexop_diag writes the
+ * diagonal d = 0.0 + Ck_e Ke[3la+d][3la+d] + ... in ascending la (pcg_solver.py:282-287, np.bincount's order).
+ * pcgb_hexop_bytes: algorithmic bytes per application (x and y once, 8 per element with a field). */
+int pcgb_hexop_create(const pcgb_hex_box *box, const double *ke_host, double ck, const double *d_ck /* NULL = uniform */,
+                      pcgb_hexop_t *out);
+int pcgb_hexop_destroy(pcgb_hexop_t H);
+int pcgb_hexop_apply(pcgb_hexop_t H, const double *d_x, double *d_y, void *stream);
+int pcgb_hexop_diag(pcgb_hexop_t H, double *d_diag, void *stream);
+int64_t pcgb_hexop_bytes(pcgb_hexop_t H);
+int pcgb_solver_create_hexop(pcgb_hexop_t H, pcgb_halo_t halo /* may be NULL */, pcgb_comm_t comm /* may be NULL */,
+                             pcgb_solver_t *out);
 
 /* ---------------------------------------------------------------- opt-in: geometric multigrid preconditioner (hex boxes)
  * z = M r is one symmetric V-cycle over nested hex boxes (across ranks: pcgb_mg_create_ranks below), for a one-rank solver whose operator (CSR, EBE or ordered EBE) is

@@ -129,6 +129,12 @@ SIGNATURES = {
     "pcgb_hex_fill": (c_int, [POINTER(HexBox), POINTER(c_double), c_double, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcgb_hex_field_check": (c_int, [POINTER(HexBox), c_void_p, c_void_p]),
     "pcgb_hex_fill_field": (c_int, [POINTER(HexBox), POINTER(c_double), c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcgb_hexop_create": (c_int, [POINTER(HexBox), POINTER(c_double), c_double, c_void_p, POINTER(c_void_p)]),
+    "pcgb_hexop_destroy": (c_int, [c_void_p]),
+    "pcgb_hexop_apply": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcgb_hexop_diag": (c_int, [c_void_p, c_void_p, c_void_p]),
+    "pcgb_hexop_bytes": (c_int64, [c_void_p]),
+    "pcgb_solver_create_hexop": (c_int, [c_void_p, c_void_p, c_void_p, POINTER(c_void_p)]),
 }
 
 _lib = None

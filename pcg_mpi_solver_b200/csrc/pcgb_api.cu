@@ -15,6 +15,7 @@
 #include "assemble.cuh"
 #include "ebe_ordered.cuh"
 #include "gmg.cuh"
+#include "hexop.cuh"
 
 using namespace pcgb;
 
@@ -41,6 +42,10 @@ struct pcgb_ebe_ordered_s {
   int device = 0;
 };
 
+struct pcgb_hexop_s {
+  HexOp H;
+};
+
 // What may differ between two solves on one handle and changes the captured iterations (the operator, the x buffers and
 // PCGB_FORK are fixed when the solver is created).
 struct GraphKey {
@@ -63,11 +68,13 @@ struct FineOp {
   pcgb_csr_t A = nullptr;
   pcgb_ebe_t E = nullptr;           // opt-in matrix-free operator
   pcgb_ebe_ordered_t O = nullptr;   // opt-in matrix-free operator with a fixed summation order
-  int64_t rows() const { return A ? A->P.nrows : E ? E->P.n : O->O.P.n; }
+  pcgb_hexop_t H = nullptr;         // opt-in index-free operator of a hex box (the ordered operator's bits)
+  int64_t rows() const { return A ? A->P.nrows : E ? E->P.n : O ? O->O.P.n : H->H.n; }
   // y = K x, without the interface sum
   int apply(const double *x, double *y, cudaStream_t st, int *nl, const int *skip) const {
     if (E) return ebe_apply(E->P, x, y, st, nl, skip);
     if (O) return ebo_apply(O->O, x, y, st, nl, skip);
+    if (H) return hexop_apply(H->H, x, y, st, nl, skip);
     return spmv_launch(A->P, x, y, false, st, nl, skip);
   }
 };
@@ -873,6 +880,12 @@ int pcgb_solver_create_ebe(pcgb_ebe_t E, pcgb_halo_t halo, pcgb_comm_t comm, pcg
 int pcgb_solver_create_ebe_ordered(pcgb_ebe_ordered_t O, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
   if (!O || !out) return fail(PCGB_ERR_ARG, "pcgb_solver_create_ebe_ordered: null argument");
   return solver_create_common(FineOp{nullptr, nullptr, O}, halo, comm, out);
+}
+
+// the index-free hex-box operator (pcg_solver.py:263-300 in the ordered operator's order)
+int pcgb_solver_create_hexop(pcgb_hexop_t H, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
+  if (!H || !out) return fail(PCGB_ERR_ARG, "pcgb_solver_create_hexop: null argument");
+  return solver_create_common(FineOp{nullptr, nullptr, nullptr, H}, halo, comm, out);
 }
 
 int pcgb_solver_destroy(pcgb_solver_t s) {
@@ -2234,5 +2247,60 @@ int pcgb_hex_fill_field(const pcgb_hex_box *box, const double *ke_host, const do
   PCGB_CHECK_LAUNCH();
   return PCGB_OK;
 }
+
+// ------------------------------------------------------------------------------------ index-free hex-box operator
+// calcMatVecProd (pcg_solver.py:263-300) on a structured box, every index computed from the node's coordinates; the
+// product and the diagonal (updatePreconditioner, :282-287) are bit-identical to the ordered EBE operator's on
+// hexmesh.hex_type_group(box).
+int pcgb_hexop_create(const pcgb_hex_box *box, const double *ke_host, double ck, const double *d_ck, pcgb_hexop_t *out) {
+  if (!box || !ke_host || !out) return fail(PCGB_ERR_ARG, "pcgb_hexop_create: null argument");
+  *out = nullptr;
+  for (int a = 0; a < 3; ++a)
+    if (box->ne[a] <= 0 || box->e0[a] < 0 || (int64_t)box->e0[a] + box->ne[a] > box->ng[a])
+      return fail(PCGB_ERR_ARG, "pcgb_hexop_create: the box must have ne > 0 and lie inside its global mesh on every axis");
+  if (!d_ck && !(std::isfinite(ck) && ck > 0.0)) return fail(PCGB_ERR_ARG, "pcgb_hexop_create: Ck must be finite and positive");
+  PCGB_TRY(require_device());
+  HexOp H;
+  H.s = hexop_shape(hex_geom(box));
+  const HexGeom &g = H.s.g;
+  if ((int64_t)H.s.nbx * H.s.nby * H.s.nbz >= (int64_t)1 << 31) return fail(PCGB_ERR_ARG, "pcgb_hexop_create: box too large");
+  const int64_t ne = (int64_t)g.nx * g.ny * g.nz;
+  if (d_ck) {
+    // the check runs on the legacy stream, which does not wait for non-blocking streams: finish the caller's writes first
+    PCGB_CUDA(cudaDeviceSynchronize());
+    int bad = 0;
+    PCGB_TRY(field_bad(ne, d_ck, 0, "pcgb_hexop_create", &bad));
+    if (bad) return fail(PCGB_ERR_ARG, "pcgb_hexop_create: every Ck of the field must be finite and positive");
+  }
+  std::memcpy(H.ke.k, ke_host, sizeof(H.ke.k));
+  for (int a = 0; a < 24; ++a) H.kd.k[a] = ke_host[a * 24 + a];
+  H.ck = d_ck ? 0.0 : ck;
+  H.d_ck = d_ck;
+  H.n = 3 * g.nfree_nodes;
+  H.bytes = 16 * H.n + (d_ck ? 8 * ne : 0);
+  pcgb_hexop_t h = new pcgb_hexop_s();
+  h->H = H;
+  *out = h;
+  return PCGB_OK;
+}
+
+int pcgb_hexop_destroy(pcgb_hexop_t H) {
+  delete H;
+  return PCGB_OK;
+}
+
+int pcgb_hexop_apply(pcgb_hexop_t H, const double *d_x, double *d_y, void *stream) {
+  if (!H || !d_x || !d_y) return fail(PCGB_ERR_ARG, "pcgb_hexop_apply: null argument");
+  const uintptr_t x0 = (uintptr_t)d_x, y0 = (uintptr_t)d_y, nb = (uintptr_t)H->H.n * sizeof(double);
+  if (x0 < y0 + nb && y0 < x0 + nb) return fail(PCGB_ERR_ARG, "pcgb_hexop_apply: x and y overlap (each y is written from x around it)");
+  return hexop_apply(H->H, d_x, d_y, (cudaStream_t)stream);
+}
+
+int pcgb_hexop_diag(pcgb_hexop_t H, double *d_diag, void *stream) {
+  if (!H || !d_diag) return fail(PCGB_ERR_ARG, "pcgb_hexop_diag: null argument");
+  return hexop_diag(H->H, d_diag, (cudaStream_t)stream);
+}
+
+int64_t pcgb_hexop_bytes(pcgb_hexop_t H) { return H ? H->H.bytes : 0; }
 
 }  // extern "C"

@@ -212,6 +212,14 @@ def generate_ebe(block: HexBlock, device="cuda", ordered: bool = False, E_field=
     return (EbeMatrixOrdered if ordered else EbeMatrix)([grp], eff, ndof, device=device)
 
 
+def generate_box_operator(block: HexBlock, device="cuda", E_field=None):
+    """The same box as the index-free matrix-free operator (hexop.HexBoxOperator): the products and the diagonal of
+    generate_ebe(block, ordered=True, E_field=E_field) bit for bit, with no index arrays on the device.  E_field: as in
+    generate_matrix."""
+    from .hexop import HexBoxOperator
+    return HexBoxOperator(block, device=device, E_field=E_field)
+
+
 def hex_mdf_model(ng, E: float = 1.0, nu: float = 0.3, h: float | None = None, traction: float = 1.0, E_field=None):
     """The structured hex problem as an in-memory `MdfModel` (the reference's model-definition schema, SURVEY
     Appendix A) so that the general pipeline - `partition_mesh(model, nparts)` with METIS, the subdomain builder,

@@ -234,10 +234,13 @@ class SubdomainOperator:
                 # every rank builds a plan (also one without neighbours): the peer-transport import is collective
                 self._halo = make_halo(comm, self.nbr_ranks, self.ovrlp, self.n)
             from .ebe import EbeMatrixOrdered
+            from .hexop import HexBoxOperator
             if isinstance(A, CsrMatrix):
                 create = lib.pcgb_solver_create
             elif isinstance(A, EbeMatrixOrdered):                       # matrix-free, fixed summation order
                 create = lib.pcgb_solver_create_ebe_ordered
+            elif isinstance(A, HexBoxOperator):                         # index-free, the ordered operator's bits
+                create = lib.pcgb_solver_create_hexop
             else:                                                      # EbeMatrix: opt-in matrix-free operator
                 create = lib.pcgb_solver_create_ebe
             _lib.check(create(A.handle, self._halo if self._halo else None,
