@@ -93,6 +93,10 @@ int pcgb_csr_plan_info(pcgb_csr_t A, int64_t info[16]);
  * outweigh the per-CTA dictionary loads; PCGB_SPMV_VDICT=0 disables it, =2 drops the size condition.  d_val is still
  * read by pcgb_csr_diag and must stay allocated. */
 int pcgb_csr_value_dict(pcgb_csr_t A);
+/* With a dictionary, the index stream holds per tile a list of at most 8 segments of consecutive nodes.  In a run segment
+ * every node has the blocks of the one before it, 3 staged x entries further on with the same ids, and only the head's
+ * block words are stored.  Returns the share of the nodes that lie in run segments (0 without a dictionary). */
+double pcgb_csr_run_share(pcgb_csr_t A);
 
 /* ---------------------------------------------------------------- vector kernels (a4-a10)
  * out[0] = sum_i a[i]*b[i]*w[i]   (w may be NULL = all ones).  np.dot(a, b*w) of

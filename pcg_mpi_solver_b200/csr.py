@@ -87,6 +87,11 @@ class CsrMatrix:
         """Distinct 3x3 blocks in the node-block kernel's value dictionary (0: the kernel streams the values)."""
         return int(_lib.load().pcgb_csr_value_dict(self._h))
 
+    def value_dict_run_share(self) -> float:
+        """Share of the nodes whose blocks the dictionary kernel reads through the head of a run (consecutive nodes of a
+        tile with the same blocks shifted by one node: a structured mesh along x); 0.0 without a dictionary."""
+        return float(_lib.load().pcgb_csr_run_share(self._h))
+
     def release_col(self) -> bool:
         """Free the 4-byte column array when the selected SpMV kernel does not read it (the persistent staged-x kernel
         streams its own 16-bit indices): 2 GB at 128^3, 16 GB at 256^3.  The diagonal is cached first.  Returns True

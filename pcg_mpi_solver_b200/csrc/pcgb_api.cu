@@ -264,19 +264,26 @@ int64_t pcgb_spmv_bytes(pcgb_csr_t A) {
 }
 
 /* bytes the selected kernel actually streams from HBM per SpMV: values 8 B per non-zero + the index stream
- * (4 B columns for the L1-gather kernel, 2 B staged positions, or 2/3 B with the column-triple index) + row offsets,
- * x, y and the tile / window tables.  With a value dictionary the values are a second 2 B per 3x3 block (the ids) and
- * the dictionary, which every resident CTA loads once. */
+ * (4 B columns for the L1-gather kernel, 2 B staged positions, 2/3 B with the column-triple index, or 2/9 B per 3x3
+ * block) + row offsets, x, y and the tile / window tables.  With a value dictionary the values are the dictionary, which
+ * every resident CTA loads once, and the index stream is the run-compressed block words (4 B each) + 8 B per tile. */
 int64_t pcgb_spmv_stream_bytes(pcgb_csr_t A) {
   if (!A) return 0;
   const CsrPlan &P = A->P;
-  const int64_t val_bytes = P.vd ? 72 * (int64_t)P.vd * P.grid_persist + (2 * P.nnz) / 9 : 8 * P.nnz;
-  const int64_t idx_bytes = P.bsr ? (2 * P.nnz) / 9 : (P.persist && P.t3) ? (2 * P.nnz) / 3 : (P.staged ? 2 * P.nnz : 4 * P.nnz);
+  const int64_t val_bytes = P.vd ? 72 * (int64_t)P.vd * P.grid_persist : 8 * P.nnz;
+  const int64_t idx_bytes = P.vd ? 4 * P.nvwords + 8 * (int64_t)P.ntiles
+                                 : P.bsr ? (2 * P.nnz) / 9 : (P.persist && P.t3) ? (2 * P.nnz) / 3 : (P.staged ? 2 * P.nnz : 4 * P.nnz);
   return val_bytes + idx_bytes + (P.rp64 ? 8 : 4) * (P.nrows + 1) + 8 * P.ncols + 8 * P.nrows +
          (P.staged ? 8 * P.nwin + 8 * (int64_t)P.ntiles : 0) + (P.persist ? 32 : 12) * (int64_t)P.ntiles;
 }
 
 int pcgb_csr_value_dict(pcgb_csr_t A) { return A ? A->P.vd : 0; }
+
+/* share of the nodes whose blocks the dictionary kernel reads through a run head (0 without a dictionary) */
+double pcgb_csr_run_share(pcgb_csr_t A) {
+  if (!A || A->P.vd == 0 || A->P.nrows < 3) return 0.0;
+  return (double)A->P.run_nodes / (double)(A->P.nrows / 3);
+}
 
 int pcgb_csr_plan_info(pcgb_csr_t A, int64_t info[16]) {
   if (!A || !info) return fail(PCGB_ERR_ARG, "pcgb_csr_plan_info: null argument");

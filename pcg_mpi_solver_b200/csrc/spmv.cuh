@@ -83,9 +83,16 @@ struct CsrPlan {
   // value dictionary of the node-block kernel: when the matrix has few bitwise-distinct 3x3 blocks (a structured mesh of
   // one element type), each is stored once and every block position streams a 16-bit id instead of its 72 bytes of values
   int vd = 0;                      // distinct blocks D (0: no dictionary, the kernel streams val)
-  uint16_t *bvid = nullptr;        // [nnz/9 + 16]  dictionary id of the block at bidx's position
+  uint16_t *bvid = nullptr;        // [nnz/9 + 16]  dictionary id of the block at bidx's position (plan time only)
   double *vdict = nullptr;         // [vd * 9]      the blocks, row-major
   int bsr_group = 0;               // tiles a CTA consumes between two barriers (k_spmv_bsr3_vd: one warp per tile)
+  // index stream of k_spmv_bsr3_vd: per tile a segment list, then block words (staged position | id << 16); a run segment
+  // (nodes whose blocks sit 3 staged doubles further on than their predecessor's, with the same ids) stores only its head
+  uint32_t *vwords = nullptr;      // [nvwords + 8]
+  int64_t *vtoff = nullptr;        // [ntiles + 1]  first word of each tile, by tile id
+  int64_t nvwords = 0, run_nodes = 0;
+  int cap_words = 0;               // words of the largest tile slice (16-byte aligned window)
+  int *split_tile = nullptr;       // [ntiles]  tile id of desc_split[k]
   // interface-first split (multi-GPU overlap): tiles that own an interface row are listed first in desc_split
   struct TileDesc *desc_split = nullptr;  // [ntiles] permutation of tile_desc
   int nb_tiles = 0;                       // leading boundary tiles of desc_split
@@ -813,30 +820,32 @@ __device__ __forceinline__ void block3_rows(const double *pv, int L, double x0, 
 }
 
 // stage of the node-block ring: sval[cap_nnz] f64 | sx[cap_x] f64 | snp[cap_nodes+2] i64 | sbidx[cap_blocks+16] u16 | meta[8] i32
-//                         VD:                      sx[cap_x] f64 | snp[cap_nodes+2] i64 | sbidx[cap_blocks+16] u16 | svid[cap_blocks+16] u16 | meta
+//                         VD:                      sx[cap_x] f64 | snp[cap_nodes+2] i64 | swords[cap_words] u32        | meta
 struct Bsr3Stage {
-  size_t off_sx, off_snp, off_sb, off_sv, off_meta;
+  size_t off_sx, off_snp, off_sb, off_meta;
 };
 template <bool VD>
-__device__ __forceinline__ Bsr3Stage bsr3_stage(int cap_nnz, int cap_x, int cap_nodes, int cap_blocks) {
-  const size_t sb_bytes = ((size_t)(cap_blocks + 16) * 2 + 15) & ~(size_t)15;
+__device__ __forceinline__ Bsr3Stage bsr3_stage(int cap_nnz, int cap_x, int cap_nodes, int cap_idx) {
+  // cap_idx: block indices (u16) of a tile, or VD: words (u32) of a tile's slice of the run-compressed stream
+  const size_t sb_bytes = VD ? (size_t)cap_idx * 4 : ((size_t)(cap_idx + 16) * 2 + 15) & ~(size_t)15;
   Bsr3Stage L;
   L.off_sx = VD ? 0 : (size_t)cap_nnz * 8;
   L.off_snp = L.off_sx + (size_t)cap_x * 8;
   L.off_sb = L.off_snp + (size_t)(cap_nodes + 2) * 8;
-  L.off_sv = L.off_sb + sb_bytes;
-  L.off_meta = L.off_sb + (VD ? 2 : 1) * sb_bytes;
+  L.off_meta = L.off_sb + sb_bytes;
   return L;
 }
 
-// producer warp p of nprod (tiles it = p, p + nprod, ...; stage it % stages, stages % nprod == 0): TMA val (VD: the block
-// ids) + block indices, cp.async node offsets + x windows.  The descriptor and the window descriptors of the NEXT tile
-// are fetched while the current one is being issued.
+// producer warp p of nprod (tiles it = p, p + nprod, ...; stage it % stages, stages % nprod == 0): TMA val + block indices
+// (VD: the tile's slice of the word stream, found through the tile id: tile_ids[k] for a permuted descriptor list, else k),
+// cp.async node offsets + x windows.  The descriptor and the window descriptors of the NEXT tile are fetched while the
+// current one is being issued.
 template <bool VD, typename RP>
 __device__ __forceinline__ void bsr3_produce(int p, int nprod, unsigned char *smem_raw, const Bsr3Stage &SL, int stages,
                                              int stage_bytes, uint64_t *full_bar, uint64_t *empty_bar,
                                              const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx,
-                                             const double *__restrict__ val, const uint16_t *__restrict__ bvid,
+                                             const double *__restrict__ val, const uint32_t *__restrict__ vwords,
+                                             const int64_t *__restrict__ vtoff, const int *__restrict__ tile_ids,
                                              const double *__restrict__ x, const TileDesc *__restrict__ desc,
                                              const int *__restrict__ win_start, const int *__restrict__ win_off, int ntiles,
                                              int64_t nnz) {
@@ -847,10 +856,16 @@ __device__ __forceinline__ void bsr3_produce(int p, int nprod, unsigned char *sm
   bool have = tile < ntiles;
   int4 d0 = make_int4(0, 0, 0, 0), d1 = make_int4(0, 0, 0, 0);
   int ws = 0, wo = 0;
+  int64_t vw0 = 0, vw1 = 0;   // VD: word range of the tile
+  auto word_range = [&](int k, int64_t &a, int64_t &b) {
+    const int g = tile_ids != nullptr ? __ldg(tile_ids + k) : k;
+    a = __ldg(vtoff + g); b = __ldg(vtoff + g + 1);
+  };
   if (have) {
     const int4 *dp = reinterpret_cast<const int4 *>(desc + tile);
     d0 = __ldg(dp); d1 = __ldg(dp + 1);
     if (lane < d1.z) { ws = __ldg(win_start + d1.y + lane); wo = __ldg(win_off + d1.y + lane); }
+    if (VD) word_range(tile, vw0, vw1);
   }
   while (have) {
     const int s = it % stages;
@@ -859,9 +874,11 @@ __device__ __forceinline__ void bsr3_produce(int p, int nprod, unsigned char *sm
     const int ntile = blockIdx.x + nit * gridDim.x;
     const bool nhave = ntile < ntiles;
     int4 nd0 = make_int4(0, 0, 0, 0), nd1 = make_int4(0, 0, 0, 0);
+    int64_t nvw0 = 0, nvw1 = 0;
     if (nhave) {
       const int4 *dp = reinterpret_cast<const int4 *>(desc + ntile);
       nd0 = __ldg(dp); nd1 = __ldg(dp + 1);
+      if (VD) word_range(ntile, nvw0, nvw1);
     }
     const int64_t k0 = ((int64_t)(uint32_t)d0.x) | ((int64_t)d0.y << 32);
     const int cnt = d0.z, r0 = d0.w, R = d1.x & 0x3fffffff, uni = (d1.x >> 30) & 1, wb = d1.y, nw = d1.z, xlen = d1.w;
@@ -875,16 +892,17 @@ __device__ __forceinline__ void bsr3_produce(int p, int nprod, unsigned char *sm
     const int64_t ka = k0 & ~(int64_t)kAlignMask;
     mbar_wait(&empty_bar[s], ph ^ 1u);
     if (lane == 0) {
-      // bidx (and bvid) are padded by 16 entries: the aligned window [ba, bend) never leaves the array
+      // bidx is padded by 16 entries, vwords by 8: the aligned windows [ba, bend) and [wa, wend) never leave the arrays
       const int64_t b0 = k0 / 9, ba = b0 & ~(int64_t)kAlignMask;
       const int64_t bend = (b0 + cnt / 9 + kAlignMask) & ~(int64_t)kAlignMask;
       const uint32_t ib = (uint32_t)(bend - ba) * 2u;
+      int sofs = (int)(b0 - ba);
       if (VD) {
-        mbar_expect_tx(&full_bar[s], 2u * ib);
-        if (ib > 0) {
-          bulk_g2s(sb, bidx + ba, ib, &full_bar[s], pol);
-          bulk_g2s(base + SL.off_sv, bvid + ba, ib, &full_bar[s], pol);
-        }
+        const int64_t wa = vw0 & ~(int64_t)3, wend = (vw1 + 3) & ~(int64_t)3;   // every tile has a header word: wend > wa
+        const uint32_t wb = (uint32_t)(wend - wa) * 4u;
+        sofs = (int)(vw0 - wa);
+        mbar_expect_tx(&full_bar[s], wb);
+        bulk_g2s(sb, vwords + wa, wb, &full_bar[s], pol);
       } else {
         int64_t kend = (k1 + kAlignMask) & ~(int64_t)kAlignMask;
         const int64_t lim = nnz & ~(int64_t)kAlignMask;
@@ -895,7 +913,7 @@ __device__ __forceinline__ void bsr3_produce(int p, int nprod, unsigned char *sm
         if (ib > 0) bulk_g2s(sb, bidx + ba, ib, &full_bar[s], pol);
       }
       meta[0] = r0; meta[1] = R; meta[2] = tile; meta[3] = cnt;
-      meta[4] = (int)(k0 & 0xffffffff); meta[5] = (int)(k0 >> 32); meta[6] = (int)(b0 - ba); meta[7] = uni;
+      meta[4] = (int)(k0 & 0xffffffff); meta[5] = (int)(k0 >> 32); meta[6] = sofs; meta[7] = uni;
     }
     if (!VD) {
       const int64_t lim = nnz & ~(int64_t)kAlignMask;
@@ -923,7 +941,7 @@ __device__ __forceinline__ void bsr3_produce(int p, int nprod, unsigned char *sm
     cp_async_arrive_noinc(&full_bar[s]);
     __syncwarp();
     if (lane == 0) mbar_arrive(&full_bar[s]);
-    d0 = nd0; d1 = nd1; ws = nws; wo = nwo; it = nit; tile = ntile; have = nhave;
+    d0 = nd0; d1 = nd1; ws = nws; wo = nwo; vw0 = nvw0; vw1 = nvw1; it = nit; tile = ntile; have = nhave;
   }
 }
 
@@ -961,7 +979,7 @@ k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, co
 
   if (warp >= CW) {
     bsr3_produce<false, RP>(warp - CW, nprod, smem_raw, SL, stages, stage_bytes, full_bar, empty_bar, rowptr, bidx, val, nullptr,
-                            x, desc, win_start, win_off, ntiles, nnz);
+                            nullptr, nullptr, x, desc, win_start, win_off, ntiles, nnz);
     return;
   }
 
@@ -1066,17 +1084,19 @@ k_spmv_bsr3(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, co
 //     phase B   after ONE named barrier per group, the tiles of the group in tile order, thread r < R of the NT = CW * 32
 //               consumer threads storing row r and adding x.y as k_spmv_bsr3's phase 2 does.
 // So every consumer thread sees the same rows in the same order as there: y and every per-CTA x.y partial are the same
-// bits, and G only sets how many stages are in flight.  Per 32 blocks (one warp step): 2 x 1 index loads, 3 x loads at
-// stride 3 doubles and five 16-byte dictionary loads that are broadcasts where the nodes share the block (the interior).
+// bits, and G only sets how many stages are in flight.  The tile's index stream (k_vd_runs) is a segment list and block
+// words (staged position | id << 16): a lane in a run segment reads its head's words, position + 3 per node after the
+// head, so its word and dictionary loads are warp-wide broadcasts; a lane in an explicit segment reads its node's own words.
+// Per 32 blocks (one warp step): one word load, 3 x loads at stride 3 doubles and five 16-byte dictionary loads.
 // The y buffers are double-buffered by group parity: the barrier of group n + 1 orders phase B of group n before phase A
 // of group n + 2.
 template <bool DOT, int CW, typename RP>
-__global__ void __launch_bounds__((CW + 4) * 32)
-k_spmv_bsr3_vd(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx, const uint16_t *__restrict__ bvid,
-               const double *__restrict__ vdict, int nvd, const double *__restrict__ x, double *__restrict__ y,
-               const TileDesc *__restrict__ desc, const int *__restrict__ win_start, const int *__restrict__ win_off,
-               int ntiles, int cap_nodes, int cap_x, int cap_blocks, int stages, int stage_bytes, int group,
-               double *__restrict__ dot_partials, const int *__restrict__ skip) {
+__global__ void __launch_bounds__((CW + 4) * 32, 2)
+k_spmv_bsr3_vd(const RP *__restrict__ rowptr, const uint32_t *__restrict__ vwords, const int64_t *__restrict__ vtoff,
+               const int *__restrict__ tile_ids, const double *__restrict__ vdict, int nvd, const double *__restrict__ x,
+               double *__restrict__ y, const TileDesc *__restrict__ desc, const int *__restrict__ win_start,
+               const int *__restrict__ win_off, int ntiles, int cap_nodes, int cap_x, int cap_words, int stages, int stage_bytes,
+               int group, double *__restrict__ dot_partials, const int *__restrict__ skip) {
   if (skip != nullptr && *skip != 0) return;
   extern __shared__ __align__(128) unsigned char smem_raw[];
   __shared__ uint64_t full_bar[kBsrMaxStages], empty_bar[kBsrMaxStages];
@@ -1091,15 +1111,15 @@ k_spmv_bsr3_vd(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx,
   }
   __syncthreads();
 
-  const Bsr3Stage SL = bsr3_stage<true>(0, cap_x, cap_nodes, cap_blocks);
+  const Bsr3Stage SL = bsr3_stage<true>(0, cap_x, cap_nodes, cap_words);
   // behind the stages: y buffers [2][group][3 * cap_nodes] f64, then the dictionary [nvd][kVdStride] f64 (16 B aligned)
   const int ylen = 3 * cap_nodes;
   double *sy = reinterpret_cast<double *>(smem_raw + (size_t)stages * stage_bytes);
   double *sdict = sy + (size_t)2 * group * ylen;
 
   if (warp >= CW) {
-    bsr3_produce<true, RP>(warp - CW, nprod, smem_raw, SL, stages, stage_bytes, full_bar, empty_bar, rowptr, bidx, nullptr, bvid,
-                           x, desc, win_start, win_off, ntiles, 0);
+    bsr3_produce<true, RP>(warp - CW, nprod, smem_raw, SL, stages, stage_bytes, full_bar, empty_bar, rowptr, nullptr, nullptr,
+                           vwords, vtoff, tile_ids, x, desc, win_start, win_off, ntiles, 0);
     return;
   }
 
@@ -1127,16 +1147,24 @@ k_spmv_bsr3_vd(const RP *__restrict__ rowptr, const uint16_t *__restrict__ bidx,
         mbar_wait(&full_bar[s], (uint32_t)((it / stages) & 1));
         const int r0 = meta[0], R = meta[1];
         const int64_t k0 = ((int64_t)(uint32_t)meta[4]) | ((int64_t)meta[5] << 32);
-        const uint16_t *sbt = reinterpret_cast<const uint16_t *>(base + SL.off_sb) + meta[6];
-        const uint16_t *svdt = reinterpret_cast<const uint16_t *>(base + SL.off_sv) + meta[6];
+        const uint32_t *swt = reinterpret_cast<const uint32_t *>(base + SL.off_sb) + meta[6];
+        const int nseg = (int)swt[0];
         double *yt = yg + warp * ylen;
         for (int i = lane; i < R / 3; i += 32) {
           const int b0 = (int)((int64_t)snp[i] - k0) / 9, b1 = (int)((int64_t)snp[i + 1] - k0) / 9;
+          int q = 0;   // segment of node i: the last one that starts at or before it
+          for (int k = 1; k < nseg; ++k) q = (int)(swt[1 + 2 * k] & 0x7fffffffu) <= i ? k : q;
+          const uint32_t head = swt[1 + 2 * q];
+          const int sbase = (int)swt[2 + 2 * q];
+          const bool run = (head >> 31) != 0;
+          const uint32_t *wt = swt + sbase + (run ? 0 : b0);   // words of block 0 of the node (run: of its head)
+          const int dpos = run ? 3 * (i - (int)(head & 0x7fffffffu)) : 0;
           double acc0 = 0.0, acc1 = 0.0, acc2 = 0.0;
 #pragma unroll 2
-          for (int b = b0; b < b1; ++b) {
-            const int ii = sbt[b];
-            const double2 *pv = reinterpret_cast<const double2 *>(sdict + kVdStride * (int)svdt[b]);
+          for (int t = 0; t < b1 - b0; ++t) {
+            const uint32_t w = wt[t];
+            const int ii = (int)(w & 0xffffu) + dpos;
+            const double2 *pv = reinterpret_cast<const double2 *>(sdict + kVdStride * (int)(w >> 16));
             const double2 v01 = pv[0], v23 = pv[1], v45 = pv[2], v67 = pv[3], v8 = pv[4];
             const double x0 = sx[ii], x1 = sx[ii + 1], x2 = sx[ii + 2];
             acc0 += fma(v23.x, x2, fma(v01.y, x1, v01.x * x0));
@@ -1286,6 +1314,74 @@ __global__ void k_vdict_finish(uint16_t *__restrict__ bvid, int64_t nblk, const 
   }
 }
 
+// ---- run-compressed index stream of the dictionary kernel
+// Within a tile, node i joins the run of node i - 1 when it has as many blocks and, block for block, the staged position
+// + 3 and the same dictionary id (a structured mesh along its fastest axis).  The tile's slice of the stream is
+//     nseg | nseg x (first node | run << 31, word base) | block words (bidx | bvid << 16)
+// A run segment (a head and >= 1 node joining it) stores the head's words once at base; an explicit segment stores the
+// words of all its nodes, node i's at base + (its first block in the tile).  More than kVdSegCap segments: the whole tile
+// is one explicit segment.  words == nullptr: count only (words per tile -> tile_words, nodes in runs -> run_nodes).
+constexpr int kVdSegCap = 8;
+template <typename RP>
+__global__ void k_vd_runs(const RP *__restrict__ rowptr, const TileDesc *__restrict__ desc, int ntiles,
+                          const uint16_t *__restrict__ bidx, const uint16_t *__restrict__ bvid, const int64_t *__restrict__ vtoff,
+                          uint32_t *__restrict__ words, int64_t *__restrict__ tile_words, unsigned long long *__restrict__ run_nodes) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= ntiles) return;
+  const int64_t n0 = desc[b].r0 / 3;
+  const int NN = (desc[b].R & 0x3fffffff) / 3;
+  const int64_t kb0 = (int64_t)rowptr[3 * n0] / 9;   // first block of the tile
+  auto blk = [&](int i) { return (int64_t)rowptr[3 * (n0 + i)] / 9; };
+  auto joins = [&](int i) {   // node i (0 < i < NN) joins the run of node i - 1
+    const int64_t a = blk(i - 1), c = blk(i), e = blk(i + 1);
+    if (e - c != c - a) return false;
+    for (int64_t t = 0; t < e - c; ++t)
+      if ((unsigned)bidx[c + t] != (unsigned)bidx[a + t] + 3u || bvid[c + t] != bvid[a + t]) return false;
+    return true;
+  };
+  int sfirst[kVdSegCap], nseg = 0;
+  unsigned srun = 0;   // bit k: segment k is a run
+  bool over = false;
+  int64_t covered = 0;
+  bool jcur = false, jnext = NN > 1 && joins(1);
+  for (int i = 0; i < NN && !over; ++i) {
+    const bool j = jcur;
+    jcur = jnext;                                 // joins(i + 1)
+    jnext = i + 2 < NN && joins(i + 2);
+    if (j) { ++covered; continue; }               // in the current run
+    const bool head = jcur;                       // starts a run
+    if (!head && nseg > 0 && !((srun >> (nseg - 1)) & 1u)) continue;   // extends the current explicit segment
+    if (nseg == kVdSegCap) { over = true; break; }
+    sfirst[nseg] = i;
+    if (head) { srun |= 1u << nseg; ++covered; }
+    ++nseg;
+  }
+  if (over) { nseg = NN > 0 ? 1 : 0; sfirst[0] = 0; srun = 0; covered = 0; }
+  // words: header, then per segment the head's blocks (run) or all its nodes' blocks (explicit)
+  int64_t nw = 1 + 2 * nseg;
+  for (int k = 0; k < nseg; ++k) {
+    const int f = sfirst[k], l = k + 1 < nseg ? sfirst[k + 1] : NN;
+    nw += ((srun >> k) & 1u) ? blk(f + 1) - blk(f) : blk(l) - blk(f);
+  }
+  if (words == nullptr) {
+    tile_words[b] = nw;
+    if (covered) atomicAdd(run_nodes, (unsigned long long)covered);
+    return;
+  }
+  uint32_t *w = words + vtoff[b];
+  w[0] = (uint32_t)nseg;
+  int64_t o = 1 + 2 * nseg;
+  for (int k = 0; k < nseg; ++k) {
+    const int f = sfirst[k], l = k + 1 < nseg ? sfirst[k + 1] : NN;
+    const bool run = (srun >> k) & 1u;
+    const int64_t c0 = blk(f), c1 = run ? blk(f + 1) : blk(l);
+    w[1 + 2 * k] = (uint32_t)f | (run ? 0x80000000u : 0u);
+    w[2 + 2 * k] = (uint32_t)(int)(run ? o : o - (c0 - kb0));   // explicit: node i's words at base + (its block - kb0)
+    for (int64_t t = c0; t < c1; ++t) w[o + t - c0] = (uint32_t)bidx[t] | ((uint32_t)bvid[t] << 16);
+    o += c1 - c0;
+  }
+}
+
 // ---- T3 plan helpers
 // every row offset a multiple of 3  <=>  every row length a multiple of 3 (rowptr[0] = 0)
 template <typename RP>
@@ -1410,6 +1506,45 @@ inline int build_vdict(CsrPlan &P, cudaStream_t st, int mode, int grid) {
   PCGB_CHECK_LAUNCH();
   PCGB_CUDA(cudaStreamSynchronize(st));   // t_map is freed on return
   P.vd = nd;
+  return PCGB_OK;
+}
+
+// The run-compressed index stream of the dictionary kernel (k_vd_runs) from bidx / bvid of the same tiles: P.vwords,
+// P.vtoff, P.cap_words, P.run_nodes.  Frees bvid, which nothing reads afterwards.
+template <typename RP>
+inline int build_vd_runs(CsrPlan &P, cudaStream_t st) {
+  const RP *rp = static_cast<const RP *>(P.rowptr);
+  const int nt = P.ntiles;
+  DevTmp t_nw, t_cov;
+  PCGB_CUDA(cudaMalloc(&t_nw.p, (size_t)nt * sizeof(int64_t)));
+  PCGB_CUDA(cudaMalloc(&t_cov.p, sizeof(unsigned long long)));
+  PCGB_CUDA(cudaMemsetAsync(t_cov.p, 0, sizeof(unsigned long long), st));
+  k_vd_runs<RP><<<(nt + 127) / 128, 128, 0, st>>>(rp, P.tile_desc, nt, P.bidx, P.bvid, nullptr, nullptr, t_nw.as<int64_t>(),
+                                                  t_cov.as<unsigned long long>());
+  PCGB_CHECK_LAUNCH();
+  std::vector<int64_t> off((size_t)nt + 1);
+  unsigned long long cov = 0;
+  PCGB_CUDA(cudaMemcpyAsync(off.data(), t_nw.p, (size_t)nt * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  PCGB_CUDA(cudaMemcpyAsync(&cov, t_cov.p, sizeof(cov), cudaMemcpyDeviceToHost, st));
+  PCGB_CUDA(cudaStreamSynchronize(st));
+  int64_t tot = 0, cap = 4;
+  for (int b = 0; b < nt; ++b) {
+    const int64_t w0 = tot;
+    tot += off[(size_t)b];
+    off[(size_t)b] = w0;
+    cap = std::max(cap, ((tot + 3) & ~(int64_t)3) - (w0 & ~(int64_t)3));   // the producer's 16-byte aligned window
+  }
+  off[(size_t)nt] = tot;
+  if (cap > (int64_t)1 << 20) return fail(PCGB_ERR_ARG, "SpMV tile index slice of %lld words", (long long)cap);
+  PCGB_CUDA(cudaMalloc(&P.vwords, ((size_t)tot + 8) * sizeof(uint32_t)));
+  PCGB_CUDA(cudaMemsetAsync(P.vwords + tot, 0, 8 * sizeof(uint32_t), st));
+  PCGB_CUDA(cudaMalloc(&P.vtoff, ((size_t)nt + 1) * sizeof(int64_t)));
+  PCGB_CUDA(cudaMemcpyAsync(P.vtoff, off.data(), ((size_t)nt + 1) * sizeof(int64_t), cudaMemcpyHostToDevice, st));
+  k_vd_runs<RP><<<(nt + 127) / 128, 128, 0, st>>>(rp, P.tile_desc, nt, P.bidx, P.bvid, P.vtoff, P.vwords, nullptr, nullptr);
+  PCGB_CHECK_LAUNCH();
+  PCGB_CUDA(cudaStreamSynchronize(st));   // `off` is read by the copy above
+  P.nvwords = tot; P.cap_words = (int)cap; P.run_nodes = (int64_t)cov;
+  cudaFree(P.bvid); P.bvid = nullptr;
   return PCGB_OK;
 }
 
@@ -1692,15 +1827,18 @@ inline int build_plan_t(CsrPlan &P, cudaStream_t st, int bsr_tile = 0, int attem
               P.grid_bsr = std::min(P.ntiles, num_sms() * P.ctas_per_sm);
               // value dictionary (PCGB_SPMV_VDICT: 0 off, 1 when it pays, 2 whenever the blocks fit it).  The tiles, the grid and
               // the consumer warps stay those of the plan without one - they fix the order in which x.y is summed, so y and
-              // x.y are the same bits either way; only the ring changes: a stage holds no values (sx | snp | bidx | bvid |
-              // meta), and behind the ring sit the y buffers of two groups of tiles and the dictionary (k_spmv_bsr3_vd).
+              // x.y are the same bits either way; only the ring changes: a stage holds no values (sx | snp | the tile's
+              // run-compressed block words | meta), and behind the ring sit the y buffers of two groups of tiles and the
+              // dictionary (k_spmv_bsr3_vd).
               const int vd_mode = env_int("PCGB_SPMV_VDICT", 1);
               if (vd_mode != 0) PCGB_TRY(build_vdict<RP>(P, st, vd_mode, P.grid_bsr));
+              if (P.vd) PCGB_TRY(build_vd_runs<RP>(P, st));
               if (P.vd) {
-                // G warps consume G tiles at once, so the ring holds the G stages of a group plus two that the producers
-                // fill for the next one: G = CW where that still fits the CTAs per SM of the plan (hex 128^3: CW 6 and 8),
-                // else the largest G that does.  PCGB_SPMV_STAGES sets the ring instead, G = min(CW, stages).
-                const int vstage = (P.cap_x * 8 + (P.cap_nodes + 2) * 8 + 2 * sb_bytes + 32 + 127) & ~127;
+                // G warps consume G tiles at once, so the ring holds the G stages of a group plus at least two that the
+                // producers fill for the next one, up to a whole second group: G = CW where G + 2 stages still fit the CTAs
+                // per SM of the plan (hex 128^3: CW 6 and 8), else the largest G that does, and then the deepest even ring
+                // up to 2 G + 2 that fits.  PCGB_SPMV_STAGES sets the ring instead, G = min(CW, stages).
+                const int vstage = (P.cap_x * 8 + (P.cap_nodes + 2) * 8 + P.cap_words * 4 + 32 + 127) & ~127;
                 auto ring_smem = [&](int g, int s) { return s * vstage + 2 * g * 3 * P.cap_nodes * 8 + kVdStride * 8 * P.vd; };
                 auto ring_fits = [&](int smem) { return smem <= 226 * 1024 && (227 * 1024) / (smem + 2048) >= P.ctas_per_sm; };
                 int vst = 0, vg = 0;
@@ -1710,17 +1848,18 @@ inline int build_plan_t(CsrPlan &P, cudaStream_t st, int bsr_tile = 0, int attem
                   vg = std::min(P.bsr_cw, vst);
                   if (!ring_fits(ring_smem(vg, vst))) vst = 0;
                 } else {
-                  for (int g = P.bsr_cw; g >= 1 && vst == 0; --g) {
-                    const int s = std::min((g + 3) & ~1, kBsrMaxStages);   // g + 2, even (producer warps: see below)
-                    if (ring_fits(ring_smem(g, s))) { vst = s; vg = g; }
-                  }
+                  for (int g = P.bsr_cw; g >= 1 && vst == 0; --g)   // even rings (producer warps: see below)
+                    for (int s = std::min((2 * g + 3) & ~1, kBsrMaxStages); s >= g + 2 && vst == 0; s -= 2)
+                      if (ring_fits(ring_smem(g, s))) { vst = s; vg = g; }
                 }
                 if (vst > 0) {
                   P.bsr_stages = vst; P.bsr_group = vg; P.bsr_stage_bytes = vstage; P.smem_bsr = ring_smem(vg, vst);
                   P.bsr_prod = vst < 4 ? vst : vst % 4 == 0 ? 4 : vst % 2 == 0 ? 2 : 1;   // stages % producers == 0
+                  cudaFree(P.bidx); P.bidx = nullptr;   // the word stream replaces it
                 } else {
-                  cudaFree(P.bvid); cudaFree(P.vdict);
-                  P.bvid = nullptr; P.vdict = nullptr; P.vd = 0;
+                  cudaFree(P.vdict); cudaFree(P.vwords); cudaFree(P.vtoff);
+                  P.vdict = nullptr; P.vwords = nullptr; P.vtoff = nullptr; P.vd = 0;
+                  P.nvwords = 0; P.run_nodes = 0; P.cap_words = 0;
                 }
               }
               P.grid_persist = P.grid_bsr; P.smem_persist = P.smem_bsr; P.stages = P.bsr_stages; P.stage_bytes = P.bsr_stage_bytes;
@@ -1835,7 +1974,7 @@ inline int launch_persist_lanes(const CsrPlan &P, const double *x, double *y, cu
 
 template <bool DOT, int CW, typename RP, bool VD>
 inline int launch_bsr_cw(const CsrPlan &P, const double *x, double *y, cudaStream_t st, const int *skip, const TileDesc *desc,
-                         int ntiles, int grid, double *dotp) {
+                         int ntiles, int grid, double *dotp, const int *tile_ids) {
   if constexpr (VD) {
     auto kern = k_spmv_bsr3_vd<DOT, CW, RP>;
     if (skip == reinterpret_cast<const int *>(1)) {
@@ -1843,9 +1982,9 @@ inline int launch_bsr_cw(const CsrPlan &P, const double *x, double *y, cudaStrea
       return PCGB_OK;
     }
     if (ntiles == 0) return PCGB_OK;
-    kern<<<grid, (CW + P.bsr_prod) * 32, P.smem_bsr, st>>>(static_cast<const RP *>(P.rowptr), P.bidx, P.bvid, P.vdict, P.vd, x, y,
-                                                           desc, P.win_start, P.win_off, ntiles, P.cap_nodes, P.cap_x, P.cap_blocks,
-                                                           P.bsr_stages, P.bsr_stage_bytes, P.bsr_group, dotp, skip);
+    kern<<<grid, (CW + P.bsr_prod) * 32, P.smem_bsr, st>>>(static_cast<const RP *>(P.rowptr), P.vwords, P.vtoff, tile_ids, P.vdict,
+                                                           P.vd, x, y, desc, P.win_start, P.win_off, ntiles, P.cap_nodes, P.cap_x,
+                                                           P.cap_words, P.bsr_stages, P.bsr_stage_bytes, P.bsr_group, dotp, skip);
   } else {
     auto kern = k_spmv_bsr3<DOT, CW, RP>;
     if (skip == reinterpret_cast<const int *>(1)) {
@@ -1863,29 +2002,30 @@ inline int launch_bsr_cw(const CsrPlan &P, const double *x, double *y, cudaStrea
 
 template <bool DOT, typename RP, bool VD>
 inline int launch_bsr_vd(const CsrPlan &P, const double *x, double *y, cudaStream_t st, const int *skip, const TileDesc *desc,
-                         int ntiles, int grid, double *dotp) {
+                         int ntiles, int grid, double *dotp, const int *tile_ids) {
   // consumer warps per CTA: 6 by default; 8 and 12 are selectable with PCGB_BSR_CW.  On H100 (hex 128^3) the three are equal
   // within noise: 1.450-1.452 ms stand-alone (tools/spmv_sweep.py), 604-606 PCG it/s in bench.py.
-  if (P.bsr_cw == 8) return launch_bsr_cw<DOT, 8, RP, VD>(P, x, y, st, skip, desc, ntiles, grid, dotp);
-  if (P.bsr_cw == 12) return launch_bsr_cw<DOT, 12, RP, VD>(P, x, y, st, skip, desc, ntiles, grid, dotp);
-  return launch_bsr_cw<DOT, 6, RP, VD>(P, x, y, st, skip, desc, ntiles, grid, dotp);
+  if (P.bsr_cw == 8) return launch_bsr_cw<DOT, 8, RP, VD>(P, x, y, st, skip, desc, ntiles, grid, dotp, tile_ids);
+  if (P.bsr_cw == 12) return launch_bsr_cw<DOT, 12, RP, VD>(P, x, y, st, skip, desc, ntiles, grid, dotp, tile_ids);
+  return launch_bsr_cw<DOT, 6, RP, VD>(P, x, y, st, skip, desc, ntiles, grid, dotp, tile_ids);
 }
 
 template <bool DOT, typename RP>
 inline int launch_bsr_inst(const CsrPlan &P, const double *x, double *y, cudaStream_t st, const int *skip, const TileDesc *desc,
-                           int ntiles, int grid, double *dotp) {
-  if (P.vd) return launch_bsr_vd<DOT, RP, true>(P, x, y, st, skip, desc, ntiles, grid, dotp);
-  return launch_bsr_vd<DOT, RP, false>(P, x, y, st, skip, desc, ntiles, grid, dotp);
+                           int ntiles, int grid, double *dotp, const int *tile_ids) {
+  if (P.vd) return launch_bsr_vd<DOT, RP, true>(P, x, y, st, skip, desc, ntiles, grid, dotp, tile_ids);
+  return launch_bsr_vd<DOT, RP, false>(P, x, y, st, skip, desc, ntiles, grid, dotp, tile_ids);
 }
 
+// tile_ids: tile id of every entry of desc (nullptr: desc is the plan's own tile order)
 inline int launch_persist_any(const CsrPlan &P, const double *x, double *y, bool with_dot, cudaStream_t st, const int *skip,
-                              const TileDesc *desc, int ntiles, int grid, double *dotp) {
+                              const TileDesc *desc, int ntiles, int grid, double *dotp, const int *tile_ids) {
   if (P.ntiles == 0) return PCGB_OK;
   if (P.bsr) {
-    if (P.rp64) return with_dot ? launch_bsr_inst<true, int64_t>(P, x, y, st, skip, desc, ntiles, grid, dotp)
-                                : launch_bsr_inst<false, int64_t>(P, x, y, st, skip, desc, ntiles, grid, dotp);
-    return with_dot ? launch_bsr_inst<true, int32_t>(P, x, y, st, skip, desc, ntiles, grid, dotp)
-                    : launch_bsr_inst<false, int32_t>(P, x, y, st, skip, desc, ntiles, grid, dotp);
+    if (P.rp64) return with_dot ? launch_bsr_inst<true, int64_t>(P, x, y, st, skip, desc, ntiles, grid, dotp, tile_ids)
+                                : launch_bsr_inst<false, int64_t>(P, x, y, st, skip, desc, ntiles, grid, dotp, tile_ids);
+    return with_dot ? launch_bsr_inst<true, int32_t>(P, x, y, st, skip, desc, ntiles, grid, dotp, tile_ids)
+                    : launch_bsr_inst<false, int32_t>(P, x, y, st, skip, desc, ntiles, grid, dotp, tile_ids);
   }
   if (P.t3) {
     if (P.rp64) return with_dot ? launch_persist_lanes<true, true, int64_t>(P, x, y, st, skip, desc, ntiles, grid, dotp)
@@ -1905,7 +2045,7 @@ inline int spmv_launch(const CsrPlan &P, const double *x, double *y, bool with_d
                        const int *skip = nullptr) {
   int rc;
   if (P.persist) {
-    rc = launch_persist_any(P, x, y, with_dot, st, skip, P.tile_desc, P.ntiles, P.grid_persist, P.dot_partials);
+    rc = launch_persist_any(P, x, y, with_dot, st, skip, P.tile_desc, P.ntiles, P.grid_persist, P.dot_partials, nullptr);
   } else if (P.staged) {
     if (P.rp64) rc = with_dot ? launch_staged_lanes<true, int64_t>(P, x, y, st, skip) : launch_staged_lanes<false, int64_t>(P, x, y, st, skip);
     else rc = with_dot ? launch_staged_lanes<true, int32_t>(P, x, y, st, skip) : launch_staged_lanes<false, int32_t>(P, x, y, st, skip);
@@ -1941,7 +2081,8 @@ inline int spmv_launch_part(const CsrPlan &P, int part, const double *x, double 
   if (nt <= 0) return PCGB_OK;
   const TileDesc *desc = P.desc_split + (part == 0 ? 0 : P.nb_tiles);
   const int grid = std::min(nt, P.grid_persist);
-  PCGB_TRY(launch_persist_any(P, x, y, with_dot, st, skip, desc, nt, grid, P.dot_partials_split + (size_t)part * P.grid_persist));
+  PCGB_TRY(launch_persist_any(P, x, y, with_dot, st, skip, desc, nt, grid, P.dot_partials_split + (size_t)part * P.grid_persist,
+                              P.split_tile + (part == 0 ? 0 : P.nb_tiles)));
   if (launches) *launches += 1;
   return PCGB_OK;
 }
@@ -1951,15 +2092,13 @@ inline int spmv_split_dot_count(const CsrPlan &P) { return 2 * P.grid_persist; }
 inline int spmv_set_boundary_rows(CsrPlan &P, const int *d_rows, int64_t count, cudaStream_t st) {
   if (!P.persist || P.nfix != 0 || P.ntiles == 0) return PCGB_OK;  // split not applicable: callers fall back to the serial order
   unsigned char *rowflag = nullptr, *tileflag = nullptr;
-  int *d_perm = nullptr;
   int rc = PCGB_OK;
   std::vector<unsigned char> hflag((size_t)P.ntiles);
   std::vector<int> perm((size_t)P.ntiles);
-  auto cleanup = [&]() { cudaFree(rowflag); cudaFree(tileflag); cudaFree(d_perm); };
+  auto cleanup = [&]() { cudaFree(rowflag); cudaFree(tileflag); };
 #define PCGB_SB(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) { cleanup(); return fail(PCGB_ERR_CUDA, "%s:%d %s -> %s", __FILE__, __LINE__, #call, cudaGetErrorString(e_)); } } while (0)
   PCGB_SB(cudaMalloc(&rowflag, (size_t)P.nrows + 1));
   PCGB_SB(cudaMalloc(&tileflag, (size_t)P.ntiles));
-  PCGB_SB(cudaMalloc(&d_perm, (size_t)P.ntiles * sizeof(int)));
   PCGB_SB(cudaMemsetAsync(rowflag, 0, (size_t)P.nrows + 1, st));
   if (count > 0) k_mark_rows<<<(unsigned)((count + 255) / 256), 256, 0, st>>>(d_rows, count, rowflag);
   k_flag_tiles<<<(P.ntiles + 255) / 256, 256, 0, st>>>(P.tile_desc, P.ntiles, rowflag, tileflag);
@@ -1971,8 +2110,9 @@ inline int spmv_set_boundary_rows(CsrPlan &P, const int *d_rows, int64_t count, 
   int k = nb;
   for (int b = 0; b < P.ntiles; ++b) if (!hflag[(size_t)b]) perm[(size_t)k++] = b;
   if (!P.desc_split) PCGB_SB(cudaMalloc(&P.desc_split, (size_t)P.ntiles * sizeof(TileDesc)));
-  PCGB_SB(cudaMemcpyAsync(d_perm, perm.data(), (size_t)P.ntiles * sizeof(int), cudaMemcpyHostToDevice, st));
-  k_gather_desc<<<(P.ntiles + 255) / 256, 256, 0, st>>>(P.tile_desc, d_perm, P.ntiles, P.desc_split);
+  if (!P.split_tile) PCGB_SB(cudaMalloc(&P.split_tile, (size_t)P.ntiles * sizeof(int)));   // the tile ids of desc_split
+  PCGB_SB(cudaMemcpyAsync(P.split_tile, perm.data(), (size_t)P.ntiles * sizeof(int), cudaMemcpyHostToDevice, st));
+  k_gather_desc<<<(P.ntiles + 255) / 256, 256, 0, st>>>(P.tile_desc, P.split_tile, P.ntiles, P.desc_split);
   PCGB_SB(cudaGetLastError());
   PCGB_SB(cudaMemsetAsync(P.dot_partials_split, 0, (size_t)2 * (size_t)std::max(P.grid_persist, 1) * sizeof(double), st));
   PCGB_SB(cudaStreamSynchronize(st));
@@ -1996,7 +2136,7 @@ inline void free_plan(CsrPlan &P) {
   cudaFree(P.fix_row); cudaFree(P.fix_first); cudaFree(P.fix_cnt);
   cudaFree(P.tile_xlen); cudaFree(P.tile_win); cudaFree(P.win_start); cudaFree(P.win_off); cudaFree(P.lidx);
   cudaFree(P.tile_desc); cudaFree(P.lidx3); cudaFree(P.bidx); cudaFree(P.desc_split); cudaFree(P.dot_partials_split); cudaFree(P.diag_cache);
-  cudaFree(P.bvid); cudaFree(P.vdict);
+  cudaFree(P.bvid); cudaFree(P.vdict); cudaFree(P.vwords); cudaFree(P.vtoff); cudaFree(P.split_tile);
 }
 
 }  // namespace pcgb
