@@ -97,6 +97,10 @@ int pcgb_csr_value_dict(pcgb_csr_t A);
  * every node has the blocks of the one before it, 3 staged x entries further on with the same ids, and only the head's
  * block words are stored.  Returns the share of the nodes that lie in run segments (0 without a dictionary). */
 double pcgb_csr_run_share(pcgb_csr_t A);
+/* The ring of the dictionary kernel, all zeros when the plan has no dictionary: out = {stages, tiles per group G,
+ * producer warps, consumer warps CW, words of the largest tile slice (cap_words), words of the index stream (nvwords),
+ * nodes per tile stage (cap_nodes), resident CTAs per SM}. */
+int pcgb_csr_vd_plan(pcgb_csr_t A, int64_t out[8]);
 
 /* ---------------------------------------------------------------- vector kernels (a4-a10)
  * out[0] = sum_i a[i]*b[i]*w[i]   (w may be NULL = all ones).  np.dot(a, b*w) of

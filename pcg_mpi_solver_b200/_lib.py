@@ -62,6 +62,7 @@ SIGNATURES = {
     "pcgb_csr_plan_info": (c_int, [c_void_p, POINTER(c_int64)]),
     "pcgb_csr_value_dict": (c_int, [c_void_p]),
     "pcgb_csr_run_share": (c_double, [c_void_p]),
+    "pcgb_csr_vd_plan": (c_int, [c_void_p, POINTER(c_int64)]),
     "pcgb_dot_w": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
     "pcgb_axpby": (c_int, [c_int64, c_double, c_void_p, c_double, c_void_p, c_void_p]),
     "pcgb_mul": (c_int, [c_int64, c_void_p, c_void_p, c_void_p, c_void_p]),

@@ -92,6 +92,13 @@ class CsrMatrix:
         tile with the same blocks shifted by one node: a structured mesh along x); 0.0 without a dictionary."""
         return float(_lib.load().pcgb_csr_run_share(self._h))
 
+    def value_dict_plan(self) -> dict:
+        """The ring of the dictionary kernel (pcgb_csr_vd_plan); every field 0 without a dictionary."""
+        out = (ctypes.c_int64 * 8)()
+        _lib.check(_lib.load().pcgb_csr_vd_plan(self._h, out))
+        keys = ["stages", "group", "producers", "consumers", "cap_words", "nvwords", "cap_nodes", "ctas_per_sm"]
+        return dict(zip(keys, [int(v) for v in out]))
+
     def release_col(self) -> bool:
         """Free the 4-byte column array when the selected SpMV kernel does not read it (the persistent staged-x kernel
         streams its own 16-bit indices): 2 GB at 128^3, 16 GB at 256^3.  The diagonal is cached first.  Returns True

@@ -285,6 +285,16 @@ double pcgb_csr_run_share(pcgb_csr_t A) {
   return (double)A->P.run_nodes / (double)(A->P.nrows / 3);
 }
 
+int pcgb_csr_vd_plan(pcgb_csr_t A, int64_t out[8]) {
+  if (!A || !out) return fail(PCGB_ERR_ARG, "pcgb_csr_vd_plan: null argument");
+  const CsrPlan &P = A->P;
+  for (int i = 0; i < 8; ++i) out[i] = 0;
+  if (P.vd == 0) return PCGB_OK;
+  out[0] = P.bsr_stages; out[1] = P.bsr_group; out[2] = P.bsr_prod; out[3] = P.bsr_cw;
+  out[4] = P.cap_words; out[5] = P.nvwords; out[6] = P.cap_nodes; out[7] = P.ctas_per_sm;
+  return PCGB_OK;
+}
+
 int pcgb_csr_plan_info(pcgb_csr_t A, int64_t info[16]) {
   if (!A || !info) return fail(PCGB_ERR_ARG, "pcgb_csr_plan_info: null argument");
   const CsrPlan &P = A->P;

@@ -9,48 +9,10 @@ import numpy as np
 import pytest
 
 from tests import spmv_cases as C
+from tests.nodeblock_cases import expected_run_nodes
 from tests.test_gpu_spmv_vdict import _GATE, _assert_same_bits, _bits, _block_positions, _env, _tensors, _with_dictionary
 
 pytestmark = pytest.mark.gpu
-SEG_CAP = 8
-
-
-# ------------------------------------------------------------------------------------------------ host restatement
-def expected_run_nodes(A, tile_items, cap=SEG_CAP):
-    """Nodes in run segments of the plan's tiles (k_partition restated by spmv_cases.tile_row_starts).  Positions are
-    compared as columns: two blocks of consecutive nodes whose columns differ by 3 lie in one staged x window."""
-    A = A.tocsr()
-    ip = A.indptr.astype(np.int64)
-    nn = (ip.size - 1) // 3
-    nb = (ip[1::3] - ip[0:-1:3]) // 3
-    pos = _block_positions(A)                                   # (blocks, 9)
-    bits = A.data.view(np.int64)[pos]
-    bcol = A.indices.astype(np.int64)[pos[:, 0]]
-    node = np.repeat(np.arange(nn), nb)
-    same = np.zeros(nn, dtype=bool)
-    same[1:] = nb[1:] == nb[:-1]
-    g = np.arange(node.size)
-    okb = np.zeros(node.size, dtype=bool)
-    m = same[node]
-    prev = g[m] - nb[node[m]]
-    okb[m] = (bcol[g[m]] == bcol[prev] + 3) & (bits[g[m]] == bits[prev]).all(axis=1)
-    bad = np.bincount(node[~okb], minlength=nn) if node.size else np.zeros(nn, np.int64)
-    join = same & (bad == 0)
-    starts = C.tile_row_starts(ip, tile_items, unit=3) // 3
-    total = 0
-    for s, e in zip(starts[:-1], starts[1:]):
-        segs, covered = [], 0                                   # (first, run)
-        for i in range(s, e):
-            if i > s and join[i]:
-                covered += 1
-                continue
-            head = i + 1 < e and join[i + 1]
-            if not head and segs and not segs[-1][1]:
-                continue
-            segs.append((i, head))
-            covered += head
-        total += covered if len(segs) <= cap else 0
-    return total
 
 
 def _run_share(M):
