@@ -439,12 +439,32 @@ int pcgb_mg_create_field(pcgb_solver_t s, const pcgb_hex_box *box, const double 
  * coarsening rule's (a box with every ne <= 2, more than PCGB_MG_MAX_LEVELS levels), and E or h <= 0. */
 int pcgb_mg_create_any(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine, double E, double h,
                        const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out);
+/* pcgb_mg_create and pcgb_mg_create_ranks with index-free coarse levels: the same hierarchy, arguments, refusals and
+ * synchronisation, the same replacement of the diagonal preconditioner (pcg_solver.py:346-352 and 446-454), but every
+ * smoothed level l >= 1 (across ranks: the ranked levels 1 .. la-1 and the replicated levels above the coarsest) applies
+ * its box with the index-free operator of pcgb_hexop_create (Ke = ke_host, Ck = E 2^glev h, glev the level of the global
+ * hierarchy; calcMatVecProd, pcg_solver.py:263-300, per node) instead of a device-generated CSR matrix and SpMV plan.
+ * D^-1 of such a level is 1 / its pcgb_hexop_diag diagonal (pcg_solver.py:282-287), after the level's exchange-add on a
+ * ranked level.  Lambda, smoothers, transfers, gather / scatter and the coarsest level's dense Cholesky factor are
+ * unchanged, so the V-cycle equals pcgb_mg_create's to rounding.  The hierarchy holds only vectors and that factor:
+ * pcgb_mg_info's bytes are 8 (5 n_0 + 6 sum n_l over the smoothed coarse levels + 2 n_c + n_c^2) on one rank (across
+ * ranks also n_l ownership weights per ranked level and 2 n_la for the gathered level).  pcgb_mg_level_csr refuses its
+ * levels.                                                                                                               */
+int pcgb_mg_create_index_free(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h,
+                              const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out);
+int pcgb_mg_create_ranks_index_free(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos,
+                                    pcgb_halo_t gather, const double *const *d_own, const double *ke_host, double E, double h,
+                                    const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out);
+/* For tests: y = A_l x on smoothed coarse level `level` (1 <= level < nlevels - 1, not the gathered level of a multi-rank
+ * handle) of either kind, the local product without the level's exchange-add.  PCGB_ERR_ARG for any other level and,
+ * before any launch, when [d_x, d_x + n_l) and [d_y, d_y + n_l) overlap. */
+int pcgb_mg_level_apply(pcgb_mg_t mg, int level, const double *d_x, double *d_y, void *stream);
 /* The element counts of level `level` (0 .. nlevels - 1) of any handle into ne[3] (x, y, z); PCGB_ERR_ARG outside. */
 int pcgb_mg_level_box(pcgb_mg_t mg, int level, int32_t *ne);
 /* For tests: level `level`'s CSR (1 <= level < nlevels - 1, the smoothed coarse levels) into caller buffers: int64 row
  * offsets (n + 1), int32 columns and values (nnz each).  With all three buffers NULL only *nnz is written.  Synchronises
- * `stream`.  PCGB_ERR_ARG for level 0 (the solver's operator), the coarsest level (held as a dense factor) and the
- * gathered level of a multi-rank handle. */
+ * `stream`.  PCGB_ERR_ARG for level 0 (the solver's operator), the coarsest level (held as a dense factor), the
+ * gathered level of a multi-rank handle and every level of an index-free hierarchy. */
 int pcgb_mg_level_csr(pcgb_mg_t mg, int level, int64_t *d_rowptr, int32_t *d_col, double *d_val, int64_t *nnz, void *stream);
 /* Set-up costs of a field hierarchy (0 for the others): device time of the Galerkin kernels in ms, and the peak device
  * bytes of element matrices held at once during create.  Either may be NULL. */

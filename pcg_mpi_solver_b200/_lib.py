@@ -121,6 +121,11 @@ SIGNATURES = {
                                    POINTER(c_void_p)]),
     "pcgb_mg_level_box": (c_int, [c_void_p, c_int, POINTER(c_int32)]),
     "pcgb_mg_level_csr": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p, POINTER(c_int64), c_void_p]),
+    "pcgb_mg_create_index_free": (c_int, [c_void_p, POINTER(HexBox), POINTER(c_double), c_double, c_double, c_void_p, c_int, c_double,
+                                          POINTER(c_void_p)]),
+    "pcgb_mg_create_ranks_index_free": (c_int, [c_void_p, POINTER(HexBox), c_int, POINTER(c_void_p), c_void_p, POINTER(c_void_p),
+                                                POINTER(c_double), c_double, c_double, c_void_p, c_int, c_double, POINTER(c_void_p)]),
+    "pcgb_mg_level_apply": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "pcgb_mg_setup_info": (c_int, [c_void_p, POINTER(c_double), POINTER(c_int64)]),
     "pcgb_mg_info_ranks": (c_int, [c_void_p, POINTER(c_int32), POINTER(c_int64)]),
     "pcgb_mg_gather": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p]),

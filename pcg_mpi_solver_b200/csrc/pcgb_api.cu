@@ -1037,6 +1037,10 @@ struct MgLevel {
   double *val = nullptr;
   CsrPlan P;
   bool has_plan = false;
+  // index-free hierarchies (pcgb_mg_create_index_free / _ranks_index_free): smoothed levels l >= 1 apply the level's box
+  // with hexop.cuh (Ke, uniform Ck = E 2^glev h) instead of the CSR above, which they leave empty
+  bool index_free = false;
+  HexOp H;
   double *dinv = nullptr;                                    // inverse diagonal (level 0: a copy of the caller's Minv)
   double *b = nullptr, *x = nullptr;                         // right-hand side and correction (level 0: the caller's r and z)
   double *r = nullptr, *d = nullptr, *q = nullptr;           // smoother residual, direction, operator product
@@ -1054,6 +1058,7 @@ struct pcgb_mg_s {
   int degree = 2;
   double lo = 0.25;
   int la = -1;                     // gathered ranked level (-1: one rank)
+  bool index_free = false;         // smoothed coarse levels are HexOps, not CSR matrices
   pcgb_halo_t gather = nullptr;    // all-to-all plan over the global box of level la (not owned)
   int nc = 0;
   double *chol = nullptr;   // coarsest level: dense Cholesky factor, L in the lower triangle mirrored into the upper
@@ -1079,8 +1084,9 @@ constexpr int kMgLanczosSteps = 20;
 // the fine halo of the iteration: every rank enqueues the same exchanges and all ranks stop at the same iteration.
 int mg_op(pcgb_mg_t mg, int l, const double *x, double *y, cudaStream_t st, int *nl, const int *skip) {
   const MgLevel &L = mg->lv[(size_t)l];
-  if (l > 0) PCGB_TRY(spmv_launch(L.P, x, y, false, st, nl, skip));
-  else PCGB_TRY(mg->s->op.apply(x, y, st, nl, skip));
+  if (l == 0) PCGB_TRY(mg->s->op.apply(x, y, st, nl, skip));
+  else if (L.index_free) PCGB_TRY(hexop_apply(L.H, x, y, st, nl, skip));
+  else PCGB_TRY(spmv_launch(L.P, x, y, false, st, nl, skip));
   return L.halo ? halo_exchange_add(L.halo, y, st, nl) : PCGB_OK;
 }
 
@@ -1666,6 +1672,19 @@ int mg_hex_csr(const HexGeom &g, const double *ke_host, double ck, int64_t **rp,
   return PCGB_OK;
 }
 
+// The index-free operator of box g: Ke (row-major 24x24) and its diagonal by value, Ck uniform or (d_ck) per element
+HexOp hexop_of(const HexGeom &g, const double *ke_host, double ck, const double *d_ck) {
+  HexOp H;
+  H.s = hexop_shape(g);
+  std::memcpy(H.ke.k, ke_host, sizeof(H.ke.k));
+  for (int a = 0; a < 24; ++a) H.kd.k[a] = ke_host[a * 24 + a];
+  H.ck = d_ck ? 0.0 : ck;
+  H.d_ck = d_ck;
+  H.n = 3 * g.nfree_nodes;
+  H.bytes = 16 * H.n + (d_ck ? 8 * (int64_t)g.nx * g.ny * g.nz : 0);
+  return H;
+}
+
 // Field hierarchies: the Galerkin element matrices of level l (l >= 1) from those of level l - 1 (level 1: from the fine
 // Ck field and Ke), into mg->kel; the level below's matrices are freed once these exist, so at most two levels' are held.
 int mg_galerkin_level(pcgb_mg_t mg, int l, const double *ke_host) {
@@ -1887,7 +1906,15 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
     PCGB_CUDA(alloc(&L.r, L.n));
     PCGB_CUDA(alloc(&L.d, L.n));
     PCGB_CUDA(alloc(&L.q, L.n));
-    if (l > 0) {
+    if (l > 0 && mg->index_free) {   // the level's box applied by hexop.cuh; D from its diagonal kernel
+      L.index_free = true;
+      L.H = hexop_of(L.g, ke_host, ck, nullptr);
+      PCGB_CUDA(alloc(&L.dinv, L.n));
+      PCGB_TRY(hexop_diag(L.H, L.r, 0));
+      if (L.halo) PCGB_TRY(halo_exchange_add(L.halo, L.r, 0));   // assembled diagonal of a ranked level
+      k_reciprocal<<<vec_grid(L.n), 256>>>(L.n, L.r, L.dinv);
+      PCGB_CHECK_LAUNCH();
+    } else if (l > 0) {
       int64_t *rp = nullptr, nnz = 0;
       const int rc = mg_hex_csr(L.g, ke_host, ck, &rp, &L.col, &L.val, &nnz, mg->kel);
       L.rowptr = rp;
@@ -1933,10 +1960,12 @@ int field_bad(int64_t n, const double *d_v, cudaStream_t st, const char *who, in
   return e == cudaSuccess ? PCGB_OK : fail(PCGB_ERR_CUDA, "%s: field check failed: %s", who, cudaGetErrorString(e));
 }
 
-// pcgb_mg_create (d_ck_fine NULL: Ck = E 2^l h on level l), pcgb_mg_create_field (Galerkin levels from d_ck_fine) and
-// pcgb_mg_create_any (any_rule: the coarsening of mg_any_box_levels, Galerkin levels from d_ck_fine or, NULL, Ck = E h)
+// pcgb_mg_create (d_ck_fine NULL: Ck = E 2^l h on level l; index_free: pcgb_mg_create_index_free), pcgb_mg_create_field
+// (Galerkin levels from d_ck_fine) and pcgb_mg_create_any (any_rule: the coarsening of mg_any_box_levels, Galerkin levels
+// from d_ck_fine or, NULL, Ck = E h)
 int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, const double *d_ck_fine,
-                  const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out, const char *who, bool any_rule = false) {
+                  const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out, const char *who, bool any_rule = false,
+                  bool index_free = false) {
   PCGB_TRY(require_device());
   if (!s || !box || !ke_host || !d_minv_fine || !out) return fail(PCGB_ERR_ARG, "%s: null argument", who);
   if (s->halo || s->comm) return fail(PCGB_ERR_ARG, "%s: one rank only (the solver has a halo plan or a communicator)", who);
@@ -1977,7 +2006,7 @@ int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_hos
     d_ck_fine = ck_uniform;
   }
   pcgb_mg_t mg = new pcgb_mg_s();
-  mg->s = s; mg->degree = degree; mg->lo = lo; mg->ck_fine = d_ck_fine;
+  mg->s = s; mg->degree = degree; mg->lo = lo; mg->ck_fine = d_ck_fine; mg->index_free = index_free;
   mg->lv.resize(geo.size());
   for (size_t l = 0; l < geo.size(); ++l) {
     MgLevel &L = mg->lv[l];
@@ -1997,6 +2026,11 @@ int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_hos
 int pcgb_mg_create(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, const double *d_minv_fine,
                    int degree, double lo, pcgb_mg_t *out) {
   return mg_create_one(s, box, ke_host, E, h, nullptr, d_minv_fine, degree, lo, out, "pcgb_mg_create");
+}
+
+int pcgb_mg_create_index_free(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h,
+                              const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
+  return mg_create_one(s, box, ke_host, E, h, nullptr, d_minv_fine, degree, lo, out, "pcgb_mg_create_index_free", false, true);
 }
 
 int pcgb_mg_create_field(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine,
@@ -2029,6 +2063,7 @@ int pcgb_mg_level_csr(pcgb_mg_t mg, int level, int64_t *d_rowptr, int32_t *d_col
     return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: level %d has no coarse CSR (levels 1 .. %d, not the gathered one)", level,
                 (int)mg->lv.size() - 2);
   const MgLevel &L = mg->lv[(size_t)level];
+  if (L.index_free) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: level %d is index-free (no CSR)", level);
   *nnz = L.P.nnz;
   if (!d_rowptr && !d_col && !d_val) return PCGB_OK;
   if (!d_rowptr || !d_col || !d_val) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: give all three buffers or none");
@@ -2048,6 +2083,19 @@ int pcgb_mg_level_csr(pcgb_mg_t mg, int level, int64_t *d_rowptr, int32_t *d_col
   return PCGB_OK;
 }
 
+int pcgb_mg_level_apply(pcgb_mg_t mg, int level, const double *d_x, double *d_y, void *stream) {
+  PCGB_TRY(require_device());
+  if (!mg || !d_x || !d_y) return fail(PCGB_ERR_ARG, "pcgb_mg_level_apply: null argument");
+  if (level <= 0 || level + 1 >= (int)mg->lv.size() || level == mg->la)
+    return fail(PCGB_ERR_ARG, "pcgb_mg_level_apply: level %d has no coarse operator (levels 1 .. %d, not the gathered one)", level,
+                (int)mg->lv.size() - 2);
+  const MgLevel &L = mg->lv[(size_t)level];
+  const uintptr_t x0 = (uintptr_t)d_x, y0 = (uintptr_t)d_y, nb = (uintptr_t)L.n * sizeof(double);
+  if (x0 < y0 + nb && y0 < x0 + nb) return fail(PCGB_ERR_ARG, "pcgb_mg_level_apply: x and y overlap");
+  const cudaStream_t st = (cudaStream_t)stream;
+  return L.index_free ? hexop_apply(L.H, d_x, d_y, st) : spmv_launch(L.P, d_x, d_y, false, st);
+}
+
 int pcgb_mg_setup_info(pcgb_mg_t mg, double *galerkin_ms, int64_t *element_matrix_peak_bytes) {
   if (!mg) return fail(PCGB_ERR_ARG, "pcgb_mg_setup_info: null argument");
   if (galerkin_ms) *galerkin_ms = mg->galerkin_ms;
@@ -2055,22 +2103,24 @@ int pcgb_mg_setup_info(pcgb_mg_t mg, double *galerkin_ms, int64_t *element_matri
   return PCGB_OK;
 }
 
-int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos, pcgb_halo_t gather,
-                         const double *const *d_own, const double *ke_host, double E, double h, const double *d_minv_fine,
-                         int degree, double lo, pcgb_mg_t *out) {
+namespace {
+// pcgb_mg_create_ranks and (index_free) pcgb_mg_create_ranks_index_free
+int mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos, pcgb_halo_t gather,
+                    const double *const *d_own, const double *ke_host, double E, double h, const double *d_minv_fine, int degree,
+                    double lo, pcgb_mg_t *out, bool index_free, const char *who) {
   PCGB_TRY(require_device());
   if (!s || !box || !level_halos || !gather || !d_own || !ke_host || !d_minv_fine || !out)
-    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: null argument");
-  if (!s->comm || s->comm->nranks < 2) return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the solver has no communicator of 2 or more ranks");
+    return fail(PCGB_ERR_ARG, "%s: null argument", who);
+  if (!s->comm || s->comm->nranks < 2) return fail(PCGB_ERR_ARG, "%s: the solver has no communicator of 2 or more ranks", who);
   if (degree < 1 || !(lo > 0.0 && lo < 1.1) || !(E > 0.0) || !(h > 0.0))
-    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: degree >= 1, 0 < lo < 1.1, E > 0 and h > 0 required");
+    return fail(PCGB_ERR_ARG, "%s: degree >= 1, 0 < lo < 1.1, E > 0 and h > 0 required", who);
   for (int a = 0; a < 3; ++a)
     if (box->ne[a] <= 0 || box->e0[a] < 0 || box->e0[a] + box->ne[a] > box->ng[a])
-      return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the box does not lie in the mesh");
+      return fail(PCGB_ERR_ARG, "%s: the box does not lie in the mesh", who);
   if (3 * hex_geom(box).nfree_nodes != s->n)
-    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the solver's operator has %lld rows, the box %lld", (long long)s->n,
+    return fail(PCGB_ERR_ARG, "%s: the solver's operator has %lld rows, the box %lld", who, (long long)s->n,
                 (long long)(3 * hex_geom(box).nfree_nodes));
-  if (n_ranked < 1) return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the fine level does not coarsen (n_ranked >= 1 required)");
+  if (n_ranked < 1) return fail(PCGB_ERR_ARG, "%s: the fine level does not coarsen (n_ranked >= 1 required)", who);
   // ranked levels 0 .. la: the rank's box halved la times, and the global box around it
   const int la = n_ranked;
   std::vector<pcgb_hex_box> rb{*box};
@@ -2079,7 +2129,7 @@ int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked,
     pcgb_hex_box c = p;
     for (int a = 0; a < 3; ++a) {
       if (p.ne[a] % 2 || p.ne[a] < 4 || p.e0[a] % 2 || p.ng[a] % 2)
-        return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: level %d cannot be halved (ne even and >= 4, e0 and ng even)", l - 1);
+        return fail(PCGB_ERR_ARG, "%s: level %d cannot be halved (ne even and >= 4, e0 and ng even)", who, l - 1);
       c.ng[a] = p.ng[a] / 2; c.e0[a] = p.e0[a] / 2; c.ne[a] = p.ne[a] / 2;
     }
     rb.push_back(c);
@@ -2087,26 +2137,26 @@ int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked,
   for (int l = 1; l <= la; ++l) {
     const pcgb_halo_t hl = level_halos[l - 1];
     if (!hl || hl->comm != s->comm || hl->nlocal != 3 * hex_geom(&rb[(size_t)l]).nfree_nodes)
-      return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the halo of level %d is missing, on another communicator or not of the level's size", l);
+      return fail(PCGB_ERR_ARG, "%s: the halo of level %d is missing, on another communicator or not of the level's size", who, l);
   }
   pcgb_hex_box gb = rb.back();
   for (int a = 0; a < 3; ++a) { gb.e0[a] = 0; gb.ne[a] = gb.ng[a]; }
   std::vector<HexGeom> geo{hex_geom(&gb)};
   const int64_t ng_dofs = 3 * geo[0].nfree_nodes;
   if (ng_dofs > kMgMaxGathered)
-    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the gathered level has %lld dofs (at most %lld)", (long long)ng_dofs, (long long)kMgMaxGathered);
+    return fail(PCGB_ERR_ARG, "%s: the gathered level has %lld dofs (at most %lld)", who, (long long)ng_dofs, (long long)kMgMaxGathered);
   if (gather->comm != s->comm || gather->nlocal != ng_dofs || gather->n_nbr != s->comm->nranks - 1 ||
       gather->m != (int64_t)(s->comm->nranks - 1) * ng_dofs)
-    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the gather plan must list all %lld dofs of the gathered level for every other rank",
+    return fail(PCGB_ERR_ARG, "%s: the gather plan must list all %lld dofs of the gathered level for every other rank", who,
                 (long long)ng_dofs);
   for (int l = 0; l <= la; ++l)
-    if (!d_own[l]) return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: null ownership weights of level %d", l);
+    if (!d_own[l]) return fail(PCGB_ERR_ARG, "%s: null ownership weights of level %d", who, l);
   mg_whole_box_levels(geo);
   if (3 * geo.back().nfree_nodes > kMgMaxCoarse)
-    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: the coarsest level has %lld dofs (at most %d)", (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
-  if ((size_t)la + 1 + geo.size() > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks: more than %d levels", PCGB_MG_MAX_LEVELS);
+    return fail(PCGB_ERR_ARG, "%s: the coarsest level has %lld dofs (at most %d)", who, (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
+  if ((size_t)la + 1 + geo.size() > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "%s: more than %d levels", who, PCGB_MG_MAX_LEVELS);
   pcgb_mg_t mg = new pcgb_mg_s();
-  mg->s = s; mg->degree = degree; mg->lo = lo; mg->la = la; mg->gather = gather;
+  mg->s = s; mg->degree = degree; mg->lo = lo; mg->la = la; mg->gather = gather; mg->index_free = index_free;
   mg->lv.resize((size_t)la + 1 + geo.size());
   for (int l = 0; l <= la; ++l) {
     MgLevel &L = mg->lv[(size_t)l];
@@ -2125,6 +2175,21 @@ int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked,
   s->mgs.push_back(mg);
   *out = mg;
   return PCGB_OK;
+}
+}  // namespace
+
+int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos, pcgb_halo_t gather,
+                         const double *const *d_own, const double *ke_host, double E, double h, const double *d_minv_fine,
+                         int degree, double lo, pcgb_mg_t *out) {
+  return mg_create_ranks(s, box, n_ranked, level_halos, gather, d_own, ke_host, E, h, d_minv_fine, degree, lo, out, false,
+                         "pcgb_mg_create_ranks");
+}
+
+int pcgb_mg_create_ranks_index_free(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos,
+                                    pcgb_halo_t gather, const double *const *d_own, const double *ke_host, double E, double h,
+                                    const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
+  return mg_create_ranks(s, box, n_ranked, level_halos, gather, d_own, ke_host, E, h, d_minv_fine, degree, lo, out, true,
+                         "pcgb_mg_create_ranks_index_free");
 }
 
 int pcgb_mg_apply(pcgb_mg_t mg, const double *d_r, double *d_z, void *stream) {
@@ -2277,24 +2342,16 @@ int pcgb_hexop_create(const pcgb_hex_box *box, const double *ke_host, double ck,
       return fail(PCGB_ERR_ARG, "pcgb_hexop_create: the box must have ne > 0 and lie inside its global mesh on every axis");
   if (!d_ck && !(std::isfinite(ck) && ck > 0.0)) return fail(PCGB_ERR_ARG, "pcgb_hexop_create: Ck must be finite and positive");
   PCGB_TRY(require_device());
-  HexOp H;
-  H.s = hexop_shape(hex_geom(box));
+  const HexOp H = hexop_of(hex_geom(box), ke_host, ck, d_ck);
   const HexGeom &g = H.s.g;
   if ((int64_t)H.s.nbx * H.s.nby * H.s.nbz >= (int64_t)1 << 31) return fail(PCGB_ERR_ARG, "pcgb_hexop_create: box too large");
-  const int64_t ne = (int64_t)g.nx * g.ny * g.nz;
   if (d_ck) {
     // the check runs on the legacy stream, which does not wait for non-blocking streams: finish the caller's writes first
     PCGB_CUDA(cudaDeviceSynchronize());
     int bad = 0;
-    PCGB_TRY(field_bad(ne, d_ck, 0, "pcgb_hexop_create", &bad));
+    PCGB_TRY(field_bad((int64_t)g.nx * g.ny * g.nz, d_ck, 0, "pcgb_hexop_create", &bad));
     if (bad) return fail(PCGB_ERR_ARG, "pcgb_hexop_create: every Ck of the field must be finite and positive");
   }
-  std::memcpy(H.ke.k, ke_host, sizeof(H.ke.k));
-  for (int a = 0; a < 24; ++a) H.kd.k[a] = ke_host[a * 24 + a];
-  H.ck = d_ck ? 0.0 : ck;
-  H.d_ck = d_ck;
-  H.n = 3 * g.nfree_nodes;
-  H.bytes = 16 * H.n + (d_ck ? 8 * ne : 0);
   pcgb_hexop_t h = new pcgb_hexop_s();
   h->H = H;
   *out = h;

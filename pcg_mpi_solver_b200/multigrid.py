@@ -15,6 +15,11 @@ so it is the same operator up to rounding.
 `coarsening="any"` (one rank) accepts a box of any size: every axis is coarsened on its own (`any_levels`), halved to
 (ne + 1) / 2 elements while ne >= 3 and kept once ne <= 2, down to at most 2x2x2 elements, and the coarse levels are always
 Galerkin products of element matrices (pcgb_mg_create_any), with or without `E_field`.
+
+`coarse="index_free"` (default coarsening, no `E_field`; one rank or across ranks) builds the same hierarchy with every
+smoothed coarse level applied by the index-free hex-box operator (csrc/hexop.cuh) instead of a CSR matrix
+(pcgb_mg_create_index_free / pcgb_mg_create_ranks_index_free): the hierarchy then holds only vectors and the coarsest
+factor (`index_free_bytes`), which is what lets MG-PCG run a 512^3 box on one 80 GB GPU.
 """
 from __future__ import annotations
 
@@ -53,6 +58,20 @@ def any_levels(ne, max_levels: int = _lib.MG_MAX_LEVELS) -> list:
     if len(out) < 2:
         raise ValueError(f"HexMultigrid: the box {tuple(ne)} does not coarsen (some ne must be >= 3)")
     return out
+
+
+def index_free_bytes(ne) -> int:
+    """Device bytes pcgb_mg_info reports for the one-rank index-free hierarchy of the whole box `ne` (default coarsening):
+    8 (5 n_0 + 6 sum n_l over the smoothed coarse levels + 2 n_c + n_c^2) - the fine level's z, D^-1 and three smoother
+    vectors, each coarse level's b, x, D^-1 and three smoother vectors, the coarsest b, x and dense factor.  The few
+    fixed-size reduction buffers are not counted.  Raises ValueError where pcgb_mg_create_index_free refuses the box."""
+    lv = _whole_levels(ne)
+    if len(lv) < 2:
+        raise ValueError(f"HexMultigrid: the box {tuple(ne)} does not coarsen (every ne must be even and >= 4)")
+    n = [3 * v[0] * (v[1] + 1) * (v[2] + 1) for v in lv]
+    if n[-1] > MAX_COARSE:
+        raise ValueError(f"HexMultigrid: the coarsest level has {n[-1]} dofs (at most {MAX_COARSE})")
+    return 8 * (5 * n[0] + 6 * sum(n[1:-1]) + 2 * n[-1] + n[-1] ** 2)
 
 
 def rank_levels(blocks) -> list:
@@ -101,10 +120,15 @@ class HexMultigrid:
     coarsening (one rank only): "even" (the default, above) or "any": a box of any size, each axis halved or kept on its own
     (`any_levels`), Galerkin levels from E_field or, without it, from Ck = block.E * block.h on every element
     (pcgb_mg_create_any).  "any" builds 4608 bytes of element matrices per level-1 element during the set-up and sets up
-    slower than the rediscretised default.  Any other string, or "any" with a multi-rank `op`, raises ValueError."""
+    slower than the rediscretised default.  Any other string, or "any" with a multi-rank `op`, raises ValueError.
+
+    coarse: "csr" (the default: every smoothed coarse level a device-generated CSR matrix) or "index_free" (those levels
+    applied by the index-free hex-box operator, Ck = block.E 2^l block.h; `index_free_bytes` gives the one-rank hierarchy's
+    device bytes).  "index_free" with E_field or coarsening="any" raises ValueError, as does any other string: Galerkin
+    coarse matrices and odd or kept axes are not one Ke on one box."""
 
     def __init__(self, op, block: HexBlock, degree: int = 2, lo: float = 0.25, minv: torch.Tensor | None = None, blocks=None,
-                 E_field=None, coarsening: str = "even"):
+                 E_field=None, coarsening: str = "even", coarse: str = "csr"):
         self.op, self.block, self.degree, self.lo = op, block, int(degree), float(lo)
         self.n = op.n
         self.device = op.device
@@ -116,6 +140,13 @@ class HexMultigrid:
         if coarsening not in ("even", "any"):
             raise ValueError(f"HexMultigrid: coarsening must be 'even' or 'any', not {coarsening!r}")
         self.coarsening = coarsening
+        if coarse not in ("csr", "index_free"):
+            raise ValueError(f"HexMultigrid: coarse must be 'csr' or 'index_free', not {coarse!r}")
+        if coarse == "index_free" and (E_field is not None or coarsening == "any"):
+            raise ValueError("HexMultigrid: coarse='index_free' needs the default coarsening and no E_field "
+                             "(Galerkin coarse levels are not one element matrix on one box)")
+        self.coarse = coarse
+        index_free = coarse == "index_free"
         if coarsening == "any":
             if ranked:
                 raise ValueError("HexMultigrid: coarsening='any' is supported on one rank only")
@@ -157,8 +188,9 @@ class HexMultigrid:
         lib = _lib.load()
         with torch.cuda.device(self.device):
             if not ranked:
-                _lib.check(lib.pcgb_mg_create(op._solver, ctypes.byref(box), kep, float(block.E), float(block.h), _lib.ptr(minv),
-                                              self.degree, self.lo, ctypes.byref(self._h)), "pcgb_mg_create")
+                name = "pcgb_mg_create_index_free" if index_free else "pcgb_mg_create"
+                _lib.check(getattr(lib, name)(op._solver, ctypes.byref(box), kep, float(block.E), float(block.h), _lib.ptr(minv),
+                                              self.degree, self.lo, ctypes.byref(self._h)), name)
                 return
             from .solver import make_halo
             la = len(self.levels) - 1
@@ -177,9 +209,9 @@ class HexMultigrid:
             halos = (ctypes.c_void_p * la)(*[h.value for h in self._halos[:la]])
             owns = (ctypes.c_void_p * (la + 1))(*[t.data_ptr() for t in own])
             torch.cuda.synchronize(self.device)
-            _lib.check(lib.pcgb_mg_create_ranks(op._solver, ctypes.byref(box), la, halos, self._gather, owns, kep,
-                                                float(block.E), float(block.h), _lib.ptr(minv), self.degree, self.lo,
-                                                ctypes.byref(self._h)), "pcgb_mg_create_ranks")
+            name = "pcgb_mg_create_ranks_index_free" if index_free else "pcgb_mg_create_ranks"
+            _lib.check(getattr(lib, name)(op._solver, ctypes.byref(box), la, halos, self._gather, owns, kep, float(block.E),
+                                          float(block.h), _lib.ptr(minv), self.degree, self.lo, ctypes.byref(self._h)), name)
 
     @property
     def handle(self):
@@ -197,8 +229,9 @@ class HexMultigrid:
 
     def info(self) -> dict:
         """levels, n per level, largest-eigenvalue estimates of D^-1 A per level (0 for the coarsest and for the gathered
-        level), device bytes; across ranks also gather_level (la, -1 on one rank), n_gathered and global_lambda (the
-        estimates of the global hierarchy: ranked levels below la, then the replicated ones)."""
+        level), device bytes, coarse ("csr" or "index_free"); across ranks also gather_level (la, -1 on one rank),
+        n_gathered and global_lambda (the estimates of the global hierarchy: ranked levels below la, then the replicated
+        ones)."""
         lib = _lib.load()
         nl = ctypes.c_int32()
         n = (ctypes.c_int64 * _lib.MG_MAX_LEVELS)()
@@ -209,7 +242,7 @@ class HexMultigrid:
         _lib.check(lib.pcgb_mg_info_ranks(self._h, ctypes.byref(la), ctypes.byref(ng)), "pcgb_mg_info_ranks")
         k = nl.value
         lams = [float(v) for v in lam[:k]]
-        out = {"levels": k, "n": [int(v) for v in n[:k]], "lambda": lams, "bytes": int(nb.value)}
+        out = {"levels": k, "n": [int(v) for v in n[:k]], "lambda": lams, "bytes": int(nb.value), "coarse": self.coarse}
         if la.value >= 0:
             out.update(gather_level=la.value, n_gathered=int(ng.value), global_lambda=lams[:la.value] + lams[la.value + 1:])
         return out
@@ -246,6 +279,14 @@ class HexMultigrid:
             _lib.check(lib.pcgb_mg_level_csr(self._h, level, _lib.ptr(rowptr), _lib.ptr(col), _lib.ptr(val), ctypes.byref(nnz),
                                              _lib.stream_ptr()), "pcgb_mg_level_csr")
         return rowptr, col, val
+
+    def level_apply(self, level: int, x: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
+        """y = A_l x on smoothed coarse level `level` (1 .. levels - 2, not the gathered level), either coarse kind: the
+        local product, without the level's exchange-add across ranks (x and out must not overlap)."""
+        y = out if out is not None else self._vec(self.info()["n"][level])
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().pcgb_mg_level_apply(self._h, level, _lib.ptr(x), _lib.ptr(y), _lib.stream_ptr()), "pcgb_mg_level_apply")
+        return y
 
     def restrict(self, level: int, rf: torch.Tensor) -> torch.Tensor:
         rc = self._vec(self.info()["n"][level + 1])

@@ -1,11 +1,13 @@
 """Time to solution of Jacobi-PCG against multigrid-preconditioned PCG (HexMultigrid) on the bench's hex box.
 
-    python tools/gmg_bench.py --block 128 --tol 1e-8 [--operator csr|ebe_ordered|ebe] [--repeats 3]
+    python tools/gmg_bench.py --block 128 --tol 1e-8 [--operator csr|ebe_ordered|ebe|hexop] [--coarse csr|index_free] [--repeats 3]
     python tools/gmg_bench.py --shape 200,150,75 --coarsening any
 
 --shape NX,NY,NZ replaces the cubic --block box (h = 1 / NX); --coarsening any builds HexMultigrid(coarsening="any"), which
 accepts any box.  Either option adds the level boxes, the Galerkin kernels' device time and the element-matrix peak of
-`setup_info` to the multigrid line; without them the output is unchanged.
+`setup_info` to the multigrid line; without them the output is unchanged.  --operator hexop runs on the index-free fine
+operator (HexBoxOperator); --coarse index_free builds HexMultigrid(coarse="index_free"), whose coarse levels are
+index-free too (the multigrid line then carries "coarse").
 
 For each arm: iterations, flag, the device time of the loop (CUDA events inside the solve), the host wall time of the whole
 solve (ending in a device synchronise), and for the multigrid arm its set-up time, the V-cycle time per application
@@ -38,7 +40,8 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--block", type=int, default=128)
     ap.add_argument("--tol", type=float, default=1e-8)
-    ap.add_argument("--operator", choices=["csr", "ebe_ordered", "ebe"], default="csr")
+    ap.add_argument("--operator", choices=["csr", "ebe_ordered", "ebe", "hexop"], default="csr")
+    ap.add_argument("--coarse", choices=["csr", "index_free"], default="csr")
     ap.add_argument("--degree", type=int, default=2)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--vcycles", type=int, default=50)
@@ -52,7 +55,7 @@ def main():
     import torch
     if not torch.cuda.is_available():
         sys.exit("gmg_bench: needs a CUDA device")
-    from pcg_mpi_solver_b200.hexmesh import HexBlock, generate_ebe, generate_matrix, load_vector
+    from pcg_mpi_solver_b200.hexmesh import HexBlock, generate_box_operator, generate_ebe, generate_matrix, load_vector
     from pcg_mpi_solver_b200.multigrid import HexMultigrid
     from pcg_mpi_solver_b200.solver import SubdomainOperator
     dev = torch.device("cuda:0")
@@ -61,6 +64,9 @@ def main():
     if a.operator == "csr":
         A = generate_matrix(blk, device=dev)
         op_bytes = A.val.numel() * 12 + A.rowptr.numel() * A.rowptr.element_size()
+    elif a.operator == "hexop":
+        A = generate_box_operator(blk, device=dev)
+        op_bytes = 0                                           # Ke is a launch parameter; no device arrays
     else:
         A = generate_ebe(blk, device=dev, ordered=a.operator == "ebe_ordered")
         op_bytes = int(A.bytes()) if hasattr(A, "bytes") else None
@@ -71,7 +77,7 @@ def main():
     torch.cuda.empty_cache()
     free0, _ = torch.cuda.mem_get_info(dev)
     t0 = time.perf_counter()
-    mg = HexMultigrid(op, blk, degree=a.degree, minv=minv, coarsening=a.coarsening)
+    mg = HexMultigrid(op, blk, degree=a.degree, minv=minv, coarsening=a.coarsening, coarse=a.coarse)
     torch.cuda.synchronize()
     setup_s = time.perf_counter() - t0
     free_drop = free0 - torch.cuda.mem_get_info(dev)[0]    # everything create took, the SpMV plans' tables included
@@ -115,6 +121,7 @@ def main():
                       "n_levels": info["n"], "lambda": [round(v, 4) for v in info["lambda"]], "hierarchy_bytes": info["bytes"], "device_free_drop_bytes": free_drop,
                       "fine_operator_bytes": op_bytes, "speedup_wall": round(wj / wm, 2),
                       "x_rel_diff_vs_jacobi": diff,
+                      **({"coarse": a.coarse} if a.coarse != "csr" else {}),
                       **({"level_shapes": [list(v) for v in mg.level_shapes()], **mg.setup_info()} if extra else {})}))
 
 

@@ -1,13 +1,14 @@
 """Jacobi-PCG against multigrid-preconditioned PCG across ranks on the bench's weak-scaled hex stacks (one box of
 --block^3 elements per rank, hexmesh.block_grid / partition_blocks), one GPU per rank.
 
-    torchrun --nproc-per-node 8 tools/gmg_dd_bench.py --block 128 --tol 1e-8 [--operator csr|ebe_ordered|ebe]
+    torchrun --nproc-per-node 8 tools/gmg_dd_bench.py --block 128 --tol 1e-8 [--operator csr|ebe_ordered|ebe] [--coarse csr|index_free]
 
 For each arm, per rank: iterations, flag, the device time of the loop (CUDA events inside the solve), the host wall time
 of the whole solve (ending in a device synchronise and a barrier), and for the multigrid arm its set-up time and the
 V-cycle time per application (CUDA events around `pcgb_mg_apply`).  Rank 0 prints one JSON line per arm with every
 rank's numbers and the card's name, SM clock limit and power limit.  Ranks sharing one GPU (PCGB_SHARED_GPU=1) run, but
-their times say nothing about speed.
+their times say nothing about speed.  --coarse index_free builds HexMultigrid(coarse="index_free"): index-free ranked and
+replicated coarse levels.
 """
 import argparse
 import datetime
@@ -29,6 +30,7 @@ def main():
     ap.add_argument("--degree", type=int, default=2)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--vcycles", type=int, default=20)
+    ap.add_argument("--coarse", choices=["csr", "index_free"], default="csr")
     a = ap.parse_args()
     import torch
     import torch.distributed as dist
@@ -61,7 +63,7 @@ def main():
     torch.cuda.synchronize()
     dist.barrier()
     t0 = time.perf_counter()
-    mg = HexMultigrid(op, blk, degree=a.degree, minv=minv, blocks=blocks)
+    mg = HexMultigrid(op, blk, degree=a.degree, minv=minv, blocks=blocks, coarse=a.coarse)
     torch.cuda.synchronize()
     setup_s = time.perf_counter() - t0
     info = mg.info()
@@ -99,7 +101,7 @@ def main():
     box = [None] * world
     dist.all_gather_object(box, mine)
     if rank == 0:
-        common = {"ranks": world, "pgrid": list(pgrid), "block": a.block, "operator": a.operator, "tol": a.tol, "card": card(),
+        common = {"ranks": world, "pgrid": list(pgrid), "block": a.block, "operator": a.operator, "coarse": a.coarse, "tol": a.tol, "card": card(),
                   "shared_gpu": shared}
         print(json.dumps({**common, "arm": "jacobi", "per_rank": [m["jacobi"] for m in box]}))
         print(json.dumps({**common, "arm": "multigrid", "degree": a.degree, "levels": info["levels"], "gather_level": info["gather_level"],
