@@ -284,9 +284,16 @@ int pcgb_assemble_symbolic(int64_t n, int ngroups, const pcgb_ebe_group *groups,
 int pcgb_assemble_numeric(pcgb_asm_t a, const int64_t *d_rowptr, int32_t *d_col, double *d_val, void *stream);
 int pcgb_assemble_destroy(pcgb_asm_t a);
 
-/* Operator-level (not reachable from pcgb_solve; tests/test_gpu_ebe_colored.py): the same operator
- * with an atomics-free deterministic scatter.  groups[] = one entry per (pattern group, colour) slice, sorted by
- * colour; phase[g] = colour of entry g; no two elements of one colour may share a dof (coloring.py).            */
+/* Operator-level (not reachable from pcgb_solve; tests/test_gpu_ebe_colored.py, tests/test_gpu_ebe_color_edges.py): the
+ * same operator with an atomics-free deterministic scatter.  groups[] = one entry per (pattern group, colour) slice, sorted
+ * by colour (PCGB_ERR_ARG otherwise); phase[g] = colour of entry g.  No two elements of one colour may share a free dof;
+ * create TRUSTS the caller's phases to be such a colouring and does not check it (EbeMatrixColored checks it on the host).
+ * Ke is row-major, Ke[i][j] = ke_host[i*nd + j], and need not be symmetric.  Apply gives, bit for bit:
+ *   for every free dof d, y_d starts from +0.0; the colours are taken in ascending order, and for the one element e of
+ *   that colour that touches d, every local index i with idx[i] = d, in ascending i, does y_d = y_d + v_{e,i}, where
+ *     u_j = s_j x_j (0.0 for a clamped dof),  acc = fma(Ke[i][j], u_j, acc) over j ascending from 0.0,
+ *     v_{e,i} = round(acc * Ck_e), negated when s_i is set.
+ *   Every y_d is written, +0.0 when no element touches d.                                                         */
 int pcgb_ebe2_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, const int32_t *phase, pcgb_ebe2_t *out);
 int pcgb_ebe2_destroy(pcgb_ebe2_t E);
 int pcgb_ebe2_apply(pcgb_ebe2_t E, const double *d_x, double *d_y, void *stream);

@@ -59,6 +59,41 @@ def color_elements(elem_nodes: np.ndarray, elem_ptr: np.ndarray | None = None, n
     return colors, c
 
 
+def color_groups(groups, ndof: int):
+    """Colour the elements of all pattern groups together on the node of EVERY local dof (node = dof // 3).  Two elements
+    that share a dof share its node, whatever order a pattern lists its dofs in, so no dof is shared inside a colour.
+    (For node-major patterns, local dof j = 3 node[j // 3] + j % 3, the node sets and so the colours are those of the
+    first dof of every triple.)  Returns (colors per group, ncolors)."""
+    flat = np.concatenate([(g.loc_dof // 3).T.ravel() for g in groups]) if groups else np.zeros(0, np.int64)
+    counts = np.concatenate([np.full(g.loc_dof.shape[1], g.loc_dof.shape[0], dtype=np.int64) for g in groups]) if groups else np.zeros(0, np.int64)
+    ptr = np.concatenate([[0], np.cumsum(counts)])
+    colors, ncolors = color_elements(flat, ptr, ndof // 3 + 1)
+    split = np.cumsum([g.loc_dof.shape[1] for g in groups])[:-1]
+    return np.split(colors, split), ncolors
+
+
+def color_conflicts(idx_per_group, colors_per_group, n: int) -> int:
+    """Number of (colour, free dof) pairs that two different elements of one colour touch; 0 for a valid colouring.
+    idx_per_group: (nd, ne) dof indices in the free numbering (-1 = clamped); an element's own repeats do not count."""
+    dofs, cols = [np.zeros(0, np.int64)], [np.zeros(0, np.int64)]
+    for idx, col in zip(idx_per_group, colors_per_group):
+        if idx.shape[1] == 0:
+            continue
+        s = np.sort(idx, axis=0)
+        keep = s >= 0
+        keep[1:] &= s[1:] != s[:-1]                  # each element's distinct free dofs once
+        dofs.append(s[keep].astype(np.int64))
+        cols.append(np.broadcast_to(np.asarray(col, dtype=np.int64)[None, :], s.shape)[keep])
+    dofs, cols = np.concatenate(dofs), np.concatenate(cols)
+    order = np.argsort(cols, kind="stable")
+    cuts = np.nonzero(np.diff(cols[order]))[0] + 1
+    bad = 0
+    for part in np.split(order, cuts):
+        if part.size:
+            bad += int((np.bincount(dofs[part], minlength=n) > 1).sum())
+    return bad
+
+
 def hex_parity_colors(ex: np.ndarray, ey: np.ndarray, ez: np.ndarray):
     """The optimal 8-colouring of a structured hex mesh: colour = parity of the element coordinates."""
     return ((ex & 1) | ((ey & 1) << 1) | ((ez & 1) << 2)).astype(np.uint8), 8

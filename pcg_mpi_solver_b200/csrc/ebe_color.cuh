@@ -1,10 +1,16 @@
-// ebe_color.cuh - operator-level variant (tests/test_gpu_ebe_colored.py):
+// ebe_color.cuh - operator-level variant (tests/test_gpu_ebe_colored.py, tests/test_gpu_ebe_color_edges.py):
 // atomics-free, bit-reproducible variant of the matrix-free operator of ebe.cuh.  The host colours the elements
-// (pcg_mpi_solver_b200/coloring.py: no two elements of a colour share a node) and passes every (pattern group,
+// (pcg_mpi_solver_b200/coloring.py: no two elements of a colour share a free dof) and passes every (pattern group,
 // colour) slice as its own group, ordered by colour ("phase").  Inside one phase the scatter y[dof] += v needs no
 // atomic; phases run as consecutive launches, so the summation order per dof is fixed (colour order) - the
 // deterministic counterpart of np.bincount (pcg_solver.py:300).  Rationale: DESIGN.md section 6 item 1 - the 24
 // fp64 RED per element are ~80 % of the first EBE kernel's time.
+//
+// The result, bit for bit (include/pcgb200.h): every free dof d starts from +0.0; colours are taken in ascending order,
+// and for the one element e of the colour that touches d, every local index i with idx[i] = d in ascending i does
+// y_d = y_d + v_{e,i}, where u_j = s_j x_j (0 for a clamped dof), acc = fma(Ke[i][j], u_j, acc) over j ascending from
+// 0.0 and v = round(acc * Ck_e), negated when s_i is set.  Every operation of the scatter is an explicit __dmul_rn /
+// __dadd_rn so that contraction cannot fuse it into an fma (hexop.cuh does the same).
 #pragma once
 #include <vector>
 
@@ -19,7 +25,7 @@ struct EbeLaunch {
 };
 
 struct EbeColorPlan {
-  EbePlan P;                       // groups (one per pattern group x colour), device tables
+  EbePlan P;                       // groups (one per pattern group x colour), device tables; each ke is Ke TRANSPOSED
   std::vector<EbeLaunch> launches; // in phase order
 };
 
@@ -45,16 +51,20 @@ k_ebe_t24p(const int *__restrict__ idx, const unsigned char *__restrict__ sign, 
     double acc = 0.0;
 #pragma unroll
     for (int j = 0; j < 24; ++j) acc = fma(c_ebe_ke24[slot][i * 24 + j], u[j], acc);
-    acc *= c;
-    if (SIGN && ((sbits >> i) & 1u)) acc = -acc;
-    if (id[i] >= 0) y[id[i]] += acc;   // no other element of this colour touches this dof
-  }
+    double v = __dmul_rn(acc, c);
+    if (SIGN && ((sbits >> i) & 1u)) v = -v;
+    if (id[i] >= 0) y[id[i]] = __dadd_rn(y[id[i]], v);   // no other element of this colour touches this dof; an element's
+  }                                                        // own repeats come in ascending i from this one thread
 }
 
+// One warp per element.  The rows go to shared memory first; then the lane of a dof's FIRST local index adds every
+// occurrence of that dof in ascending local index, so an element that lists a dof twice (in one 32-lane pass or in two)
+// loses no update and sums it in the documented order.
 __global__ void __launch_bounds__(kEbeWarpsPerBlock * 32)
 k_ebe_warp_p(const EbeGroup *__restrict__ groups, const int *__restrict__ blk_group, const int64_t *__restrict__ blk_e0, int blk0,
              const double *__restrict__ x, double *__restrict__ y) {
   __shared__ double su[kEbeWarpsPerBlock][96];
+  __shared__ double sv[kEbeWarpsPerBlock][96];
   __shared__ int sid[kEbeWarpsPerBlock][96];
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int blk = blk0 + blockIdx.x;
@@ -62,24 +72,35 @@ k_ebe_warp_p(const EbeGroup *__restrict__ groups, const int *__restrict__ blk_gr
   const int64_t e = blk_e0[blk] + warp;
   if (e >= g.ne) return;
   const int nd = g.nd;
-  for (int j = lane; j < nd; j += 32) {
+  unsigned sneg = 0;   // bit k: sign of local index lane + 32 k (the gather and the rows visit the same indices per lane)
+  for (int j = lane, k = 0; j < nd; j += 32, ++k) {
     const int id = g.idx[(int64_t)j * g.ne + e];
     double v = id >= 0 ? __ldg(x + id) : 0.0;
     const bool s = g.sign != nullptr && g.sign[(int64_t)j * g.ne + e] != 0;
     su[warp][j] = s ? -v : v;
-    sid[warp][j] = s ? (id | (int)0x40000000) : id;
+    sid[warp][j] = id;
+    if (s) sneg |= 1u << k;
   }
   __syncwarp();
   const double c = g.ck[e];
-  for (int i = lane; i < nd; i += 32) {
+  for (int i = lane, k = 0; i < nd; i += 32, ++k) {
     double acc = 0.0;
-    for (int j = 0; j < nd; ++j) acc = fma(__ldg(g.ke + (int64_t)j * nd + i), su[warp][j], acc);
-    acc *= c;
-    int id = sid[warp][i];
-    if (id >= 0) {
-      if (id & 0x40000000) { acc = -acc; id &= 0x3fffffff; }
-      y[id] += acc;
-    }
+    for (int j = 0; j < nd; ++j) acc = fma(__ldg(g.ke + (int64_t)j * nd + i), su[warp][j], acc);   // ke = Ke^T: row i of Ke
+    double v = __dmul_rn(acc, c);
+    if ((sneg >> k) & 1u) v = -v;
+    sv[warp][i] = v;
+  }
+  __syncwarp();
+  for (int i = lane; i < nd; i += 32) {
+    const int id = sid[warp][i];
+    if (id < 0) continue;
+    int j = 0;
+    while (sid[warp][j] != id) ++j;
+    if (j < i) continue;                 // not the first occurrence: that lane adds this one
+    double yv = __dadd_rn(y[id], sv[warp][i]);
+    for (j = i + 1; j < nd; ++j)
+      if (sid[warp][j] == id) yv = __dadd_rn(yv, sv[warp][j]);
+    y[id] = yv;
   }
 }
 

@@ -643,12 +643,20 @@ static int check_group(const pcgb_ebe_group &src, int g, int max_nd, int64_t max
   return PCGB_OK;
 }
 
-// device copy of the group's pattern matrix Ke (nd x nd)
-static int upload_ke(const pcgb_ebe_group &src, const double **d_ke, const char *who) {
+// device copy of the group's pattern matrix Ke (nd x nd), or of its transpose
+static int upload_ke(const pcgb_ebe_group &src, const double **d_ke, const char *who, bool transpose = false) {
   const size_t bytes = (size_t)src.nd * src.nd * sizeof(double);
+  std::vector<double> kt;
+  const double *h = src.ke_host;
+  if (transpose) {
+    kt.resize((size_t)src.nd * src.nd);
+    for (int i = 0; i < src.nd; ++i)
+      for (int j = 0; j < src.nd; ++j) kt[(size_t)j * src.nd + i] = src.ke_host[(size_t)i * src.nd + j];
+    h = kt.data();
+  }
   double *d = nullptr;
   cudaError_t ce = cudaMalloc(&d, bytes);
-  if (ce == cudaSuccess) ce = cudaMemcpy(d, src.ke_host, bytes, cudaMemcpyHostToDevice);
+  if (ce == cudaSuccess) ce = cudaMemcpy(d, h, bytes, cudaMemcpyHostToDevice);
   if (ce != cudaSuccess) { cudaFree(d); return fail(PCGB_ERR_CUDA, "%s: %s", who, cudaGetErrorString(ce)); }
   *d_ke = d;
   return PCGB_OK;
@@ -656,8 +664,10 @@ static int upload_ke(const pcgb_ebe_group &src, const double **d_ke, const char 
 
 // Groups of an EBE plan (atomic, ordered or coloured operator): device copies of Ke, constant-memory slots of the 24-dof
 // patterns, the warp-kernel block tables (blocks in group order).  On failure P holds what was acquired so far, which
-// ebe_plan_free releases.
-static int ebe_plan_build(EbePlan &P, int64_t n, int ngroups, const pcgb_ebe_group *groups, const char *who) {
+// ebe_plan_free releases.  ke_transposed: the device copies hold Ke^T, so that a warp kernel reading column i of the copy
+// (coalesced across lanes) gets row i of Ke.
+static int ebe_plan_build(EbePlan &P, int64_t n, int ngroups, const pcgb_ebe_group *groups, const char *who,
+                          bool ke_transposed = false) {
   P.n = n;
   std::vector<int> blk_group;
   std::vector<int64_t> blk_e0;
@@ -667,7 +677,7 @@ static int ebe_plan_build(EbePlan &P, int64_t n, int ngroups, const pcgb_ebe_gro
     PCGB_TRY(check_group(src, g, 96, INT64_MAX, who));
     EbeGroup eg;
     eg.nd = src.nd; eg.ne = src.ne; eg.idx = src.d_idx; eg.sign = src.d_sign; eg.ck = src.d_ck;
-    PCGB_TRY(upload_ke(src, &eg.ke, who));
+    PCGB_TRY(upload_ke(src, &eg.ke, who, ke_transposed));
     if (src.nd == 24) eg.slot = ebe_slot_acquire(src.ke_host);
     if (eg.slot < 0)
       for (int64_t e0 = 0; e0 < src.ne; e0 += kEbeWarpsPerBlock) { blk_group.push_back((int)P.groups.size()); blk_e0.push_back(e0); }
@@ -801,7 +811,8 @@ int pcgb_assemble_destroy(pcgb_asm_t a) {
 
 // ------------------------------------------------------------------------------------ coloured EBE operator (operator level)
 // groups[] holds one entry per (pattern group, colour), sorted by colour; phase[g] is the colour.  Pattern matrices of
-// the 24-dof groups are de-duplicated into the constant-memory slots by content of ke_host.
+// the 24-dof groups are de-duplicated into the constant-memory slots by content of ke_host.  The colouring itself is
+// trusted (EbeMatrixColored checks it on the host).
 int pcgb_ebe2_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, const int32_t *phase, pcgb_ebe2_t *out) {
   if (!out || n < 0 || ngroups < 0 || (ngroups > 0 && (!groups || !phase))) return fail(PCGB_ERR_ARG, "pcgb_ebe2_create: bad argument");
   if (n >= (1 << 30)) return fail(PCGB_ERR_ARG, "pcgb_ebe2_create: more than 2^30 dofs");
@@ -810,12 +821,12 @@ int pcgb_ebe2_create(int64_t n, int ngroups, const pcgb_ebe_group *groups, const
     if (phase[g] < phase[g - 1]) return fail(PCGB_ERR_ARG, "pcgb_ebe2_create: groups must be sorted by phase (colour)");
   pcgb_ebe2_t E = new pcgb_ebe2_s();
   cudaGetDevice(&E->device);
-  const int rc = ebe_plan_build(E->C.P, n, ngroups, groups, "pcgb_ebe2_create");
+  const int rc = ebe_plan_build(E->C.P, n, ngroups, groups, "pcgb_ebe2_create", true);
   if (rc != PCGB_OK) { pcgb_ebe2_destroy(E); return rc; }
   // Launches in colour order: the colour's t24 groups in group order, then one warp launch over the colour's blocks, which
   // are contiguous in the block tables because the groups arrive sorted by colour.  A t24 launch and a warp launch of one
   // colour may touch the same dofs only if the colouring was done per pattern group; the Python side colours ALL elements
-  // of the subdomain together, so they cannot.
+  // of the subdomain together and checks that no free dof is shared inside a colour, so they cannot.
   int blk = 0;
   for (int g = 0; g < ngroups;) {
     const int blk0 = blk;
@@ -838,7 +849,7 @@ int pcgb_ebe2_destroy(pcgb_ebe2_t E) {
 }
 
 int pcgb_ebe2_apply(pcgb_ebe2_t E, const double *d_x, double *d_y, void *stream) {
-  if (!E || !d_x || !d_y) return fail(PCGB_ERR_ARG, "pcgb_ebe2_apply: null argument");
+  if (!E || (E->C.P.n > 0 && (!d_x || !d_y))) return fail(PCGB_ERR_ARG, "pcgb_ebe2_apply: null argument");   // n = 0: no vector
   return ebe_color_apply(E->C, d_x, d_y, (cudaStream_t)stream);
 }
 

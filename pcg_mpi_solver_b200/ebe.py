@@ -103,36 +103,51 @@ class EbeMatrixOrdered(EbeMatrix):
 
 
 class EbeMatrixColored:
-    """Operator-level variant (tests/test_gpu_ebe_colored.py): the same operator with an atomics-free,
-    bit-reproducible scatter.  All elements of the subdomain are coloured together (coloring.color_elements: no two
-    elements of a colour share a node), every (pattern group, colour) slice becomes its own group, slices are passed
-    in colour order and the kernels of one colour use plain `y[dof] += v` (csrc/ebe_color.cuh)."""
+    """Operator-level variant (tests/test_gpu_ebe_colored.py, tests/test_gpu_ebe_color_edges.py): the same operator with
+    an atomics-free, bit-reproducible scatter.  All elements of the subdomain are coloured together
+    (coloring.color_groups: on the node of every local dof, so that no two elements of a colour share a dof), every
+    (pattern group, colour) slice becomes its own group, slices are passed in colour order and the kernels of one colour
+    use plain `y[dof] += v` (csrc/ebe_color.cuh).
+
+    The result, bit for bit (include/pcgb200.h): every free dof d starts from +0.0; the colours are taken in ascending
+    order, and for the one element e of that colour that touches d, every local index i with idx[i] = d, in ascending i,
+    does y_d = y_d + v_{e,i}, with u_j = s_j x_j (0.0 for a clamped dof), acc = fma(Ke[i][j], u_j, acc) over j ascending
+    from 0.0, and v_{e,i} = round(acc * Ck_e), negated when s_i is set.
+
+    `colors_per_group` (one integer array of ne_g colours per group) replaces the computed colouring.  Either colouring is
+    checked before anything reaches the device: ValueError when two different elements of one colour touch the same
+    free dof (an element may list a dof more than once), and ValueError for a pattern matrix that is not symmetric, as
+    EbeMatrix.  pcgb_ebe2_create itself trusts the phases it is given."""
 
     def __init__(self, groups, loc_dof_eff: np.ndarray, ndof: int, device="cuda", colors_per_group=None):
-        from .coloring import color_elements
+        from .coloring import color_conflicts, color_groups
         self.device = torch.device(device)
         n = int(len(loc_dof_eff))
         self.shape = (n, n)
         eff_map = np.full(ndof, -1, dtype=np.int32)
         eff_map[loc_dof_eff] = np.arange(n, dtype=np.int32)
+        for g in groups:
+            ke = np.asarray(g.ke, dtype=np.float64)
+            if not np.allclose(ke, ke.T, rtol=1e-12, atol=1e-12 * np.abs(ke).max()):
+                raise ValueError("EbeMatrixColored: pattern matrices must be symmetric")
         if colors_per_group is None:
-            # element -> node lists over ALL groups (dofs come in triples per node: node = dof // 3; a pattern whose size is
-            # not a multiple of 3 ends with a partial node, which row 3k still names)
-            flat = np.concatenate([(g.loc_dof[0::3, :] // 3).T.ravel() for g in groups])
-            counts = np.concatenate([np.full(g.loc_dof.shape[1], (g.loc_dof.shape[0] + 2) // 3, dtype=np.int64) for g in groups])
-            ptr = np.concatenate([[0], np.cumsum(counts)])
-            colors, ncolors = color_elements(flat, ptr, ndof // 3 + 1)
-            split = np.cumsum([g.loc_dof.shape[1] for g in groups])[:-1]
-            colors_per_group = np.split(colors, split)
+            colors_per_group, ncolors = color_groups(groups, ndof)
         else:
-            ncolors = int(max(int(c.max()) for c in colors_per_group if c.size) + 1)
+            colors_per_group = [np.asarray(c) for c in colors_per_group]
+            if len(colors_per_group) != len(groups) or any(c.shape != (g.loc_dof.shape[1],) or (c.size and (c.dtype.kind not in "iu" or c.min() < 0))
+                                                           for g, c in zip(groups, colors_per_group)):
+                raise ValueError("EbeMatrixColored: colors_per_group needs one array of non-negative integer colours per element of every group")
+            ncolors = int(max([int(c.max()) for c in colors_per_group if c.size], default=-1) + 1)
+        idx_per_group = [eff_map[g.loc_dof] for g in groups]
+        bad = color_conflicts(idx_per_group, colors_per_group, n)
+        if bad:
+            raise ValueError(f"EbeMatrixColored: {bad} free dofs are touched by two elements of one colour")
         self.ncolors = ncolors
         self._keep = []
         entries = []     # (colour, nd, ne, d_idx, d_sign, d_ck, ke)
-        for g, col in zip(groups, colors_per_group):
+        for g, col, idx_all in zip(groups, colors_per_group, idx_per_group):
             ke = np.ascontiguousarray(g.ke, dtype=np.float64)   # ONE array per pattern group: its address identifies the pattern
             self._keep.append(ke)
-            idx_all = eff_map[g.loc_dof].astype(np.int32)
             has_sign = bool(g.sign.any())
             for c in range(ncolors):
                 sel = np.nonzero(col == c)[0]

@@ -1,5 +1,5 @@
 """Quick timing of the experimental EBE operator against the CSR kernel on the 128^3 hex box (1 GPU)."""
-import json, sys, time
+import gc, json, sys, time
 sys.path.insert(0, ".")
 import numpy as np, torch
 from pcg_mpi_solver_b200.hexmesh import HexBlock, generate_ebe
@@ -34,9 +34,32 @@ e0.record()
 for _ in range(20): C.apply_local(x)
 e1.record(); torch.cuda.synchronize()
 ms_col = e0.elapsed_time(e1) / 20
+yc2 = C.apply_local(x).clone()
+colored = {"colored_apply_ms": ms_col, "colors": C.ncolors, "launches": C.launches()}
 E.apply_local(x, out=y)
-print(json.dumps({"colored_apply_ms": ms_col, "colors": C.ncolors, "launches": C.launches(), "colored_vs_atomic_max_rel_diff": float((yc - y).abs().max() / y.abs().max()),
-                  "colored_bit_reproducible": bool(torch.equal(C.apply_local(x), yc))}))
-print(json.dumps({"block": B, "n": n, "elements": B ** 3, "ebe_apply_ms": ms, "ebe_bytes": E.spmv_bytes(),
-                  "ebe_GBps": E.spmv_bytes() / ms / 1e6, "pcg_ms_per_iter": info.loop_ms / 200, "pcg_it_per_s": 200 / (info.loop_ms * 1e-3),
-                  "setup_s": time.time() - t0}))
+atomic = {"block": B, "n": n, "elements": B ** 3, "ebe_apply_ms": ms, "ebe_bytes": E.spmv_bytes(), "ebe_GBps": E.spmv_bytes() / ms / 1e6,
+          "pcg_ms_per_iter": info.loop_ms / 200, "pcg_it_per_s": 200 / (info.loop_ms * 1e-3), "setup_s": time.time() - t0}
+# the same coloured operator with every constant-memory slot taken by other pattern matrices: its 24-dof slices run on
+# the warp kernel (Ke from global memory, the repeated-dof scan in the scatter)
+from pcg_mpi_solver_b200.ebe import EbeMatrix
+from pcg_mpi_solver_b200.partition import TypeGroup
+del C, E, op
+gc.collect()
+rng = np.random.default_rng(0)
+held = []
+for _ in range(8):
+    k = rng.standard_normal((24, 24))
+    held.append(EbeMatrix([TypeGroup(0, np.arange(24)[:, None], np.zeros((24, 1), bool), np.ones(1), k + k.T, np.arange(1))],
+                          np.arange(24), 24, device=dev))
+Cw = EbeMatrixColored([grp], eff, ndof, device=dev)
+ycw = Cw.apply_local(x).clone()
+torch.cuda.synchronize()
+e0.record()
+for _ in range(20): Cw.apply_local(x)
+e1.record(); torch.cuda.synchronize()
+ms_warp = e0.elapsed_time(e1) / 20
+colored_warp = {"colored_warp_apply_ms": ms_warp, "warp_launches": Cw.launches(), "warp_same_bits": bool(torch.equal(ycw, yc))}
+del Cw, held
+print(json.dumps({**colored, "colored_vs_atomic_max_rel_diff": float((yc - y).abs().max() / y.abs().max()),
+                  "colored_bit_reproducible": bool(torch.equal(yc2, yc)), **colored_warp}))
+print(json.dumps(atomic))
