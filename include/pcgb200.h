@@ -430,6 +430,27 @@ int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked,
  * from any stream).  d_ck_fine is not read after create returns. */
 int pcgb_mg_create_field(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine,
                          const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out);
+/* The voxel-model preconditioner across ranks: pcgb_mg_create_ranks (same boxes, levels, halo plans, ownership weights,
+ * gather plan, collective call and V-cycle) with the Galerkin element matrices of pcgb_mg_create_field instead of
+ * rediscretisations, for the domain decomposition of a heterogeneous model (the reference's per-element ElemList_Ck,
+ * partition_mesh.py:437-479, split over ranks; it replaces the diagonal preconditioner of pcg_solver.py:346-352 and
+ * 446-454).  d_ck_fine: the rank's fine Ck per element of `box`, in the order of pcgb_hex_fill_field.  Each rank builds
+ * the element matrices of its own boxes only (levels 1 .. la, k_mg_galerkin from that element's eight children, so each
+ * is bit-identical to the one-rank matrix of the same element of the global mesh); levels 1 .. la-1 are assembled into
+ * the rank's sub-assembled CSR.  Level la's matrices are written into a zeroed array of the whole global box of level la
+ * and completed by one exchange-add over kel_gather, a plan over 576 * (elements of that box) entries that lists all of
+ * them for every other rank: one non-zero term per entry, so every rank holds the same matrices bit for bit.  They are
+ * the matrices of level la + 1, from which the replicated levels continue as in pcgb_mg_create_field; their CSR and
+ * lambda are those of the one-rank field hierarchy of the global mesh.  kel_gather is only used during the call (the
+ * caller may destroy it when create returns); its buffers grow with (ranks - 1) * 576 * elements, so the gathered box
+ * may hold at most 4096 elements.  Refusals: those of pcgb_mg_create_ranks (without E and h), and PCGB_ERR_ARG before
+ * anything is allocated for a null d_ck_fine or kel_gather, an element plan that is not all-to-all over the gathered
+ * box's matrices, a gathered box above 4096 elements, and an entry of d_ck_fine that is not finite and positive (a
+ * device check after a device synchronise; it sees the rank's own entries only, so a caller checks the global field
+ * before the collective call, as multigrid.HexMultigrid does).  d_ck_fine is not read after create returns. */
+int pcgb_mg_create_ranks_field(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos,
+                               pcgb_halo_t gather, pcgb_halo_t kel_gather, const double *const *d_own, const double *ke_host,
+                               const double *d_ck_fine, const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out);
 /* The one-rank preconditioner for a box of any size, uniform or a voxel model; like pcgb_mg_create and
  * pcgb_mg_create_field it replaces the diagonal preconditioner of pcg_solver.py:346-352 and 446-454.  Every axis of a
  * level is coarsened on its own while some axis has ne >= 3: an axis with ne >= 3 is halved to (ne + 1) / 2 elements,

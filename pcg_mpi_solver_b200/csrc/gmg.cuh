@@ -199,6 +199,22 @@ k_mg_scatter(HexGeom g, MgPlace p, const double *__restrict__ in, double *__rest
   for (int d = 0; d < 3; ++d) v[3 * t + d] = in[3 * gi + d];
 }
 
+// Gather of a rank's element matrices at the last ranked level into the global box's (pcgb_mg_create_ranks_field): one
+// thread per entry, element (X, Y, Z) of the rank's box g to global element e0 + (X, Y, Z) of p.glob, every other entry of
+// kg left as the caller zeroed it.  The exchange-add over the all-to-all element plan then completes kg: every global
+// element lies in exactly one rank's box, so each entry has one non-zero term and every rank holds the same matrices.
+__global__ void __launch_bounds__(256)
+k_mg_gather_elements(HexGeom g, MgPlace p, const double *__restrict__ kel, double *__restrict__ kg) {
+  const int64_t n = 576 * (int64_t)g.nx * g.ny * g.nz;
+  const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+  for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += stride) {
+    const int64_t e = i / 576;
+    const int X = (int)(e % g.nx), Y = (int)((e / g.nx) % g.ny), Z = (int)(e / ((int64_t)g.nx * g.ny));
+    const int64_t E = ((int64_t)(Z + p.e0z) * p.glob.ny + (Y + p.e0y)) * p.glob.nx + (X + p.e0x);
+    kg[576 * E + i % 576] = kel[i];
+  }
+}
+
 // rz and the count of non-finite z entries of z = M r: (sum z*(r*w), #(!isfinite z)) into partials[0] / partials[kMaxVecGrid]
 // (slots 3 and 4 of the iteration's partials).  A V-cycle spreads a NaN of the fine Minv over all of z, so NaN counts like
 // inf here: the loop stops with flag 2 as MATLAB pcg does for a non-finite preconditioned residual.

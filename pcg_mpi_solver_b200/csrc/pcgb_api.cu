@@ -1078,8 +1078,11 @@ struct pcgb_mg_s {
   int *d_bad = nullptr;
   int64_t bytes = 0;
   // field hierarchies (pcgb_mg_create_field): the fine per-element Ck, the Galerkin element matrices of the level being
-  // built (freed once the next level's exist), their peak device bytes and the device time of k_mg_galerkin
+  // built (freed once the next level's exist), their peak device bytes and the device time of k_mg_galerkin.  Across
+  // ranks (pcgb_mg_create_ranks_field) also the all-to-all plan over the element matrices of level la's global box, used
+  // by the set-up only (not owned, not kept after create)
   const double *ck_fine = nullptr;
+  pcgb_halo_t kel_gather = nullptr;
   double *kel = nullptr;
   int64_t kel_peak = 0;
   double galerkin_ms = 0.0;
@@ -1730,6 +1733,26 @@ int mg_galerkin_level(pcgb_mg_t mg, int l, const double *ke_host) {
   return PCGB_OK;
 }
 
+// Field hierarchies across ranks: the rank's element matrices of level la (mg->kel) into a zeroed array of the whole global
+// box of la, completed by one exchange-add over mg->kel_gather; it replaces mg->kel as the matrices of level la + 1.
+int mg_gather_elements(pcgb_mg_t mg) {
+  const MgLevel &A = mg->lv[(size_t)mg->la];
+  const int64_t nel = (int64_t)A.g.nx * A.g.ny * A.g.nz;
+  const int64_t nge = (int64_t)A.place.glob.nx * A.place.glob.ny * A.place.glob.nz;
+  double *kg = nullptr;
+  PCGB_CUDA(cudaMalloc(&kg, (size_t)nge * 576 * sizeof(double)));
+  mg->kel_peak = std::max(mg->kel_peak, (nel + nge) * 576 * (int64_t)sizeof(double));
+  cudaError_t e = cudaMemset(kg, 0, (size_t)nge * 576 * sizeof(double));
+  if (e == cudaSuccess) {
+    k_mg_gather_elements<<<(unsigned)std::min<int64_t>((576 * nel + 255) / 256, 65536), 256>>>(A.g, A.place, mg->kel, kg);
+    e = cudaGetLastError();
+  }
+  cudaFree(mg->kel);   // stream-ordered after the gather on the legacy stream
+  mg->kel = kg;
+  if (e != cudaSuccess) return fail(PCGB_ERR_CUDA, "pcgb_mg_create_ranks_field: element gather failed: %s", cudaGetErrorString(e));
+  return halo_exchange_add(mg->kel_gather, kg, 0);
+}
+
 // largest eigenvalue of the symmetric tridiagonal matrix (diagonal a, off-diagonal b) by bisection on the Sturm count
 double tridiag_max_eig(const std::vector<double> &a, const std::vector<double> &b) {
   const size_t k = a.size();
@@ -1856,6 +1879,9 @@ void mg_any_box_levels(std::vector<HexGeom> &geo, std::vector<int> &keep, std::v
 
 // largest global box a multi-rank hierarchy gathers onto every rank
 constexpr int64_t kMgMaxGathered = 1 << 17;
+// most elements of that box whose matrices a multi-rank field hierarchy gathers (4608 bytes each, and a plan of
+// (ranks - 1) * 576 entries per element)
+constexpr int64_t kMgMaxGatheredElements = 4096;
 
 // Builds the levels whose geometry (g, place, glev) and halos the caller has set in mg->lv.  own: ownership weights of
 // the ranked levels 0 .. la (copied).
@@ -1888,9 +1914,16 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
     if (l <= mg->la) {
       PCGB_CUDA(alloc(&L.own, L.n));
       PCGB_CUDA(cudaMemcpy(L.own, own[l], (size_t)L.n * sizeof(double), cudaMemcpyDeviceToDevice));
-      if (l == mg->la) continue;   // gathered: no operator, no smoother
+      if (l == mg->la) {   // gathered: no operator, no smoother
+        if (mg->ck_fine) {   // field: the rank's Galerkin element matrices, gathered into level la + 1's global box
+          PCGB_TRY(mg_galerkin_level(mg, l, ke_host));
+          PCGB_TRY(mg_gather_elements(mg));
+        }
+        continue;
+      }
     }
-    if (mg->ck_fine && l > 0) PCGB_TRY(mg_galerkin_level(mg, l, ke_host));   // field: the level's Galerkin element matrices
+    // field: the level's Galerkin element matrices (level la + 1, the global box of la, holds the gathered ones)
+    if (mg->ck_fine && l > 0 && l != mg->la + 1) PCGB_TRY(mg_galerkin_level(mg, l, ke_host));
     if (l == nlev - 1) {   // coarsest: dense Cholesky factor of its matrix
       int64_t *rp = nullptr, nnz = 0;
       int *col = nullptr;
@@ -2115,13 +2148,15 @@ int pcgb_mg_setup_info(pcgb_mg_t mg, double *galerkin_ms, int64_t *element_matri
 }
 
 namespace {
-// pcgb_mg_create_ranks and (index_free) pcgb_mg_create_ranks_index_free
+// pcgb_mg_create_ranks, (index_free) pcgb_mg_create_ranks_index_free and (d_ck_fine, kel_gather) pcgb_mg_create_ranks_field
 int mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos, pcgb_halo_t gather,
                     const double *const *d_own, const double *ke_host, double E, double h, const double *d_minv_fine, int degree,
-                    double lo, pcgb_mg_t *out, bool index_free, const char *who) {
+                    double lo, pcgb_mg_t *out, bool index_free, const char *who, const double *d_ck_fine = nullptr,
+                    pcgb_halo_t kel_gather = nullptr) {
   PCGB_TRY(require_device());
   if (!s || !box || !level_halos || !gather || !d_own || !ke_host || !d_minv_fine || !out)
     return fail(PCGB_ERR_ARG, "%s: null argument", who);
+  if ((d_ck_fine == nullptr) != (kel_gather == nullptr)) return fail(PCGB_ERR_ARG, "%s: null argument", who);
   if (!s->comm || s->comm->nranks < 2) return fail(PCGB_ERR_ARG, "%s: the solver has no communicator of 2 or more ranks", who);
   if (degree < 1 || !(lo > 0.0 && lo < 1.1) || !(E > 0.0) || !(h > 0.0))
     return fail(PCGB_ERR_ARG, "%s: degree >= 1, 0 < lo < 1.1, E > 0 and h > 0 required", who);
@@ -2166,8 +2201,25 @@ int mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, cons
   if (3 * geo.back().nfree_nodes > kMgMaxCoarse)
     return fail(PCGB_ERR_ARG, "%s: the coarsest level has %lld dofs (at most %d)", who, (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
   if ((size_t)la + 1 + geo.size() > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "%s: more than %d levels", who, PCGB_MG_MAX_LEVELS);
+  if (d_ck_fine) {
+    const int64_t nge = (int64_t)geo[0].nx * geo[0].ny * geo[0].nz;
+    if (nge > kMgMaxGatheredElements)
+      return fail(PCGB_ERR_ARG, "%s: the gathered level has %lld elements (at most %lld)", who, (long long)nge,
+                  (long long)kMgMaxGatheredElements);
+    if (kel_gather->comm != s->comm || kel_gather->nlocal != 576 * nge || kel_gather->n_nbr != s->comm->nranks - 1 ||
+        kel_gather->m != (int64_t)(s->comm->nranks - 1) * 576 * nge)
+      return fail(PCGB_ERR_ARG, "%s: the element plan must list all %lld entries of the gathered level's element matrices for "
+                  "every other rank", who, (long long)(576 * nge));
+    // the check runs on the legacy stream, which does not wait for non-blocking streams: finish whatever work of the caller
+    // may still be writing d_ck_fine first
+    PCGB_CUDA(cudaDeviceSynchronize());
+    int bad = 0;
+    PCGB_TRY(field_bad((int64_t)box->ne[0] * box->ne[1] * box->ne[2], d_ck_fine, 0, who, &bad));
+    if (bad) return fail(PCGB_ERR_ARG, "%s: every Ck of the field must be finite and positive", who);
+  }
   pcgb_mg_t mg = new pcgb_mg_s();
   mg->s = s; mg->degree = degree; mg->lo = lo; mg->la = la; mg->gather = gather; mg->index_free = index_free;
+  mg->ck_fine = d_ck_fine; mg->kel_gather = kel_gather;
   mg->lv.resize((size_t)la + 1 + geo.size());
   for (int l = 0; l <= la; ++l) {
     MgLevel &L = mg->lv[(size_t)l];
@@ -2182,6 +2234,8 @@ int mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, cons
     L.g = geo[k]; L.glev = la + (int)k; L.place = MgPlace{geo[k], 0, 0, 0};
   }
   const int rc = mg_build(mg, ke_host, E, h, d_minv_fine, d_own);
+  mg->ck_fine = nullptr;      // the caller's array and plan: not used after create
+  mg->kel_gather = nullptr;
   if (rc != PCGB_OK) { pcgb_mg_destroy(mg); return rc; }
   s->mgs.push_back(mg);
   *out = mg;
@@ -2201,6 +2255,17 @@ int pcgb_mg_create_ranks_index_free(pcgb_solver_t s, const pcgb_hex_box *box, in
                                     const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
   return mg_create_ranks(s, box, n_ranked, level_halos, gather, d_own, ke_host, E, h, d_minv_fine, degree, lo, out, true,
                          "pcgb_mg_create_ranks_index_free");
+}
+
+int pcgb_mg_create_ranks_field(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos,
+                               pcgb_halo_t gather, pcgb_halo_t kel_gather, const double *const *d_own, const double *ke_host,
+                               const double *d_ck_fine, const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
+  if (!d_ck_fine || !kel_gather) {
+    PCGB_TRY(require_device());
+    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks_field: null argument");
+  }
+  return mg_create_ranks(s, box, n_ranked, level_halos, gather, d_own, ke_host, 1.0, 1.0, d_minv_fine, degree, lo, out, false,
+                         "pcgb_mg_create_ranks_field", d_ck_fine, kel_gather);
 }
 
 int pcgb_mg_apply(pcgb_mg_t mg, const double *d_r, double *d_z, void *stream) {

@@ -12,6 +12,11 @@ level from `hexmesh.interface_lists`; the first level where some rank cannot hal
 as the one-rank hierarchy of its global box.  The global boxes are those of the one-rank preconditioner on the global mesh,
 so it is the same operator up to rounding.
 
+`E_field` (a voxel model, one Young's modulus per element) makes every coarse level a Galerkin product of element matrices,
+on one rank (pcgb_mg_create_field) and across ranks (pcgb_mg_create_ranks_field).  Across ranks E_field is the field of the
+whole mesh: each rank builds the element matrices of its own boxes, the gathered level's matrices are collected onto every
+rank (at most MAX_GATHERED_ELEMENTS elements), and the replicated levels are the one-rank field hierarchy's bit for bit.
+
 `coarsening="any"` (one rank) accepts a box of any size: every axis is coarsened on its own (`any_levels`), halved to
 (ne + 1) / 2 elements while ne >= 3 and kept once ne <= 2, down to at most 2x2x2 elements, and the coarse levels are always
 Galerkin products of element matrices (pcgb_mg_create_any), with or without `E_field`.
@@ -29,10 +34,11 @@ import numpy as np
 import torch
 
 from . import _lib
-from .hexmesh import HexBlock, field_ck, hex_element_stiffness, interface_lists
+from .hexmesh import HexBlock, block_field, check_field, field_ck, hex_element_stiffness, interface_lists
 
 MAX_GATHERED = 1 << 17    # dofs of the largest global box gathered onto every rank (kMgMaxGathered)
 MAX_COARSE = 1536         # dofs of the largest coarsest level (kMgMaxCoarse)
+MAX_GATHERED_ELEMENTS = 4096   # elements of the gathered global box of a multi-rank field hierarchy (kMgMaxGatheredElements)
 
 
 def _halve(b: HexBlock) -> HexBlock:
@@ -74,6 +80,31 @@ def index_free_bytes(ne) -> int:
     return 8 * (5 * n[0] + 6 * sum(n[1:-1]) + 2 * n[-1] + n[-1] ** 2)
 
 
+def gathered_elements(levels) -> int:
+    """Elements of the global box of the gathered level of `rank_levels`' list, whose element matrices a multi-rank field
+    hierarchy gathers onto every rank.  Raises ValueError, as pcgb_mg_create_ranks_field refuses, above MAX_GATHERED_ELEMENTS:
+    the matrices take 4608 bytes per element and the gather plan (ranks - 1) * 576 entries per element."""
+    g = levels[-1][0].ng
+    n = int(g[0]) * int(g[1]) * int(g[2])
+    if n > MAX_GATHERED_ELEMENTS:
+        raise ValueError(f"HexMultigrid: the gathered level has {n} elements (at most {MAX_GATHERED_ELEMENTS} with E_field across ranks)")
+    return n
+
+
+def check_global_field(E_field, ng, device=None):
+    """A Young's modulus per element of the whole mesh ng (shape (ng[2], ng[1], ng[0]), float64, numpy or a tensor on the
+    CPU or `device`), every value finite and positive; raises ValueError otherwise.  Checked the same way on every rank,
+    since all ranks hold the same field, before any collective step."""
+    check_field(E_field, HexBlock(tuple(ng), (0, 0, 0), tuple(ng)), device)
+    if isinstance(E_field, torch.Tensor):
+        ok = bool(torch.all(torch.isfinite(E_field) & (E_field > 0)))
+    else:
+        ok = bool(np.all(np.isfinite(E_field) & (E_field > 0)))
+    if not ok:
+        raise ValueError("E_field: every value must be finite and positive")
+    return E_field
+
+
 def rank_levels(blocks) -> list:
     """Per-level box lists of a multi-rank hierarchy: [blocks, halved blocks, ...] up to the gathered level la (the last
     entry; la = len - 1).  Raises ValueError, identically on every rank (all hold the same `blocks`), when the boxes do
@@ -113,9 +144,15 @@ class HexMultigrid:
     blocks lists every rank's box and block is blocks[op.comm.rank]; construction is collective and refuses (ValueError,
     on every rank alike, before anything is allocated) what `rank_levels` refuses.
 
-    E_field (one rank only): the per-element Young's modulus `op` was generated with (hexmesh.generate_matrix / generate_ebe
-    with E_field; shape (ne[2], ne[1], ne[0]), float64).  The coarse levels are then Galerkin products of element matrices
-    (pcgb_mg_create_field) instead of rediscretisations with block.E.  With a multi-rank `op` it raises ValueError.
+    E_field: the per-element Young's modulus `op` was generated with (hexmesh.generate_matrix / generate_ebe /
+    generate_box_operator with E_field; float64, a numpy array or a tensor).  The coarse levels are then Galerkin products of
+    element matrices instead of rediscretisations with block.E.  One rank: the field of the box, shape (ne[2], ne[1], ne[0])
+    (pcgb_mg_create_field, which checks its values on the device).  Across ranks: the field of the WHOLE mesh, shape
+    (ng[2], ng[1], ng[0]), the array every rank passes to hexmesh.block_field for its operator (pcgb_mg_create_ranks_field
+    with the rank's block_field slice).  Every rank checks the whole field on the host (shape, finite and positive values)
+    and the gathered level's element count (`gathered_elements`, at most MAX_GATHERED_ELEMENTS), so a refusal is a ValueError
+    on every rank alike, before anything is allocated; a rank's block-shaped slice is refused.  The set-up holds up to two
+    levels' element matrices of the rank's boxes, then the gathered level's (setup_info).
 
     coarsening (one rank only): "even" (the default, above) or "any": a box of any size, each axis halved or kept on its own
     (`any_levels`), Galerkin levels from E_field or, without it, from Ck = block.E * block.h on every element
@@ -160,9 +197,7 @@ class HexMultigrid:
                                                           _lib.ptr(ck), float(block.E), float(block.h), _lib.ptr(minv), self.degree,
                                                           self.lo, ctypes.byref(self._h)), "pcgb_mg_create_any")
             return
-        if E_field is not None:
-            if ranked:
-                raise ValueError("HexMultigrid: E_field is supported on one rank only")
+        if E_field is not None and not ranked:
             ck = field_ck(E_field, block, self.device)
             minv = op.jacobi() if minv is None else minv.to(self.device, torch.float64).contiguous()
             ke = np.ascontiguousarray(hex_element_stiffness(1.0, block.nu))
@@ -181,6 +216,9 @@ class HexMultigrid:
             if block.n != op.n:
                 raise ValueError(f"HexMultigrid: the operator has {op.n} rows, the box {block.n}")
             self.levels = rank_levels(blocks)
+            if E_field is not None:
+                check_global_field(E_field, block.ng, self.device)
+                nge = gathered_elements(self.levels)
         minv = op.jacobi() if minv is None else minv.to(self.device, torch.float64).contiguous()
         ke = np.ascontiguousarray(hex_element_stiffness(1.0, block.nu))
         kep = ke.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
@@ -208,6 +246,19 @@ class HexMultigrid:
             self._halos.append(self._gather)
             halos = (ctypes.c_void_p * la)(*[h.value for h in self._halos[:la]])
             owns = (ctypes.c_void_p * (la + 1))(*[t.data_ptr() for t in own])
+            if E_field is not None:
+                # the rank's slice of the global field, and a plan over the gathered level's element matrices used by the
+                # set-up only
+                ck = field_ck(block_field(E_field, block), block, self.device)
+                kg = make_halo(comm, others, [np.arange(576 * nge, dtype=np.int64)] * len(others), 576 * nge)
+                try:
+                    torch.cuda.synchronize(self.device)
+                    _lib.check(lib.pcgb_mg_create_ranks_field(op._solver, ctypes.byref(box), la, halos, self._gather, kg, owns, kep,
+                                                              _lib.ptr(ck), _lib.ptr(minv), self.degree, self.lo, ctypes.byref(self._h)),
+                               "pcgb_mg_create_ranks_field")
+                finally:
+                    lib.pcgb_halo_destroy(kg)
+                return
             torch.cuda.synchronize(self.device)
             name = "pcgb_mg_create_ranks_index_free" if index_free else "pcgb_mg_create_ranks"
             _lib.check(getattr(lib, name)(op._solver, ctypes.byref(box), la, halos, self._gather, owns, kep, float(block.E),

@@ -9,6 +9,12 @@ V-cycle time per application (CUDA events around `pcgb_mg_apply`).  Rank 0 print
 rank's numbers and the card's name, SM clock limit and power limit.  Ranks sharing one GPU (PCGB_SHARED_GPU=1) run, but
 their times say nothing about speed.  --coarse index_free builds HexMultigrid(coarse="index_free"): index-free ranked and
 replicated coarse levels.
+
+--contrast C (opt-in, with --fraction and --seed) draws hexmesh.inclusion_field over the whole global mesh (inclusions of
+Young's modulus C in a matrix of 1), every rank generates its operator from its block_field slice, and both arms solve
+that voxel model: the multigrid arm builds HexMultigrid(..., E_field=field) with Galerkin coarse levels
+(pcgb_mg_create_ranks_field).  The multigrid line then also reports each rank's Galerkin time and peak element-matrix
+bytes (setup_info) and the drop in free device memory across the set-up.  Without --contrast the output is unchanged.
 """
 import argparse
 import datetime
@@ -31,6 +37,9 @@ def main():
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--vcycles", type=int, default=20)
     ap.add_argument("--coarse", choices=["csr", "index_free"], default="csr")
+    ap.add_argument("--contrast", type=float, default=None)
+    ap.add_argument("--fraction", type=float, default=0.4)
+    ap.add_argument("--seed", type=int, default=0)
     a = ap.parse_args()
     import torch
     import torch.distributed as dist
@@ -46,7 +55,8 @@ def main():
         dist.init_process_group("gloo", timeout=timeout)
     else:
         dist.init_process_group("nccl", device_id=dev, timeout=timeout)
-    from pcg_mpi_solver_b200.hexmesh import HexBlock, block_grid, generate_ebe, generate_matrix, interface_lists, load_vector, partition_blocks
+    from pcg_mpi_solver_b200.hexmesh import (HexBlock, block_field, block_grid, generate_ebe, generate_matrix, inclusion_field, interface_lists,
+                                             load_vector, partition_blocks)
     from pcg_mpi_solver_b200.multigrid import HexMultigrid
     from pcg_mpi_solver_b200.solver import Communicator, SubdomainOperator
     comm = Communicator.from_torch_distributed(dev, nccl=not shared)
@@ -54,7 +64,10 @@ def main():
     ng = tuple(pgrid[ax] * a.block for ax in range(3))
     blocks = [HexBlock(b.ng, b.e0, b.ne, h=1.0 / ng[0]) for b in partition_blocks(ng, pgrid)]
     blk = blocks[rank]
-    A = generate_matrix(blk, device=dev) if a.operator == "csr" else generate_ebe(blk, device=dev, ordered=a.operator == "ebe_ordered")
+    field = None if a.contrast is None else inclusion_field(ng, a.fraction, (2.0, 6.0), 1.0, a.contrast, a.seed)
+    fb = None if field is None else block_field(field, blk)
+    A = (generate_matrix(blk, device=dev, E_field=fb) if a.operator == "csr"
+         else generate_ebe(blk, device=dev, ordered=a.operator == "ebe_ordered", E_field=fb))
     nbr, lists, w = interface_lists(blocks, rank)
     n_global = 3 * ng[0] * (ng[1] + 1) * (ng[2] + 1)
     op = SubdomainOperator(A, comm, nbr, lists, w, n_global=n_global)
@@ -62,10 +75,15 @@ def main():
     minv = op.jacobi()
     torch.cuda.synchronize()
     dist.barrier()
+    free0 = torch.cuda.mem_get_info(dev)[0]
     t0 = time.perf_counter()
-    mg = HexMultigrid(op, blk, degree=a.degree, minv=minv, blocks=blocks, coarse=a.coarse)
+    if field is None:
+        mg = HexMultigrid(op, blk, degree=a.degree, minv=minv, blocks=blocks, coarse=a.coarse)
+    else:
+        mg = HexMultigrid(op, blk, degree=a.degree, minv=minv, blocks=blocks, coarse=a.coarse, E_field=field)
     torch.cuda.synchronize()
     setup_s = time.perf_counter() - t0
+    setup_mem = free0 - torch.cuda.mem_get_info(dev)[0]
     info = mg.info()
 
     def run(M, maxiter):
@@ -98,11 +116,15 @@ def main():
     mine = {"jacobi": {"flag": ij.flag, "iters": ij.iters, "loop_ms": round(ij.loop_ms, 3), "wall_s": round(wj, 4)},
             "multigrid": {"flag": im.flag, "iters": im.iters, "loop_ms": round(im.loop_ms, 3), "wall_s": round(wm, 4),
                           "setup_s": round(setup_s, 3), "vcycle_ms": round(vc_ms, 4)}}
+    if field is not None:
+        mine["multigrid"].update(mg.setup_info(), bytes=info["bytes"], setup_free_drop_bytes=int(setup_mem))
     box = [None] * world
     dist.all_gather_object(box, mine)
     if rank == 0:
         common = {"ranks": world, "pgrid": list(pgrid), "block": a.block, "operator": a.operator, "coarse": a.coarse, "tol": a.tol, "card": card(),
                   "shared_gpu": shared}
+        if field is not None:
+            common.update(contrast=a.contrast, fraction=a.fraction, seed=a.seed)
         print(json.dumps({**common, "arm": "jacobi", "per_rank": [m["jacobi"] for m in box]}))
         print(json.dumps({**common, "arm": "multigrid", "degree": a.degree, "levels": info["levels"], "gather_level": info["gather_level"],
                           "n_gathered": info["n_gathered"], "per_rank": [m["multigrid"] for m in box]}))
