@@ -37,6 +37,7 @@ typedef struct pcgb_ebe2_s *pcgb_ebe2_t;   /* coloured (atomics-free, bit-reprod
 typedef struct pcgb_ebe_ordered_s *pcgb_ebe_ordered_t; /* EBE operator with a fixed summation order (bit-reproducible, solver-ready) */
 typedef struct pcgb_hexop_s *pcgb_hexop_t; /* index-free matrix-free operator of a hex box (the ordered operator's bits) */
 typedef struct pcgb_mg_s *pcgb_mg_t;       /* geometric multigrid preconditioner of a hex-box solver (one V-cycle) */
+typedef struct pcgb_fields_s *pcgb_fields_t; /* strain / stress recovery of a hex box (element fields, nodal averages) */
 
 /* error codes */
 #define PCGB_OK 0
@@ -503,6 +504,35 @@ int pcgb_mg_info_ranks(pcgb_mg_t mg, int32_t *gather_level, int64_t *n_gathered)
 /* level la's ranked vector into its global box on every rank (gather + exchange), and the rank's entries back out */
 int pcgb_mg_gather(pcgb_mg_t mg, const double *d_ranked, double *d_global, void *stream);
 int pcgb_mg_scatter(pcgb_mg_t mg, const double *d_global, double *d_ranked, void *stream);
+
+/* ---------------------------------------------------------------- strain and stress recovery of a hex box
+ * Replaces updateElemStrain (pcg_solver.py:601-618), getPrincipalStress / getPrincipalStrain (file_operations.py:251-301)
+ * and getNodalPS (pcg_solver.py:730-814) with its exchange (:784-809) for the boxes of the pcgb_hex_* numbering; the
+ * arithmetic contract (centroid Q1 gradient, stress law, invariant-form principal values and their two deviations, the
+ * fixed nodal summation order) is the header comment of csrc/fields.cuh.  d_x: the box's free-dof vector (n =
+ * pcgb_hex_nrows doubles, clamped nodes u = 0).  Elements e = (z ne[1] + y) ne[0] + x; nodes of the whole box, clamped
+ * line included: node = (z (ne[1]+1) + y) (ne[0]+1) + x.
+ * pcgb_fields_create: h the element edge, E the uniform Young's modulus, nu Poisson's ratio (lambda and mu of the Q1
+ * matrix's D); d_E (device, ne[0]*ne[1]*ne[2] doubles, caller-owned, must outlive the handle) replaces E per element.
+ * PCGB_ERR_ARG, holding no device memory: a box with some ne <= 0 or outside its global mesh, h or E not finite and
+ * positive, nu outside (-1, 0.5), an entry of d_E that is not finite and positive (checked on the device after a device
+ * synchronise).  The handle holds no device memory.
+ * pcgb_fields_element: one pass over the box writing the outputs that are not NULL, element-major: strain (6 per element,
+ * Voigt 11, 22, 33, 23, 13, 12, tensor shears), stress (6), principal stress (3: P1 >= P2 >= P3), principal strain (3).
+ * PCGB_ERR_ARG when x overlaps an output.
+ * pcgb_fields_nodal: the nodal average of the principal stresses (kind 0) or strains (kind 1): d_work (4 doubles per node)
+ * receives (sum_0, sum_1, sum_2, count) over the node's elements, then, with a halo plan (pcgb_halo_create over the 4 *
+ * nodes entries of d_work, listing 4 node + k, k = 0..3, of each shared node), the neighbours' copies; d_out (3 per node)
+ * = sum / (count + 1e-15).  Scratch of 3 doubles per element is allocated and freed on `stream` within the call.
+ * PCGB_ERR_ARG before any launch: kind not 0 or 1, a halo whose vector length is not 4 * nodes, x, work and out
+ * overlapping. */
+int pcgb_fields_create(const pcgb_hex_box *box, double h, double E, double nu, const double *d_E /* NULL = uniform E */,
+                       pcgb_fields_t *out);
+int pcgb_fields_destroy(pcgb_fields_t F);
+int pcgb_fields_element(pcgb_fields_t F, const double *d_x, double *d_strain, double *d_stress, double *d_ps, double *d_pe,
+                        void *stream);
+int pcgb_fields_nodal(pcgb_fields_t F, const double *d_x, int kind /* 0 stress, 1 strain */, pcgb_halo_t halo /* NULL on one rank */,
+                      double *d_work /* 4 per node */, double *d_out /* 3 per node */, void *stream);
 
 #ifdef __cplusplus
 }

@@ -5,10 +5,13 @@ Public surface (mirrors the reference's solver/partition API for this path, SURV
     partition_mesh(model, nparts)   METIS dual partition + subdomain builder
                                     (run_metis.py + partition_mesh.py)
     CsrMatrix, SubdomainOperator, Communicator
+    HexFields(block, ...)           strains, stresses, principal values and their nodal averages of a hex box
+                                    (updateElemStrain / getNodalPS, pcg_solver.py:601-618, 730-814)
 Everything numerical runs in csrc/libpcgb200.so (hand-written sm_90a CUDA, C ABI in include/pcgb200.h).
 """
 from .solver import Communicator, SolveInfo, SubdomainOperator, solve  # noqa: F401
 from .csr import CsrMatrix  # noqa: F401
+from .fields import HexFields  # noqa: F401
 
 
 def partition_mesh(*args, **kwargs):
@@ -16,4 +19,4 @@ def partition_mesh(*args, **kwargs):
     return _pm(*args, **kwargs)
 
 
-__all__ = ["solve", "partition_mesh", "CsrMatrix", "SubdomainOperator", "Communicator", "SolveInfo"]
+__all__ = ["solve", "partition_mesh", "CsrMatrix", "SubdomainOperator", "Communicator", "SolveInfo", "HexFields"]

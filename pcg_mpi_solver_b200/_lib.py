@@ -144,6 +144,10 @@ SIGNATURES = {
     "pcgb_hexop_diag": (c_int, [c_void_p, c_void_p, c_void_p]),
     "pcgb_hexop_bytes": (c_int64, [c_void_p]),
     "pcgb_solver_create_hexop": (c_int, [c_void_p, c_void_p, c_void_p, POINTER(c_void_p)]),
+    "pcgb_fields_create": (c_int, [POINTER(HexBox), c_double, c_double, c_double, c_void_p, POINTER(c_void_p)]),
+    "pcgb_fields_destroy": (c_int, [c_void_p]),
+    "pcgb_fields_element": (c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p]),
+    "pcgb_fields_nodal": (c_int, [c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_void_p]),
 }
 
 _lib = None

@@ -16,6 +16,7 @@
 #include "ebe_ordered.cuh"
 #include "gmg.cuh"
 #include "hexop.cuh"
+#include "fields.cuh"
 
 using namespace pcgb;
 
@@ -44,6 +45,12 @@ struct pcgb_ebe_ordered_s {
 
 struct pcgb_hexop_s {
   HexOp H;
+};
+
+struct pcgb_fields_s {
+  FieldsShape s;
+  const double *d_E = nullptr;   // per-element E (caller-owned), or NULL
+  int64_t ne = 0, nnodes = 0, n = 0;   // elements, nodes (clamped line included), free dofs
 };
 
 // What may differ between two solves on one handle and changes the captured iterations (the operator, the x buffers and
@@ -2452,5 +2459,91 @@ int pcgb_hexop_diag(pcgb_hexop_t H, double *d_diag, void *stream) {
 }
 
 int64_t pcgb_hexop_bytes(pcgb_hexop_t H) { return H ? H->H.bytes : 0; }
+
+// ------------------------------------------------------------------------------------ strain and stress recovery
+// updateElemStrain (pcg_solver.py:601-618), getNodalPS (:730-814) and getPrincipalStress / getPrincipalStrain
+// (file_operations.py:251-301) on a hex box; the arithmetic contract is in fields.cuh.
+int pcgb_fields_create(const pcgb_hex_box *box, double h, double E, double nu, const double *d_E, pcgb_fields_t *out) {
+  if (!box || !out) return fail(PCGB_ERR_ARG, "pcgb_fields_create: null argument");
+  *out = nullptr;
+  for (int a = 0; a < 3; ++a)
+    if (box->ne[a] <= 0 || box->e0[a] < 0 || (int64_t)box->e0[a] + box->ne[a] > box->ng[a])
+      return fail(PCGB_ERR_ARG, "pcgb_fields_create: the box must have ne > 0 and lie inside its global mesh on every axis");
+  if (!(std::isfinite(h) && h > 0.0) || !(std::isfinite(E) && E > 0.0) || !(nu > -1.0 && nu < 0.5))
+    return fail(PCGB_ERR_ARG, "pcgb_fields_create: h and E must be finite and positive and -1 < nu < 0.5");
+  PCGB_TRY(require_device());
+  const HexGeom g = hex_geom(box);
+  FieldsShape s = fields_shape(g);
+  if ((int64_t)s.nbx * s.nby * s.nbz >= (int64_t)1 << 31) return fail(PCGB_ERR_ARG, "pcgb_fields_create: box too large");
+  const int64_t ne = (int64_t)g.nx * g.ny * g.nz;
+  if (d_E) {
+    // the check runs on the legacy stream, which does not wait for non-blocking streams: finish the caller's writes first
+    PCGB_CUDA(cudaDeviceSynchronize());
+    int bad = 0;
+    PCGB_TRY(field_bad(ne, d_E, 0, "pcgb_fields_create", &bad));
+    if (bad) return fail(PCGB_ERR_ARG, "pcgb_fields_create: every E of the field must be finite and positive");
+  }
+  // lambda and mu as hexmesh.hex_element_stiffness(1.0, nu) computes them
+  const double one = 1.0;
+  s.q = 0.25 / h;
+  s.E = E;
+  s.lam = one * nu / ((1 + nu) * (1 - 2 * nu));
+  s.m2 = 2 * (one / (2 * (1 + nu)));
+  pcgb_fields_t F = new pcgb_fields_s();
+  F->s = s;
+  F->d_E = d_E;
+  F->ne = ne;
+  F->nnodes = (int64_t)(g.nx + 1) * (g.ny + 1) * (g.nz + 1);
+  F->n = 3 * g.nfree_nodes;
+  *out = F;
+  return PCGB_OK;
+}
+
+int pcgb_fields_destroy(pcgb_fields_t F) {
+  delete F;
+  return PCGB_OK;
+}
+
+static bool overlap(const double *a, int64_t na, const double *b, int64_t nb) {
+  if (!a || !b) return false;
+  const uintptr_t a0 = (uintptr_t)a, b0 = (uintptr_t)b;
+  return a0 < b0 + (uintptr_t)nb * sizeof(double) && b0 < a0 + (uintptr_t)na * sizeof(double);
+}
+
+int pcgb_fields_element(pcgb_fields_t F, const double *d_x, double *d_strain, double *d_stress, double *d_ps, double *d_pe, void *stream) {
+  if (!F || !d_x) return fail(PCGB_ERR_ARG, "pcgb_fields_element: null argument");
+  const int64_t ne = F->ne;
+  if (overlap(d_x, F->n, d_strain, 6 * ne) || overlap(d_x, F->n, d_stress, 6 * ne) || overlap(d_x, F->n, d_ps, 3 * ne) ||
+      overlap(d_x, F->n, d_pe, 3 * ne))
+    return fail(PCGB_ERR_ARG, "pcgb_fields_element: x overlaps an output");
+  return fields_elem(F->s, F->d_E, d_x, d_strain, d_stress, d_ps, d_pe, (cudaStream_t)stream);
+}
+
+int pcgb_fields_nodal(pcgb_fields_t F, const double *d_x, int kind, pcgb_halo_t halo, double *d_work, double *d_out, void *stream) {
+  if (!F || !d_x || !d_work || !d_out) return fail(PCGB_ERR_ARG, "pcgb_fields_nodal: null argument");
+  if (kind != 0 && kind != 1) return fail(PCGB_ERR_ARG, "pcgb_fields_nodal: kind must be 0 (stress) or 1 (strain)");
+  const int64_t nn = F->nnodes;
+  if (halo && halo->nlocal != 4 * nn)
+    return fail(PCGB_ERR_ARG, "pcgb_fields_nodal: the halo plan exchanges %lld entries, the box needs 4 per node (%lld)",
+                (long long)halo->nlocal, (long long)(4 * nn));
+  if (overlap(d_x, F->n, d_work, 4 * nn) || overlap(d_x, F->n, d_out, 3 * nn) || overlap(d_work, 4 * nn, d_out, 3 * nn))
+    return fail(PCGB_ERR_ARG, "pcgb_fields_nodal: x, work and out must not overlap");
+  const cudaStream_t st = (cudaStream_t)stream;
+  double *pv = nullptr;   // the element principal values, 3 per element, for this call only
+  PCGB_CUDA(cudaMallocAsync((void **)&pv, (size_t)(3 * F->ne) * sizeof(double), st));
+  int rc = fields_elem(F->s, F->d_E, d_x, nullptr, nullptr, kind == 0 ? pv : nullptr, kind == 1 ? pv : nullptr, st);
+  if (rc == PCGB_OK) {
+    k_fields_nodal<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>(F->s.g, pv, d_work);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) rc = fail(PCGB_ERR_CUDA, "pcgb_fields_nodal: %s", cudaGetErrorString(e));
+  }
+  const cudaError_t fe = cudaFreeAsync(pv, st);
+  if (rc != PCGB_OK) return rc;
+  if (fe != cudaSuccess) return fail(PCGB_ERR_CUDA, "pcgb_fields_nodal: %s", cudaGetErrorString(fe));
+  if (halo) PCGB_TRY(halo_exchange_add(halo, d_work, st));
+  k_fields_divide<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>(nn, d_work, d_out);
+  PCGB_CHECK_LAUNCH();
+  return PCGB_OK;
+}
 
 }  // extern "C"

@@ -377,3 +377,26 @@ def interface_lists(blocks, rank):
             w[dofs] = 0.0
     del ng
     return nbr, lists, w
+
+
+def interface_node_lists(blocks, rank):
+    """Neighbour ranks and, per neighbour, the box nodes `rank` shares with it (local numbering of all the box's nodes,
+    node = (lz * (ne[1] + 1) + ly) * (ne[0] + 1) + lx, clamped line included) in ascending global node id: the rule of
+    interface_lists over every node, as the reference's OvrlpLocalNodeIdVecList covers them (getNodalPS,
+    pcg_solver.py:784-809).  The list of rank a for b and that of b for a name the same global nodes in the same order."""
+    me = blocks[rank]
+    mine = me.node_ranges()
+    nbr, lists = [], []
+    for other_id, other in enumerate(blocks):
+        if other_id == rank:
+            continue
+        theirs = other.node_ranges()
+        lo = [max(mine[a][0], theirs[a][0]) for a in range(3)]
+        hi = [min(mine[a][1], theirs[a][1]) for a in range(3)]
+        if any(lo[a] > hi[a] for a in range(3)):
+            continue
+        gz, gy, gx = np.meshgrid(np.arange(lo[2], hi[2] + 1), np.arange(lo[1], hi[1] + 1), np.arange(lo[0], hi[0] + 1), indexing="ij")
+        node = ((gz.ravel() - me.e0[2]) * (me.ne[1] + 1) + (gy.ravel() - me.e0[1])) * (me.ne[0] + 1) + (gx.ravel() - me.e0[0])
+        nbr.append(other_id)
+        lists.append(node.astype(np.int64))
+    return nbr, lists

@@ -12,7 +12,9 @@ and writes what it writes (pcg_solver.py:142-209, 841-896, 943-961; file_operati
     <Scratch>/Results_Run<R>/PlotData/<Model>_MP<N>_TimeData.{npz,mat}   (Flag / Iter / RelRes per load step, timers)
 so that `src/data/export_vtk.py` keeps working unchanged.  The time-step shell (pcg_solver.py:1002-1008:
 updateBC -> updatePreconditioner -> PCG -> export, same A and M for every load step) is kept as thin host code.
-Displacement `U` is the only export variable supported (the others need post-processing outside the hot path).
+Displacement `U` is the only export variable supported: reference-format parts carry no strain modes, so the `PS`/`PE`
+exports of pcg_solver.py:879-889 cannot run on them.  For hex boxes and voxel models, `fields.HexFields` recovers element
+strains and stresses, principal values and their nodal averages on the device (DESIGN §2.10).
 """
 from __future__ import annotations
 
