@@ -484,6 +484,23 @@ int pcgb_mg_create_index_free(pcgb_solver_t s, const pcgb_hex_box *box, const do
 int pcgb_mg_create_ranks_index_free(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos,
                                     pcgb_halo_t gather, const double *const *d_own, const double *ke_host, double E, double h,
                                     const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out);
+/* pcgb_mg_create_field with a matrix-free level 1, for voxel models whose level-1 Galerkin matrices do not fit on the
+ * device (at 512^3 they take 77 GB as element matrices, 49 GB as CSR).  Arguments, checks and refusals are those of
+ * pcgb_mg_create_field, plus PCGB_ERR_ARG before anything is allocated for a box whose hierarchy has fewer than 3 levels
+ * (level 1 would be the coarsest, not smoothed).  Level 1 applies y_1 = P^T A_0 P x_1 in one kernel (k_mg_rap1) from
+ * d_ck_fine and ke_host, bit-identical to pcgb_mg_prolong_add of x_1 into a zero fine vector, the index-free fine
+ * operator of pcgb_hexop_create with d_ck_fine, and pcgb_mg_restrict; it holds no matrix.  Levels >= 2 are those of
+ * pcgb_mg_create_field bit for bit (CSR, D^-1, lambda, coarsest factor): level 2's element matrices are built from slabs
+ * of level-1 element layers (at most 1 GiB, at least two layers) in ascending z, so level 1's are never held whole, and
+ * level 1's D^-1 is the field hierarchy's bit for bit.  d_ck_fine is read by every V-cycle: it must outlive the handle.
+ * pcgb_mg_level_csr refuses level 1; pcgb_mg_setup_info reports the level-2 matrices plus the slab (or, when larger, the
+ * level-2 and level-3 matrices) and the device time of the Galerkin kernels. */
+int pcgb_mg_create_field_rap(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine,
+                             const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out);
+/* For tests: the inverse diagonal of smoothed level `level` (0 .. nlevels - 2, not the gathered level of a multi-rank
+ * handle; level 0: the copy of d_minv_fine) of any handle into d_out (n_l doubles), ordered on `stream`.  PCGB_ERR_ARG
+ * for any other level. */
+int pcgb_mg_level_dinv(pcgb_mg_t mg, int level, double *d_out, void *stream);
 /* For tests: y = A_l x on smoothed coarse level `level` (1 <= level < nlevels - 1, not the gathered level of a multi-rank
  * handle) of either kind, the local product without the level's exchange-add.  PCGB_ERR_ARG for any other level and,
  * before any launch, when [d_x, d_x + n_l) and [d_y, d_y + n_l) overlap. */
@@ -493,7 +510,7 @@ int pcgb_mg_level_box(pcgb_mg_t mg, int level, int32_t *ne);
 /* For tests: level `level`'s CSR (1 <= level < nlevels - 1, the smoothed coarse levels) into caller buffers: int64 row
  * offsets (n + 1), int32 columns and values (nnz each).  With all three buffers NULL only *nnz is written.  Synchronises
  * `stream`.  PCGB_ERR_ARG for level 0 (the solver's operator), the coarsest level (held as a dense factor), the
- * gathered level of a multi-rank handle and every level of an index-free hierarchy. */
+ * gathered level of a multi-rank handle, every level of an index-free hierarchy and level 1 of a rap hierarchy. */
 int pcgb_mg_level_csr(pcgb_mg_t mg, int level, int64_t *d_rowptr, int32_t *d_col, double *d_val, int64_t *nnz, void *stream);
 /* Set-up costs of a field hierarchy (0 for the others): device time of the Galerkin kernels in ms, and the peak device
  * bytes of element matrices held at once during create.  Either may be NULL. */

@@ -258,16 +258,19 @@ __device__ __forceinline__ double mg_child_weight(int c, int l, int k) {
 // element, one thread per entry (i, j): T = K_c Q_c in shared memory (l ascending), then (Q_c^T T)[i][j] (l ascending),
 // added to the entry in ascending c.  No atomics: a repeated set-up is bit-identical.  The result is written mirrored
 // from its upper triangle, so every element matrix, and every CSR assembled from them, is exactly symmetric.
+// Slabs (gmg_rap.cuh): CTA b builds coarse element E = e_off + b into kc[576 b ..], and child k is read at index k - child_off
+// of ck / kf; both offsets are 0 for a whole level.
 constexpr int kMgGalerkinThreads = 576;
 __global__ void __launch_bounds__(kMgGalerkinThreads)
-k_mg_galerkin(int cnx, int cny, int fnx, int fny, const double *__restrict__ ck, const double *__restrict__ kf, double *__restrict__ kc) {
+k_mg_galerkin(int cnx, int cny, int fnx, int fny, const double *__restrict__ ck, const double *__restrict__ kf, double *__restrict__ kc,
+              int64_t e_off = 0, int64_t child_off = 0) {
   __shared__ double K[576], T[576];
   const int t = threadIdx.x, i = t / 24, j = t % 24;
-  const int64_t E = blockIdx.x;
+  const int64_t E = blockIdx.x + e_off;
   const int X = (int)(E % cnx), Y = (int)((E / cnx) % cny), Z = (int)(E / ((int64_t)cnx * cny));
   double acc = 0.0;
   for (int c = 0; c < 8; ++c) {
-    const int64_t child = ((int64_t)(2 * Z + (c >> 2)) * fny + (2 * Y + ((c >> 1) & 1))) * fnx + (2 * X + (c & 1));
+    const int64_t child = ((int64_t)(2 * Z + (c >> 2)) * fny + (2 * Y + ((c >> 1) & 1))) * fnx + (2 * X + (c & 1)) - child_off;
     K[t] = kf ? kf[576 * child + t] : ck[child] * c_hex_ke[t];
     __syncthreads();
     double s = 0.0;
@@ -282,7 +285,7 @@ k_mg_galerkin(int cnx, int cny, int fnx, int fny, const double *__restrict__ ck,
   }
   K[t] = acc;   // every thread is past its last read of K (the second barrier of c = 7)
   __syncthreads();
-  kc[576 * E + t] = i <= j ? K[t] : K[j * 24 + i];
+  kc[576 * (int64_t)blockIdx.x + t] = i <= j ? K[t] : K[j * 24 + i];
 }
 
 // ---- boxes of any size (pcgb_mg_create_any).  Every axis of a level is coarsened on its own: halved (ne >= 3; coarse node

@@ -46,6 +46,39 @@ inline HexOpShape hexop_shape(const HexGeom &g) {
   return s;
 }
 
+// The three rows of free node (lx, ly, lz) of K x, in the order stated at the top of this file: la outer over the elements
+// inside the box, b = (lb, e) inner with an fma chain from 0.0, then the element's sum added to the row.  ck_at(ax, ay, az)
+// is the Ck of element node - (ax, ay, az); x_at(dx, dy, dz) points at the three staged x of node + (dx, dy, dz), d in
+// {-1, 0, 1}, 0.0 for a clamped node or one outside the box.  k_hexop and the multigrid's fused level-1 product (gmg_rap.cuh)
+// both call it, so their per-node arithmetic is one piece of code.
+template <class CkAt, class XAt>
+__device__ __forceinline__ void hex_node_rows(const HexKe &ke, const HexGeom &g, int lx, int ly, int lz, CkAt ck_at, XAt x_at,
+                                              double &r0, double &r1, double &r2) {
+  r0 = 0.0; r1 = 0.0; r2 = 0.0;
+#pragma unroll
+  for (int la = 0; la < 8; ++la) {
+    const int ax = la & 1, ay = (la >> 1) & 1, az = la >> 2;
+    const int ox = lx - ax, oy = ly - ay, oz = lz - az;
+    if (ox < 0 || ox >= g.nx || oy < 0 || oy >= g.ny || oz < 0 || oz >= g.nz) continue;
+    const double c = ck_at(ax, ay, az);
+    double a0 = 0.0, a1 = 0.0, a2 = 0.0;
+#pragma unroll
+    for (int lb = 0; lb < 8; ++lb) {
+      const double *xs = x_at((lb & 1) - ax, ((lb >> 1) & 1) - ay, (lb >> 2) - az);
+#pragma unroll
+      for (int e = 0; e < 3; ++e) {
+        const double u = __dmul_rn(c, xs[e]);                                   // :279  Ck * U
+        a0 = __fma_rn(ke.k[(3 * la + 0) * 24 + 3 * lb + e], u, a0);              // :279  Ke @ (Ck * U)
+        a1 = __fma_rn(ke.k[(3 * la + 1) * 24 + 3 * lb + e], u, a1);
+        a2 = __fma_rn(ke.k[(3 * la + 2) * 24 + 3 * lb + e], u, a2);
+      }
+    }
+    r0 = __dadd_rn(r0, a0);                                                     // :300  np.bincount's order
+    r1 = __dadd_rn(r1, a1);
+    r2 = __dadd_rn(r2, a2);
+  }
+}
+
 template <bool kField>
 __global__ void __launch_bounds__(kHxThreads)
 k_hexop(const __grid_constant__ HexKe ke, HexOpShape s, double ck, const double *__restrict__ ckf, const double *__restrict__ x,
@@ -80,29 +113,10 @@ k_hexop(const __grid_constant__ HexKe ke, HexOpShape s, double ck, const double 
   const int tx = threadIdx.x % kHxBX, ty = (threadIdx.x / kHxBX) % kHxBY, tz = threadIdx.x / (kHxBX * kHxBY);
   const int lx = lx0 + tx, ly = ly0 + ty, lz = lz0 + tz;
   if (lx > g.nx || ly > g.ny || lz > g.nz) return;
-  double r0 = 0.0, r1 = 0.0, r2 = 0.0;
-#pragma unroll
-  for (int la = 0; la < 8; ++la) {
-    const int ax = la & 1, ay = (la >> 1) & 1, az = la >> 2;
-    const int ox = lx - ax, oy = ly - ay, oz = lz - az;
-    if (ox < 0 || ox >= g.nx || oy < 0 || oy >= g.ny || oz < 0 || oz >= g.nz) continue;
-    const double c = kField ? sc[kField ? tz + 1 - az : 0][kField ? ty + 1 - ay : 0][kField ? tx + 1 - ax : 0] : ck;
-    double a0 = 0.0, a1 = 0.0, a2 = 0.0;
-#pragma unroll
-    for (int lb = 0; lb < 8; ++lb) {
-      const double *xs = &sx[tz + 1 - az + (lb >> 2)][ty + 1 - ay + ((lb >> 1) & 1)][3 * (tx + 1 - ax + (lb & 1))];
-#pragma unroll
-      for (int e = 0; e < 3; ++e) {
-        const double u = __dmul_rn(c, xs[e]);                                   // :279  Ck * U
-        a0 = __fma_rn(ke.k[(3 * la + 0) * 24 + 3 * lb + e], u, a0);              // :279  Ke @ (Ck * U)
-        a1 = __fma_rn(ke.k[(3 * la + 1) * 24 + 3 * lb + e], u, a1);
-        a2 = __fma_rn(ke.k[(3 * la + 2) * 24 + 3 * lb + e], u, a2);
-      }
-    }
-    r0 = __dadd_rn(r0, a0);                                                     // :300  np.bincount's order
-    r1 = __dadd_rn(r1, a1);
-    r2 = __dadd_rn(r2, a2);
-  }
+  double r0, r1, r2;
+  hex_node_rows(ke, g, lx, ly, lz,
+                [&](int ax, int ay, int az) { return kField ? sc[kField ? tz + 1 - az : 0][kField ? ty + 1 - ay : 0][kField ? tx + 1 - ax : 0] : ck; },
+                [&](int dx, int dy, int dz) { return &sx[tz + 1 + dz][ty + 1 + dy][3 * (tx + 1 + dx)]; }, r0, r1, r2);
   const int64_t node = ((int64_t)lz * (g.ny + 1) + ly) * g.nxf + (lx - g.x_lo);
   y[3 * node + 0] = r0;
   y[3 * node + 1] = r1;

@@ -16,6 +16,7 @@
 #include "ebe_ordered.cuh"
 #include "gmg.cuh"
 #include "hexop.cuh"
+#include "gmg_rap.cuh"
 #include "fields.cuh"
 
 using namespace pcgb;
@@ -1059,6 +1060,11 @@ struct MgLevel {
   // with hexop.cuh (Ke, uniform Ck = E 2^glev h) instead of the CSR above, which they leave empty
   bool index_free = false;
   HexOp H;
+  // level 1 of a rap hierarchy (pcgb_mg_create_field_rap): y = P^T A_0 P x by k_mg_rap1 from the fine Ck field, no matrix
+  bool rap = false;
+  RapShape R{};
+  HexKe ke{};
+  const double *ck_fine = nullptr;
   double *dinv = nullptr;                                    // inverse diagonal (level 0: a copy of the caller's Minv)
   double *b = nullptr, *x = nullptr;                         // right-hand side and correction (level 0: the caller's r and z)
   double *r = nullptr, *d = nullptr, *q = nullptr;           // smoother residual, direction, operator product
@@ -1077,6 +1083,7 @@ struct pcgb_mg_s {
   double lo = 0.25;
   int la = -1;                     // gathered ranked level (-1: one rank)
   bool index_free = false;         // smoothed coarse levels are HexOps, not CSR matrices
+  bool rap = false;                // field hierarchy with a matrix-free level 1 (pcgb_mg_create_field_rap)
   pcgb_halo_t gather = nullptr;    // all-to-all plan over the global box of level la (not owned)
   int nc = 0;
   double *chol = nullptr;   // coarsest level: dense Cholesky factor, L in the lower triangle mirrored into the upper
@@ -1101,12 +1108,22 @@ namespace {
 
 constexpr int kMgLanczosSteps = 20;
 
+// y_1 = P^T A_0 P x_1 on level 1 of a rap hierarchy
+int rap1_apply(const MgLevel &L, const double *x, double *y, cudaStream_t st, int *nl, const int *skip) {
+  const unsigned grid = (unsigned)((int64_t)L.R.nbx * L.R.nby * L.R.nbz);
+  k_mg_rap1<<<grid, kRapThreads, kRapSmem, st>>>(L.ke, L.R, L.ck_fine, x, y, skip);
+  PCGB_CHECK_LAUNCH();
+  if (nl) *nl += 1;
+  return PCGB_OK;
+}
+
 // y = A x on level l, then the level's exchange-add on a ranked level.  The exchange runs whatever the loop state, like
 // the fine halo of the iteration: every rank enqueues the same exchanges and all ranks stop at the same iteration.
 int mg_op(pcgb_mg_t mg, int l, const double *x, double *y, cudaStream_t st, int *nl, const int *skip) {
   const MgLevel &L = mg->lv[(size_t)l];
   if (l == 0) PCGB_TRY(mg->s->op.apply(x, y, st, nl, skip));
   else if (L.index_free) PCGB_TRY(hexop_apply(L.H, x, y, st, nl, skip));
+  else if (L.rap) PCGB_TRY(rap1_apply(L, x, y, st, nl, skip));
   else PCGB_TRY(spmv_launch(L.P, x, y, false, st, nl, skip));
   return L.halo ? halo_exchange_add(L.halo, y, st, nl) : PCGB_OK;
 }
@@ -1760,6 +1777,61 @@ int mg_gather_elements(pcgb_mg_t mg) {
   return halo_exchange_add(mg->kel_gather, kg, 0);
 }
 
+// largest slab of level-1 element matrices a rap set-up holds (at least one pair of element layers)
+constexpr int64_t kMgRapSlabBytes = int64_t(1) << 30;
+
+// Rap hierarchies: level 1 applied by k_mg_rap1, and level 2's Galerkin element matrices (into mg->kel) built without holding
+// level 1's.  In ascending z, a slab of level-1 element layers (an even number, at most kMgRapSlabBytes, at least 2) is built
+// from the fine field with k_mg_galerkin, its diagonal entries are added into level 1's diagonal (L1.r, zeroed), and each
+// finished pair of layers gives one layer of level-2 matrices, k_mg_galerkin from the slab.  Every level-1 matrix is the
+// field hierarchy's bit for bit, so are the level-2 matrices and the diagonal.  Then D^-1 = 1 / diagonal.
+int mg_rap_level1(pcgb_mg_t mg, const double *ke_host) {
+  MgLevel &L1 = mg->lv[1];
+  const HexGeom &G0 = mg->lv[0].g, &G1 = L1.g, &G2 = mg->lv[2].g;
+  const int64_t layer = (int64_t)G1.nx * G1.ny, layer2 = (int64_t)G2.nx * G2.ny;
+  const int64_t layer_bytes = 576 * (int64_t)sizeof(double) * layer;
+  const int per = (int)std::min<int64_t>(G1.nz, std::max<int64_t>(2, (kMgRapSlabBytes / layer_bytes) & ~int64_t(1)));
+  const int64_t bytes2 = 576 * (int64_t)sizeof(double) * layer2 * G2.nz;
+  L1.rap = true;
+  L1.R = rap_shape(G0, G1);
+  std::memcpy(L1.ke.k, ke_host, sizeof(L1.ke.k));
+  L1.ck_fine = mg->ck_fine;
+  PCGB_CUDA(cudaFuncSetAttribute(k_mg_rap1, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kRapSmem));
+  PCGB_CUDA(cudaMemcpyToSymbol(c_hex_ke, ke_host, 24 * 24 * sizeof(double)));
+  PCGB_CUDA(cudaMemset(L1.r, 0, (size_t)L1.n * sizeof(double)));
+  PCGB_CUDA(cudaMalloc(&mg->kel, (size_t)bytes2));   // freed by the build or by pcgb_mg_destroy
+  double *slab = nullptr;
+  PCGB_CUDA(cudaMalloc(&slab, (size_t)(per * layer_bytes)));
+  mg->kel_peak = std::max(mg->kel_peak, bytes2 + per * layer_bytes);
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  cudaEventCreate(&e0);
+  cudaEventCreate(&e1);
+  cudaError_t err = cudaSuccess;
+  for (int z0 = 0; z0 < G1.nz && err == cudaSuccess; z0 += per) {
+    const int k = std::min(per, G1.nz - z0);   // even: G1.nz and per are
+    cudaEventRecord(e0, 0);
+    k_mg_galerkin<<<(unsigned)(k * layer), kMgGalerkinThreads>>>(G1.nx, G1.ny, G0.nx, G0.ny, mg->ck_fine, nullptr, slab, z0 * layer, 0);
+    k_mg_galerkin<<<(unsigned)(k / 2 * layer2), kMgGalerkinThreads>>>(G2.nx, G2.ny, G1.nx, G1.ny, nullptr, slab,
+                                                                      mg->kel + 576 * (z0 / 2) * layer2, z0 / 2 * layer2, z0 * layer);
+    cudaEventRecord(e1, 0);
+    const int64_t nodes = (int64_t)G1.nxf * (G1.ny + 1) * (k + 1);
+    k_mg_rap_diag<<<(unsigned)((nodes + 255) / 256), 256>>>(G1, z0, z0 + k, slab, L1.r);
+    err = cudaGetLastError();
+    if (err == cudaSuccess) err = cudaEventSynchronize(e1);
+    float ms = 0.0f;
+    if (err == cudaSuccess) cudaEventElapsedTime(&ms, e0, e1);
+    mg->galerkin_ms += ms;
+  }
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  if (err == cudaSuccess) err = cudaDeviceSynchronize();
+  cudaFree(slab);
+  if (err != cudaSuccess) return fail(PCGB_ERR_CUDA, "pcgb_mg_create_field_rap: level-1 set-up failed: %s", cudaGetErrorString(err));
+  k_reciprocal<<<vec_grid(L1.n), 256>>>(L1.n, L1.r, L1.dinv);
+  PCGB_CHECK_LAUNCH();
+  return PCGB_OK;
+}
+
 // largest eigenvalue of the symmetric tridiagonal matrix (diagonal a, off-diagonal b) by bisection on the Sturm count
 double tridiag_max_eig(const std::vector<double> &a, const std::vector<double> &b) {
   const size_t k = a.size();
@@ -1930,7 +2002,8 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
       }
     }
     // field: the level's Galerkin element matrices (level la + 1, the global box of la, holds the gathered ones)
-    if (mg->ck_fine && l > 0 && l != mg->la + 1) PCGB_TRY(mg_galerkin_level(mg, l, ke_host));
+    // (rap: levels 1 and 2 come from mg_rap_level1)
+    if (mg->ck_fine && l > 0 && l != mg->la + 1 && !(mg->rap && l <= 2)) PCGB_TRY(mg_galerkin_level(mg, l, ke_host));
     if (l == nlev - 1) {   // coarsest: dense Cholesky factor of its matrix
       int64_t *rp = nullptr, nnz = 0;
       int *col = nullptr;
@@ -1957,7 +2030,10 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
     PCGB_CUDA(alloc(&L.r, L.n));
     PCGB_CUDA(alloc(&L.d, L.n));
     PCGB_CUDA(alloc(&L.q, L.n));
-    if (l > 0 && mg->index_free) {   // the level's box applied by hexop.cuh; D from its diagonal kernel
+    if (l == 1 && mg->rap) {
+      PCGB_CUDA(alloc(&L.dinv, L.n));
+      PCGB_TRY(mg_rap_level1(mg, ke_host));
+    } else if (l > 0 && mg->index_free) {   // the level's box applied by hexop.cuh; D from its diagonal kernel
       L.index_free = true;
       L.H = hexop_of(L.g, ke_host, ck, nullptr);
       PCGB_CUDA(alloc(&L.dinv, L.n));
@@ -2016,7 +2092,7 @@ int field_bad(int64_t n, const double *d_v, cudaStream_t st, const char *who, in
 // from d_ck_fine or, NULL, Ck = E h)
 int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, const double *d_ck_fine,
                   const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out, const char *who, bool any_rule = false,
-                  bool index_free = false) {
+                  bool index_free = false, bool rap = false) {
   PCGB_TRY(require_device());
   if (!s || !box || !ke_host || !d_minv_fine || !out) return fail(PCGB_ERR_ARG, "%s: null argument", who);
   if (s->halo || s->comm) return fail(PCGB_ERR_ARG, "%s: one rank only (the solver has a halo plan or a communicator)", who);
@@ -2037,6 +2113,8 @@ int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_hos
     mg_whole_box_levels(geo);
     if (geo.size() < 2) return fail(PCGB_ERR_ARG, "%s: the box does not coarsen (every ne must be even and >= 4)", who);
   }
+  if (rap && geo.size() < 3)
+    return fail(PCGB_ERR_ARG, "%s: the hierarchy has %d levels (at least 3, so that level 1 is smoothed)", who, (int)geo.size());
   if (3 * geo.back().nfree_nodes > kMgMaxCoarse)
     return fail(PCGB_ERR_ARG, "%s: the coarsest level has %lld dofs (at most %d)", who, (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
   if (geo.size() > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "%s: more than %d levels", who, PCGB_MG_MAX_LEVELS);
@@ -2057,7 +2135,7 @@ int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_hos
     d_ck_fine = ck_uniform;
   }
   pcgb_mg_t mg = new pcgb_mg_s();
-  mg->s = s; mg->degree = degree; mg->lo = lo; mg->ck_fine = d_ck_fine; mg->index_free = index_free;
+  mg->s = s; mg->degree = degree; mg->lo = lo; mg->ck_fine = d_ck_fine; mg->index_free = index_free; mg->rap = rap;
   mg->lv.resize(geo.size());
   for (size_t l = 0; l < geo.size(); ++l) {
     MgLevel &L = mg->lv[l];
@@ -2065,7 +2143,7 @@ int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_hos
     if (l < any.size()) { L.any = any[l] != 0; L.keep = keep[l]; }
   }
   const int rc = mg_build(mg, ke_host, E, h, d_minv_fine, nullptr);
-  mg->ck_fine = nullptr;   // the caller's array: not read after create
+  mg->ck_fine = nullptr;   // the caller's array: not read after create (a rap level 1 keeps it, as the caller does)
   cudaFree(ck_uniform);
   if (rc != PCGB_OK) { pcgb_mg_destroy(mg); return rc; }
   s->mgs.push_back(mg);
@@ -2093,6 +2171,16 @@ int pcgb_mg_create_field(pcgb_solver_t s, const pcgb_hex_box *box, const double 
   return mg_create_one(s, box, ke_host, 1.0, 1.0, d_ck_fine, d_minv_fine, degree, lo, out, "pcgb_mg_create_field");
 }
 
+int pcgb_mg_create_field_rap(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine,
+                             const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
+  if (!d_ck_fine) {
+    PCGB_TRY(require_device());
+    return fail(PCGB_ERR_ARG, "pcgb_mg_create_field_rap: null argument");
+  }
+  return mg_create_one(s, box, ke_host, 1.0, 1.0, d_ck_fine, d_minv_fine, degree, lo, out, "pcgb_mg_create_field_rap", false, false,
+                       true);
+}
+
 int pcgb_mg_create_any(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine, double E, double h,
                        const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
   return mg_create_one(s, box, ke_host, E, h, d_ck_fine, d_minv_fine, degree, lo, out, "pcgb_mg_create_any", true);
@@ -2115,6 +2203,7 @@ int pcgb_mg_level_csr(pcgb_mg_t mg, int level, int64_t *d_rowptr, int32_t *d_col
                 (int)mg->lv.size() - 2);
   const MgLevel &L = mg->lv[(size_t)level];
   if (L.index_free) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: level %d is index-free (no CSR)", level);
+  if (L.rap) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: level %d is applied as P^T A P from the fine field (no CSR)", level);
   *nnz = L.P.nnz;
   if (!d_rowptr && !d_col && !d_val) return PCGB_OK;
   if (!d_rowptr || !d_col || !d_val) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: give all three buffers or none");
@@ -2144,7 +2233,19 @@ int pcgb_mg_level_apply(pcgb_mg_t mg, int level, const double *d_x, double *d_y,
   const uintptr_t x0 = (uintptr_t)d_x, y0 = (uintptr_t)d_y, nb = (uintptr_t)L.n * sizeof(double);
   if (x0 < y0 + nb && y0 < x0 + nb) return fail(PCGB_ERR_ARG, "pcgb_mg_level_apply: x and y overlap");
   const cudaStream_t st = (cudaStream_t)stream;
+  if (L.rap) return rap1_apply(L, d_x, d_y, st, nullptr, nullptr);
   return L.index_free ? hexop_apply(L.H, d_x, d_y, st) : spmv_launch(L.P, d_x, d_y, false, st);
+}
+
+int pcgb_mg_level_dinv(pcgb_mg_t mg, int level, double *d_out, void *stream) {
+  PCGB_TRY(require_device());
+  if (!mg || !d_out) return fail(PCGB_ERR_ARG, "pcgb_mg_level_dinv: null argument");
+  if (level < 0 || level + 1 >= (int)mg->lv.size() || level == mg->la)
+    return fail(PCGB_ERR_ARG, "pcgb_mg_level_dinv: level %d is not smoothed (levels 0 .. %d, not the gathered one)", level,
+                (int)mg->lv.size() - 2);
+  const MgLevel &L = mg->lv[(size_t)level];
+  PCGB_CUDA(cudaMemcpyAsync(d_out, L.dinv, (size_t)L.n * sizeof(double), cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
+  return PCGB_OK;
 }
 
 int pcgb_mg_setup_info(pcgb_mg_t mg, double *galerkin_ms, int64_t *element_matrix_peak_bytes) {

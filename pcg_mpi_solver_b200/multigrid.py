@@ -25,6 +25,12 @@ Galerkin products of element matrices (pcgb_mg_create_any), with or without `E_f
 smoothed coarse level applied by the index-free hex-box operator (csrc/hexop.cuh) instead of a CSR matrix
 (pcgb_mg_create_index_free / pcgb_mg_create_ranks_index_free): the hierarchy then holds only vectors and the coarsest
 factor (`index_free_bytes`), which is what lets MG-PCG run a 512^3 box on one 80 GB GPU.
+
+`coarse="rap"` (one rank, default coarsening, with `E_field`) is the field hierarchy with a matrix-free level 1
+(pcgb_mg_create_field_rap): level 1 applies P^T A_0 P from the fine Ck field in one kernel (csrc/gmg_rap.cuh) and levels >= 2
+are the field hierarchy's CSR levels bit for bit, built from slabs of level-1 element matrices that are never held whole
+(`rap_bytes`, `rap_setup_peak_bytes`).  It preconditions a 512^3 voxel model on one 80 GB GPU, where the CSR field
+hierarchy's level 1 alone would take about 49 GB.
 """
 from __future__ import annotations
 
@@ -39,6 +45,8 @@ from .hexmesh import HexBlock, block_field, check_field, field_ck, hex_element_s
 MAX_GATHERED = 1 << 17    # dofs of the largest global box gathered onto every rank (kMgMaxGathered)
 MAX_COARSE = 1536         # dofs of the largest coarsest level (kMgMaxCoarse)
 MAX_GATHERED_ELEMENTS = 4096   # elements of the gathered global box of a multi-rank field hierarchy (kMgMaxGatheredElements)
+RAP_SLAB_BYTES = 1 << 30       # largest slab of level-1 element matrices a rap set-up holds (kMgRapSlabBytes)
+ELEMENT_MATRIX_BYTES = 576 * 8
 
 
 def _halve(b: HexBlock) -> HexBlock:
@@ -78,6 +86,51 @@ def index_free_bytes(ne) -> int:
     if n[-1] > MAX_COARSE:
         raise ValueError(f"HexMultigrid: the coarsest level has {n[-1]} dofs (at most {MAX_COARSE})")
     return 8 * (5 * n[0] + 6 * sum(n[1:-1]) + 2 * n[-1] + n[-1] ** 2)
+
+
+def _rap_levels(ne):
+    """The default coarsening's levels and free dofs, refused (ValueError) as pcgb_mg_create_field_rap refuses the box."""
+    lv = _whole_levels(ne)
+    if len(lv) < 2:
+        raise ValueError(f"HexMultigrid: the box {tuple(ne)} does not coarsen (every ne must be even and >= 4)")
+    n = [3 * v[0] * (v[1] + 1) * (v[2] + 1) for v in lv]
+    if n[-1] > MAX_COARSE:
+        raise ValueError(f"HexMultigrid: the coarsest level has {n[-1]} dofs (at most {MAX_COARSE})")
+    if len(lv) < 3:
+        raise ValueError(f"HexMultigrid: coarse='rap' needs at least 3 levels, the box {tuple(ne)} has {len(lv)} "
+                         "(level 1 would be the coarsest)")
+    return lv, n
+
+
+def hex_csr_nnz(ne) -> int:
+    """Non-zeros of the clamped stiffness matrix of the whole box ne (x = 0 nodes dropped): 9 times the free neighbour pairs,
+    which factor per axis into 3 m - 2 for an axis of m free nodes (nx on x, ny + 1 and nz + 1 on y and z)."""
+    return 9 * (3 * ne[0] - 2) * (3 * (ne[1] + 1) - 2) * (3 * (ne[2] + 1) - 2)
+
+
+def rap_bytes(ne) -> int:
+    """Device bytes pcgb_mg_info reports for the rap hierarchy of the whole box `ne`: the vectors of `index_free_bytes`,
+    plus levels 2 .. L-2 as CSR, 12 nnz + 4 (n + 1) bytes each (8 (n + 1) from 2^31 - 1 non-zeros on, int64 row offsets).
+    Raises ValueError where pcgb_mg_create_field_rap refuses the box."""
+    lv, n = _rap_levels(ne)
+    vectors = 8 * (5 * n[0] + 6 * sum(n[1:-1]) + 2 * n[-1] + n[-1] ** 2)
+    csr = 0
+    for l in range(2, len(lv) - 1):
+        nnz = hex_csr_nnz(lv[l])
+        csr += 12 * nnz + (4 if nnz < 2**31 - 1 else 8) * (n[l] + 1)
+    return vectors + csr
+
+
+def rap_setup_peak_bytes(ne) -> int:
+    """Peak bytes of element matrices a rap set-up holds (pcgb_mg_setup_info): level 2's, plus the larger of a slab of level-1
+    layers (an even number of layers of 4608 nx_1 ny_1 bytes, at most RAP_SLAB_BYTES, at least 2, at most nz_1) and level
+    3's (built from level 2's; 0 when there are only 3 levels).  Raises ValueError where create refuses the box."""
+    lv, _ = _rap_levels(ne)
+    layer = ELEMENT_MATRIX_BYTES * lv[1][0] * lv[1][1]
+    per = min(lv[1][2], max(2, (RAP_SLAB_BYTES // layer) & ~1))
+    elems = [v[0] * v[1] * v[2] for v in lv]
+    l3 = ELEMENT_MATRIX_BYTES * elems[3] if len(lv) > 3 else 0
+    return ELEMENT_MATRIX_BYTES * elems[2] + max(per * layer, l3)
 
 
 def gathered_elements(levels) -> int:
@@ -159,10 +212,14 @@ class HexMultigrid:
     (pcgb_mg_create_any).  "any" builds 4608 bytes of element matrices per level-1 element during the set-up and sets up
     slower than the rediscretised default.  Any other string, or "any" with a multi-rank `op`, raises ValueError.
 
-    coarse: "csr" (the default: every smoothed coarse level a device-generated CSR matrix) or "index_free" (those levels
+    coarse: "csr" (the default: every smoothed coarse level a device-generated CSR matrix), "index_free" (those levels
     applied by the index-free hex-box operator, Ck = block.E 2^l block.h; `index_free_bytes` gives the one-rank hierarchy's
-    device bytes).  "index_free" with E_field or coarsening="any" raises ValueError, as does any other string: Galerkin
-    coarse matrices and odd or kept axes are not one Ke on one box."""
+    device bytes) or "rap" (one rank, default coarsening, E_field required: level 1 applied as P^T A_0 P from the fine Ck
+    field without a matrix, levels >= 2 the CSR field hierarchy's bit for bit; `rap_bytes` and `rap_setup_peak_bytes`).
+    "index_free" with E_field or coarsening="any" raises ValueError, as does any other string: Galerkin coarse matrices and
+    odd or kept axes are not one Ke on one box.  "rap" raises ValueError before any library call without E_field, with
+    coarsening="any", with a multi-rank `op` and for a box `rap_bytes` refuses (fewer than 3 levels among them).  A rap
+    handle keeps the fine Ck field on the device (8 bytes per element) and reads it in every V-cycle."""
 
     def __init__(self, op, block: HexBlock, degree: int = 2, lo: float = 0.25, minv: torch.Tensor | None = None, blocks=None,
                  E_field=None, coarsening: str = "even", coarse: str = "csr"):
@@ -172,16 +229,25 @@ class HexMultigrid:
         self._h = ctypes.c_void_p()
         self._halos = []
         self.levels = None
+        self._ck = None
         comm = getattr(op, "comm", None)
         ranked = comm is not None and comm.nranks > 1
         if coarsening not in ("even", "any"):
             raise ValueError(f"HexMultigrid: coarsening must be 'even' or 'any', not {coarsening!r}")
         self.coarsening = coarsening
-        if coarse not in ("csr", "index_free"):
-            raise ValueError(f"HexMultigrid: coarse must be 'csr' or 'index_free', not {coarse!r}")
+        if coarse not in ("csr", "index_free", "rap"):
+            raise ValueError(f"HexMultigrid: coarse must be 'csr', 'index_free' or 'rap', not {coarse!r}")
         if coarse == "index_free" and (E_field is not None or coarsening == "any"):
             raise ValueError("HexMultigrid: coarse='index_free' needs the default coarsening and no E_field "
                              "(Galerkin coarse levels are not one element matrix on one box)")
+        if coarse == "rap":
+            if E_field is None:
+                raise ValueError("HexMultigrid: coarse='rap' needs E_field (its level 1 is P^T A P of the fine field)")
+            if coarsening != "even":
+                raise ValueError("HexMultigrid: coarse='rap' needs the default coarsening")
+            if ranked:
+                raise ValueError("HexMultigrid: coarse='rap' is supported on one rank only")
+            rap_bytes(block.ne)
         self.coarse = coarse
         index_free = coarse == "index_free"
         if coarsening == "any":
@@ -202,11 +268,13 @@ class HexMultigrid:
             minv = op.jacobi() if minv is None else minv.to(self.device, torch.float64).contiguous()
             ke = np.ascontiguousarray(hex_element_stiffness(1.0, block.nu))
             box = block.cbox()
+            name = "pcgb_mg_create_field_rap" if coarse == "rap" else "pcgb_mg_create_field"
             with torch.cuda.device(self.device):
                 torch.cuda.synchronize(self.device)
-                _lib.check(_lib.load().pcgb_mg_create_field(op._solver, ctypes.byref(box), ke.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
-                                                            _lib.ptr(ck), _lib.ptr(minv), self.degree, self.lo, ctypes.byref(self._h)),
-                           "pcgb_mg_create_field")
+                _lib.check(getattr(_lib.load(), name)(op._solver, ctypes.byref(box), ke.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
+                                                      _lib.ptr(ck), _lib.ptr(minv), self.degree, self.lo, ctypes.byref(self._h)), name)
+            if coarse == "rap":
+                self._ck = ck          # read by every V-cycle: it lives as long as the handle
             return
         if ranked:
             if blocks is None or len(blocks) != comm.nranks:
@@ -280,7 +348,7 @@ class HexMultigrid:
 
     def info(self) -> dict:
         """levels, n per level, largest-eigenvalue estimates of D^-1 A per level (0 for the coarsest and for the gathered
-        level), device bytes, coarse ("csr" or "index_free"); across ranks also gather_level (la, -1 on one rank),
+        level), device bytes, coarse ("csr", "index_free" or "rap"); across ranks also gather_level (la, -1 on one rank),
         n_gathered and global_lambda (the estimates of the global hierarchy: ranked levels below la, then the replicated
         ones)."""
         lib = _lib.load()
@@ -330,6 +398,13 @@ class HexMultigrid:
             _lib.check(lib.pcgb_mg_level_csr(self._h, level, _lib.ptr(rowptr), _lib.ptr(col), _lib.ptr(val), ctypes.byref(nnz),
                                              _lib.stream_ptr()), "pcgb_mg_level_csr")
         return rowptr, col, val
+
+    def level_dinv(self, level: int) -> torch.Tensor:
+        """D^-1 of smoothed level `level` (0 .. levels - 2, not the gathered level) as a device tensor, any hierarchy kind."""
+        d = self._vec(self.info()["n"][level])
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().pcgb_mg_level_dinv(self._h, level, _lib.ptr(d), _lib.stream_ptr()), "pcgb_mg_level_dinv")
+        return d
 
     def level_apply(self, level: int, x: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
         """y = A_l x on smoothed coarse level `level` (1 .. levels - 2, not the gathered level), either coarse kind: the
