@@ -1044,6 +1044,12 @@ int trace_host(pcgb_solver_t s, int kind, const PcgCtrl &c, double rr, bool has_
 // copy of a shared dof holds the full value) and every operator application and restriction is followed by the level's
 // exchange-add.  Level la is not smoothed: its vector is gathered into the global box, which levels la+1 .. hold as a
 // replicated one-rank hierarchy on every rank.  One rank: la = -1 and every level is a whole box.
+
+// What a level applies: the solver's operator (level 0), the level's CSR matrix, the index-free operator of its box
+// (pcgb_mg_create_index_free / _ranks_index_free: Ke, uniform Ck = E 2^glev h), P^T A_0 P from the fine Ck field (level 1
+// of pcgb_mg_create_field_rap), or nothing (the gathered level and the coarsest level).
+enum class MgOp { None, Fine, Csr, Hex, Rap };
+
 struct MgLevel {
   HexGeom g{};
   MgPlace place{};             // the box inside the level's global box (one rank: the box itself at e0 = 0)
@@ -1051,18 +1057,13 @@ struct MgLevel {
   pcgb_halo_t halo = nullptr;  // ranked levels: exchange-add of the level (level 0: the solver's halo; not owned)
   double *own = nullptr;       // ranked levels: 0/1 ownership of the dofs (copy)
   int64_t n = 0;
-  void *rowptr = nullptr;   // coarse levels above the coarsest: device-generated CSR (int32 offsets below 2^31 non-zeros)
+  MgOp op = MgOp::None;
+  void *rowptr = nullptr;   // Csr: device-generated CSR (int32 offsets below 2^31 non-zeros)
   int *col = nullptr;
   double *val = nullptr;
   CsrPlan P;
-  bool has_plan = false;
-  // index-free hierarchies (pcgb_mg_create_index_free / _ranks_index_free): smoothed levels l >= 1 apply the level's box
-  // with hexop.cuh (Ke, uniform Ck = E 2^glev h) instead of the CSR above, which they leave empty
-  bool index_free = false;
-  HexOp H;
-  // level 1 of a rap hierarchy (pcgb_mg_create_field_rap): y = P^T A_0 P x by k_mg_rap1 from the fine Ck field, no matrix
-  bool rap = false;
-  RapShape R{};
+  HexOp H;                  // Hex
+  RapShape R{};             // Rap: y = P^T A_0 P x by k_mg_rap1 from Ke and the fine Ck field, no matrix
   HexKe ke{};
   const double *ck_fine = nullptr;
   double *dinv = nullptr;                                    // inverse diagonal (level 0: a copy of the caller's Minv)
@@ -1082,8 +1083,6 @@ struct pcgb_mg_s {
   int degree = 2;
   double lo = 0.25;
   int la = -1;                     // gathered ranked level (-1: one rank)
-  bool index_free = false;         // smoothed coarse levels are HexOps, not CSR matrices
-  bool rap = false;                // field hierarchy with a matrix-free level 1 (pcgb_mg_create_field_rap)
   pcgb_halo_t gather = nullptr;    // all-to-all plan over the global box of level la (not owned)
   int nc = 0;
   double *chol = nullptr;   // coarsest level: dense Cholesky factor, L in the lower triangle mirrored into the upper
@@ -1108,23 +1107,31 @@ namespace {
 
 constexpr int kMgLanczosSteps = 20;
 
-// y_1 = P^T A_0 P x_1 on level 1 of a rap hierarchy
-int rap1_apply(const MgLevel &L, const double *x, double *y, cudaStream_t st, int *nl, const int *skip) {
-  const unsigned grid = (unsigned)((int64_t)L.R.nbx * L.R.nby * L.R.nbz);
-  k_mg_rap1<<<grid, kRapThreads, kRapSmem, st>>>(L.ke, L.R, L.ck_fine, x, y, skip);
-  PCGB_CHECK_LAUNCH();
-  if (nl) *nl += 1;
-  return PCGB_OK;
+// whether level l is smoothed: every level above the coarsest but the gathered one
+bool mg_smoothed(pcgb_mg_t mg, int l) { return l >= 0 && l + 1 < (int)mg->lv.size() && l != mg->la; }
+
+// y = A x on level l, the rank's local product (no exchange-add)
+int level_apply(pcgb_mg_t mg, int l, const double *x, double *y, cudaStream_t st, int *nl, const int *skip) {
+  const MgLevel &L = mg->lv[(size_t)l];
+  switch (L.op) {
+    case MgOp::Fine: return mg->s->op.apply(x, y, st, nl, skip);
+    case MgOp::Csr: return spmv_launch(L.P, x, y, false, st, nl, skip);
+    case MgOp::Hex: return hexop_apply(L.H, x, y, st, nl, skip);
+    case MgOp::Rap:
+      k_mg_rap1<<<(unsigned)((int64_t)L.R.nbx * L.R.nby * L.R.nbz), kRapThreads, kRapSmem, st>>>(L.ke, L.R, L.ck_fine, x, y, skip);
+      PCGB_CHECK_LAUNCH();
+      if (nl) *nl += 1;
+      return PCGB_OK;
+    case MgOp::None: break;
+  }
+  return fail(PCGB_ERR_ARG, "level %d has no operator", l);
 }
 
 // y = A x on level l, then the level's exchange-add on a ranked level.  The exchange runs whatever the loop state, like
 // the fine halo of the iteration: every rank enqueues the same exchanges and all ranks stop at the same iteration.
 int mg_op(pcgb_mg_t mg, int l, const double *x, double *y, cudaStream_t st, int *nl, const int *skip) {
   const MgLevel &L = mg->lv[(size_t)l];
-  if (l == 0) PCGB_TRY(mg->s->op.apply(x, y, st, nl, skip));
-  else if (L.index_free) PCGB_TRY(hexop_apply(L.H, x, y, st, nl, skip));
-  else if (L.rap) PCGB_TRY(rap1_apply(L, x, y, st, nl, skip));
-  else PCGB_TRY(spmv_launch(L.P, x, y, false, st, nl, skip));
+  PCGB_TRY(level_apply(mg, l, x, y, st, nl, skip));
   return L.halo ? halo_exchange_add(L.halo, y, st, nl) : PCGB_OK;
 }
 
@@ -1673,7 +1680,7 @@ int pcgb_mg_destroy(pcgb_mg_t mg) {
   if (s) s->mgs.erase(std::remove(s->mgs.begin(), s->mgs.end(), mg), s->mgs.end());
   for (size_t l = 0; l < mg->lv.size(); ++l) {
     MgLevel &L = mg->lv[l];
-    if (L.has_plan) free_plan(L.P);
+    if (L.op == MgOp::Csr) free_plan(L.P);
     cudaFree(L.rowptr); cudaFree(L.col); cudaFree(L.val); cudaFree(L.dinv); cudaFree(L.own);
     if (l > 0) { cudaFree(L.b); cudaFree(L.x); }
     cudaFree(L.r); cudaFree(L.d); cudaFree(L.q);
@@ -1784,7 +1791,7 @@ constexpr int64_t kMgRapSlabBytes = int64_t(1) << 30;
 // level 1's.  In ascending z, a slab of level-1 element layers (an even number, at most kMgRapSlabBytes, at least 2) is built
 // from the fine field with k_mg_galerkin, its diagonal entries are added into level 1's diagonal (L1.r, zeroed), and each
 // finished pair of layers gives one layer of level-2 matrices, k_mg_galerkin from the slab.  Every level-1 matrix is the
-// field hierarchy's bit for bit, so are the level-2 matrices and the diagonal.  Then D^-1 = 1 / diagonal.
+// field hierarchy's bit for bit, so are the level-2 matrices and the diagonal.
 int mg_rap_level1(pcgb_mg_t mg, const double *ke_host) {
   MgLevel &L1 = mg->lv[1];
   const HexGeom &G0 = mg->lv[0].g, &G1 = L1.g, &G2 = mg->lv[2].g;
@@ -1792,7 +1799,6 @@ int mg_rap_level1(pcgb_mg_t mg, const double *ke_host) {
   const int64_t layer_bytes = 576 * (int64_t)sizeof(double) * layer;
   const int per = (int)std::min<int64_t>(G1.nz, std::max<int64_t>(2, (kMgRapSlabBytes / layer_bytes) & ~int64_t(1)));
   const int64_t bytes2 = 576 * (int64_t)sizeof(double) * layer2 * G2.nz;
-  L1.rap = true;
   L1.R = rap_shape(G0, G1);
   std::memcpy(L1.ke.k, ke_host, sizeof(L1.ke.k));
   L1.ck_fine = mg->ck_fine;
@@ -1826,10 +1832,8 @@ int mg_rap_level1(pcgb_mg_t mg, const double *ke_host) {
   cudaEventDestroy(e1);
   if (err == cudaSuccess) err = cudaDeviceSynchronize();
   cudaFree(slab);
-  if (err != cudaSuccess) return fail(PCGB_ERR_CUDA, "pcgb_mg_create_field_rap: level-1 set-up failed: %s", cudaGetErrorString(err));
-  k_reciprocal<<<vec_grid(L1.n), 256>>>(L1.n, L1.r, L1.dinv);
-  PCGB_CHECK_LAUNCH();
-  return PCGB_OK;
+  return err == cudaSuccess ? PCGB_OK
+                            : fail(PCGB_ERR_CUDA, "pcgb_mg_create_field_rap: level-1 set-up failed: %s", cudaGetErrorString(err));
 }
 
 // largest eigenvalue of the symmetric tridiagonal matrix (diagonal a, off-diagonal b) by bisection on the Sturm count
@@ -1962,9 +1966,11 @@ constexpr int64_t kMgMaxGathered = 1 << 17;
 // (ranks - 1) * 576 entries per element)
 constexpr int64_t kMgMaxGatheredElements = 4096;
 
-// Builds the levels whose geometry (g, place, glev) and halos the caller has set in mg->lv.  own: ownership weights of
-// the ranked levels 0 .. la (copied).
-int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const double *d_minv_fine, const double *const *own) {
+// Builds the levels whose geometry (g, place, glev) and halos the caller has set in mg->lv.  coarse: what the smoothed
+// coarse levels apply (Rap: level 1, with CSR matrices below it).  own: ownership weights of the ranked levels 0 .. la
+// (copied).
+int mg_build(pcgb_mg_t mg, MgOp coarse, const double *ke_host, double E, double h, const double *d_minv_fine,
+             const double *const *own) {
   const int nlev = (int)mg->lv.size();
   auto alloc = [&](double **p, int64_t n) -> cudaError_t {
     mg->bytes += 8 * n;
@@ -1982,10 +1988,9 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
     MgLevel &L = mg->lv[(size_t)l];
     L.n = 3 * L.g.nfree_nodes;
     const double ck = E * h * (double)(1ll << L.glev);
+    L.op = l == 0 ? MgOp::Fine : l == mg->la || l == nlev - 1 ? MgOp::None : coarse == MgOp::Rap && l > 1 ? MgOp::Csr : coarse;
     if (l == 0) {
       PCGB_CUDA(alloc(&mg->z, L.n));
-      PCGB_CUDA(alloc(&L.dinv, L.n));
-      PCGB_CUDA(cudaMemcpy(L.dinv, d_minv_fine, (size_t)L.n * sizeof(double), cudaMemcpyDeviceToDevice));
     } else {
       PCGB_CUDA(alloc(&L.b, L.n));
       PCGB_CUDA(alloc(&L.x, L.n));
@@ -2003,7 +2008,7 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
     }
     // field: the level's Galerkin element matrices (level la + 1, the global box of la, holds the gathered ones)
     // (rap: levels 1 and 2 come from mg_rap_level1)
-    if (mg->ck_fine && l > 0 && l != mg->la + 1 && !(mg->rap && l <= 2)) PCGB_TRY(mg_galerkin_level(mg, l, ke_host));
+    if (mg->ck_fine && l > 0 && l != mg->la + 1 && !(coarse == MgOp::Rap && l <= 2)) PCGB_TRY(mg_galerkin_level(mg, l, ke_host));
     if (l == nlev - 1) {   // coarsest: dense Cholesky factor of its matrix
       int64_t *rp = nullptr, nnz = 0;
       int *col = nullptr;
@@ -2030,38 +2035,36 @@ int mg_build(pcgb_mg_t mg, const double *ke_host, double E, double h, const doub
     PCGB_CUDA(alloc(&L.r, L.n));
     PCGB_CUDA(alloc(&L.d, L.n));
     PCGB_CUDA(alloc(&L.q, L.n));
-    if (l == 1 && mg->rap) {
-      PCGB_CUDA(alloc(&L.dinv, L.n));
-      PCGB_TRY(mg_rap_level1(mg, ke_host));
-    } else if (l > 0 && mg->index_free) {   // the level's box applied by hexop.cuh; D from its diagonal kernel
-      L.index_free = true;
-      L.H = hexop_of(L.g, ke_host, ck, nullptr);
-      PCGB_CUDA(alloc(&L.dinv, L.n));
-      PCGB_TRY(hexop_diag(L.H, L.r, 0));
-      if (L.halo) PCGB_TRY(halo_exchange_add(L.halo, L.r, 0));   // assembled diagonal of a ranked level
-      k_reciprocal<<<vec_grid(L.n), 256>>>(L.n, L.r, L.dinv);
-      PCGB_CHECK_LAUNCH();
-    } else if (l > 0) {
-      int64_t *rp = nullptr, nnz = 0;
-      const int rc = mg_hex_csr(L.g, ke_host, ck, &rp, &L.col, &L.val, &nnz, mg->kel);
-      L.rowptr = rp;
-      PCGB_TRY(rc);
-      mg->bytes += 12 * nnz + 8 * (L.n + 1);
-      L.P.nrows = L.n; L.P.ncols = L.n; L.P.nnz = nnz; L.P.rowptr = rp; L.P.rp64 = true; L.P.col = L.col; L.P.val = L.val;
-      if (nnz < INT32_MAX) {   // int32 row offsets, as the fine hex matrices use below 2^31 non-zeros
-        std::vector<int64_t> r64((size_t)L.n + 1);
-        PCGB_CUDA(cudaMemcpy(r64.data(), rp, r64.size() * sizeof(int64_t), cudaMemcpyDeviceToHost));
-        std::vector<int32_t> r32(r64.begin(), r64.end());
-        int32_t *rp32 = nullptr;
-        PCGB_CUDA(upload(&rp32, r32));
-        cudaFree(rp);
-        L.rowptr = rp32; L.P.rowptr = rp32; L.P.rp64 = false;
-        mg->bytes -= 4 * (L.n + 1);
+    PCGB_CUDA(alloc(&L.dinv, L.n));
+    if (l == 0) {   // D^-1 is the caller's Minv
+      PCGB_CUDA(cudaMemcpy(L.dinv, d_minv_fine, (size_t)L.n * sizeof(double), cudaMemcpyDeviceToDevice));
+    } else {
+      // the level's operator, and the rank's part of its diagonal into L.r
+      if (L.op == MgOp::Rap) {
+        PCGB_TRY(mg_rap_level1(mg, ke_host));
+      } else if (L.op == MgOp::Hex) {
+        L.H = hexop_of(L.g, ke_host, ck, nullptr);
+        PCGB_TRY(hexop_diag(L.H, L.r, 0));
+      } else {
+        int64_t *rp = nullptr, nnz = 0;
+        const int rc = mg_hex_csr(L.g, ke_host, ck, &rp, &L.col, &L.val, &nnz, mg->kel);
+        L.rowptr = rp;
+        PCGB_TRY(rc);
+        mg->bytes += 12 * nnz + 8 * (L.n + 1);
+        L.P.nrows = L.n; L.P.ncols = L.n; L.P.nnz = nnz; L.P.rowptr = rp; L.P.rp64 = true; L.P.col = L.col; L.P.val = L.val;
+        if (nnz < INT32_MAX) {   // int32 row offsets, as the fine hex matrices use below 2^31 non-zeros
+          std::vector<int64_t> r64((size_t)L.n + 1);
+          PCGB_CUDA(cudaMemcpy(r64.data(), rp, r64.size() * sizeof(int64_t), cudaMemcpyDeviceToHost));
+          std::vector<int32_t> r32(r64.begin(), r64.end());
+          int32_t *rp32 = nullptr;
+          PCGB_CUDA(upload(&rp32, r32));
+          cudaFree(rp);
+          L.rowptr = rp32; L.P.rowptr = rp32; L.P.rp64 = false;
+          mg->bytes -= 4 * (L.n + 1);
+        }
+        PCGB_TRY(L.P.rp64 ? build_plan_t<int64_t>(L.P, 0) : build_plan_t<int32_t>(L.P, 0));
+        PCGB_TRY(csr_diag_compute(L.P, L.r, 0));
       }
-      L.has_plan = true;
-      PCGB_TRY(L.P.rp64 ? build_plan_t<int64_t>(L.P, 0) : build_plan_t<int32_t>(L.P, 0));
-      PCGB_CUDA(alloc(&L.dinv, L.n));
-      PCGB_TRY(csr_diag_compute(L.P, L.r, 0));
       if (L.halo) PCGB_TRY(halo_exchange_add(L.halo, L.r, 0));   // assembled diagonal of a ranked level
       k_reciprocal<<<vec_grid(L.n), 256>>>(L.n, L.r, L.dinv);
       PCGB_CHECK_LAUNCH();
@@ -2087,23 +2090,64 @@ int field_bad(int64_t n, const double *d_v, cudaStream_t st, const char *who, in
   return e == cudaSuccess ? PCGB_OK : fail(PCGB_ERR_CUDA, "%s: field check failed: %s", who, cudaGetErrorString(e));
 }
 
-// pcgb_mg_create (d_ck_fine NULL: Ck = E 2^l h on level l; index_free: pcgb_mg_create_index_free), pcgb_mg_create_field
-// (Galerkin levels from d_ck_fine) and pcgb_mg_create_any (any_rule: the coarsening of mg_any_box_levels, Galerkin levels
-// from d_ck_fine or, NULL, Ck = E h)
-int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, const double *d_ck_fine,
-                  const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out, const char *who, bool any_rule = false,
-                  bool index_free = false, bool rap = false) {
+// ---- checks and tail shared by mg_create_one and mg_create_ranks
+int mg_check_ranges(int degree, double lo, double E, double h, const char *who) {
+  if (degree >= 1 && lo > 0.0 && lo < 1.1 && E > 0.0 && h > 0.0) return PCGB_OK;
+  return fail(PCGB_ERR_ARG, "%s: degree >= 1, 0 < lo < 1.1, E > 0 and h > 0 required", who);
+}
+
+int mg_check_rows(pcgb_solver_t s, const pcgb_hex_box *box, const char *who) {
+  const int64_t n = 3 * hex_geom(box).nfree_nodes;
+  if (n == s->n) return PCGB_OK;
+  return fail(PCGB_ERR_ARG, "%s: the solver's operator has %lld rows, the box %lld", who, (long long)s->n, (long long)n);
+}
+
+// geo: the whole-box levels from the global box down; nlev: the levels of the whole hierarchy
+int mg_check_levels(const std::vector<HexGeom> &geo, size_t nlev, const char *who) {
+  if (3 * geo.back().nfree_nodes > kMgMaxCoarse)
+    return fail(PCGB_ERR_ARG, "%s: the coarsest level has %lld dofs (at most %d)", who, (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
+  if (nlev > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "%s: more than %d levels", who, PCGB_MG_MAX_LEVELS);
+  return PCGB_OK;
+}
+
+// the caller's fine Ck field of nel elements
+int mg_check_field(int64_t nel, const double *d_ck_fine, const char *who) {
+  // the check runs on the legacy stream, which does not wait for non-blocking streams: finish whatever work of the caller
+  // may still be writing d_ck_fine first
+  PCGB_CUDA(cudaDeviceSynchronize());
+  int bad = 0;
+  PCGB_TRY(field_bad(nel, d_ck_fine, 0, who, &bad));
+  return bad ? fail(PCGB_ERR_ARG, "%s: every Ck of the field must be finite and positive", who) : PCGB_OK;
+}
+
+// Builds the hierarchy the caller has laid out in mg, forgets the caller's field and element plan (not used after create; a
+// rap level 1 keeps the field, as the caller does), and registers the handle with the solver; destroys it on failure.
+int mg_finish(pcgb_mg_t mg, MgOp coarse, const double *ke_host, double E, double h, const double *d_minv_fine,
+              const double *const *own, pcgb_mg_t *out) {
+  const int rc = mg_build(mg, coarse, ke_host, E, h, d_minv_fine, own);
+  mg->ck_fine = nullptr;
+  mg->kel_gather = nullptr;
+  if (rc != PCGB_OK) { pcgb_mg_destroy(mg); return rc; }
+  mg->s->mgs.push_back(mg);
+  *out = mg;
+  return PCGB_OK;
+}
+
+// pcgb_mg_create (d_ck_fine NULL: Ck = E 2^l h on level l; coarse Hex: pcgb_mg_create_index_free), pcgb_mg_create_field
+// (field: Galerkin levels from d_ck_fine, which must be given; coarse Rap: pcgb_mg_create_field_rap) and pcgb_mg_create_any
+// (any_rule: the coarsening of mg_any_box_levels, Galerkin levels from d_ck_fine or, NULL, Ck = E h)
+int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, bool field,
+                  const double *d_ck_fine, const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out, const char *who,
+                  bool any_rule = false, MgOp coarse = MgOp::Csr) {
   PCGB_TRY(require_device());
-  if (!s || !box || !ke_host || !d_minv_fine || !out) return fail(PCGB_ERR_ARG, "%s: null argument", who);
+  if (!s || !box || !ke_host || !d_minv_fine || !out || (field && !d_ck_fine)) return fail(PCGB_ERR_ARG, "%s: null argument", who);
   if (s->halo || s->comm) return fail(PCGB_ERR_ARG, "%s: one rank only (the solver has a halo plan or a communicator)", who);
-  if (degree < 1 || !(lo > 0.0 && lo < 1.1) || !(E > 0.0) || !(h > 0.0))
-    return fail(PCGB_ERR_ARG, "%s: degree >= 1, 0 < lo < 1.1, E > 0 and h > 0 required", who);
+  PCGB_TRY(mg_check_ranges(degree, lo, E, h, who));
   for (int a = 0; a < 3; ++a)
     if (box->e0[a] != 0 || box->ng[a] != box->ne[a] || box->ne[a] <= 0)
       return fail(PCGB_ERR_ARG, "%s: the box must be the whole mesh (e0 = 0, ng = ne)", who);
+  PCGB_TRY(mg_check_rows(s, box, who));
   std::vector<HexGeom> geo{hex_geom(box)};
-  if (3 * geo[0].nfree_nodes != s->n) return fail(PCGB_ERR_ARG, "%s: the solver's operator has %lld rows, the box %lld",
-                                                  who, (long long)s->n, (long long)(3 * geo[0].nfree_nodes));
   std::vector<int> keep;
   std::vector<char> any;
   if (any_rule) {
@@ -2113,19 +2157,10 @@ int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_hos
     mg_whole_box_levels(geo);
     if (geo.size() < 2) return fail(PCGB_ERR_ARG, "%s: the box does not coarsen (every ne must be even and >= 4)", who);
   }
-  if (rap && geo.size() < 3)
+  if (coarse == MgOp::Rap && geo.size() < 3)
     return fail(PCGB_ERR_ARG, "%s: the hierarchy has %d levels (at least 3, so that level 1 is smoothed)", who, (int)geo.size());
-  if (3 * geo.back().nfree_nodes > kMgMaxCoarse)
-    return fail(PCGB_ERR_ARG, "%s: the coarsest level has %lld dofs (at most %d)", who, (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
-  if (geo.size() > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "%s: more than %d levels", who, PCGB_MG_MAX_LEVELS);
-  if (d_ck_fine) {
-    // the check runs on the legacy stream, which does not wait for non-blocking streams: finish whatever work of the caller
-    // may still be writing d_ck_fine first
-    PCGB_CUDA(cudaDeviceSynchronize());
-    int bad = 0;
-    PCGB_TRY(field_bad((int64_t)geo[0].nx * geo[0].ny * geo[0].nz, d_ck_fine, 0, who, &bad));
-    if (bad) return fail(PCGB_ERR_ARG, "%s: every Ck of the field must be finite and positive", who);
-  }
+  PCGB_TRY(mg_check_levels(geo, geo.size(), who));
+  if (d_ck_fine) PCGB_TRY(mg_check_field((int64_t)geo[0].nx * geo[0].ny * geo[0].nz, d_ck_fine, who));
   // a uniform box under the any rule: Galerkin levels from Ck = E h on every fine element (freed once the levels exist)
   double *ck_uniform = nullptr;
   if (any_rule && !d_ck_fine) {
@@ -2135,55 +2170,44 @@ int mg_create_one(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_hos
     d_ck_fine = ck_uniform;
   }
   pcgb_mg_t mg = new pcgb_mg_s();
-  mg->s = s; mg->degree = degree; mg->lo = lo; mg->ck_fine = d_ck_fine; mg->index_free = index_free; mg->rap = rap;
+  mg->s = s; mg->degree = degree; mg->lo = lo; mg->ck_fine = d_ck_fine;
   mg->lv.resize(geo.size());
   for (size_t l = 0; l < geo.size(); ++l) {
     MgLevel &L = mg->lv[l];
     L.g = geo[l]; L.glev = (int)l; L.place = MgPlace{geo[l], 0, 0, 0};
     if (l < any.size()) { L.any = any[l] != 0; L.keep = keep[l]; }
   }
-  const int rc = mg_build(mg, ke_host, E, h, d_minv_fine, nullptr);
-  mg->ck_fine = nullptr;   // the caller's array: not read after create (a rap level 1 keeps it, as the caller does)
+  const int rc = mg_finish(mg, coarse, ke_host, E, h, d_minv_fine, nullptr, out);
   cudaFree(ck_uniform);
-  if (rc != PCGB_OK) { pcgb_mg_destroy(mg); return rc; }
-  s->mgs.push_back(mg);
-  *out = mg;
-  return PCGB_OK;
+  return rc;
 }
 }  // namespace
 
 int pcgb_mg_create(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h, const double *d_minv_fine,
                    int degree, double lo, pcgb_mg_t *out) {
-  return mg_create_one(s, box, ke_host, E, h, nullptr, d_minv_fine, degree, lo, out, "pcgb_mg_create");
+  return mg_create_one(s, box, ke_host, E, h, false, nullptr, d_minv_fine, degree, lo, out, "pcgb_mg_create");
 }
 
 int pcgb_mg_create_index_free(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, double E, double h,
                               const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
-  return mg_create_one(s, box, ke_host, E, h, nullptr, d_minv_fine, degree, lo, out, "pcgb_mg_create_index_free", false, true);
+  return mg_create_one(s, box, ke_host, E, h, false, nullptr, d_minv_fine, degree, lo, out, "pcgb_mg_create_index_free", false,
+                       MgOp::Hex);
 }
 
 int pcgb_mg_create_field(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine,
                          const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
-  if (!d_ck_fine) {
-    PCGB_TRY(require_device());
-    return fail(PCGB_ERR_ARG, "pcgb_mg_create_field: null argument");
-  }
-  return mg_create_one(s, box, ke_host, 1.0, 1.0, d_ck_fine, d_minv_fine, degree, lo, out, "pcgb_mg_create_field");
+  return mg_create_one(s, box, ke_host, 1.0, 1.0, true, d_ck_fine, d_minv_fine, degree, lo, out, "pcgb_mg_create_field");
 }
 
 int pcgb_mg_create_field_rap(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine,
                              const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
-  if (!d_ck_fine) {
-    PCGB_TRY(require_device());
-    return fail(PCGB_ERR_ARG, "pcgb_mg_create_field_rap: null argument");
-  }
-  return mg_create_one(s, box, ke_host, 1.0, 1.0, d_ck_fine, d_minv_fine, degree, lo, out, "pcgb_mg_create_field_rap", false, false,
-                       true);
+  return mg_create_one(s, box, ke_host, 1.0, 1.0, true, d_ck_fine, d_minv_fine, degree, lo, out, "pcgb_mg_create_field_rap", false,
+                       MgOp::Rap);
 }
 
 int pcgb_mg_create_any(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine, double E, double h,
                        const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
-  return mg_create_one(s, box, ke_host, E, h, d_ck_fine, d_minv_fine, degree, lo, out, "pcgb_mg_create_any", true);
+  return mg_create_one(s, box, ke_host, E, h, false, d_ck_fine, d_minv_fine, degree, lo, out, "pcgb_mg_create_any", true);
 }
 
 int pcgb_mg_level_box(pcgb_mg_t mg, int level, int32_t *ne) {
@@ -2198,12 +2222,12 @@ int pcgb_mg_level_box(pcgb_mg_t mg, int level, int32_t *ne) {
 int pcgb_mg_level_csr(pcgb_mg_t mg, int level, int64_t *d_rowptr, int32_t *d_col, double *d_val, int64_t *nnz, void *stream) {
   PCGB_TRY(require_device());
   if (!mg || !nnz) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: null argument");
-  if (level <= 0 || level + 1 >= (int)mg->lv.size() || level == mg->la)
+  if (level == 0 || !mg_smoothed(mg, level))
     return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: level %d has no coarse CSR (levels 1 .. %d, not the gathered one)", level,
                 (int)mg->lv.size() - 2);
   const MgLevel &L = mg->lv[(size_t)level];
-  if (L.index_free) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: level %d is index-free (no CSR)", level);
-  if (L.rap) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: level %d is applied as P^T A P from the fine field (no CSR)", level);
+  if (L.op == MgOp::Hex) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: level %d is index-free (no CSR)", level);
+  if (L.op == MgOp::Rap) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: level %d is applied as P^T A P from the fine field (no CSR)", level);
   *nnz = L.P.nnz;
   if (!d_rowptr && !d_col && !d_val) return PCGB_OK;
   if (!d_rowptr || !d_col || !d_val) return fail(PCGB_ERR_ARG, "pcgb_mg_level_csr: give all three buffers or none");
@@ -2226,21 +2250,19 @@ int pcgb_mg_level_csr(pcgb_mg_t mg, int level, int64_t *d_rowptr, int32_t *d_col
 int pcgb_mg_level_apply(pcgb_mg_t mg, int level, const double *d_x, double *d_y, void *stream) {
   PCGB_TRY(require_device());
   if (!mg || !d_x || !d_y) return fail(PCGB_ERR_ARG, "pcgb_mg_level_apply: null argument");
-  if (level <= 0 || level + 1 >= (int)mg->lv.size() || level == mg->la)
+  if (level == 0 || !mg_smoothed(mg, level))
     return fail(PCGB_ERR_ARG, "pcgb_mg_level_apply: level %d has no coarse operator (levels 1 .. %d, not the gathered one)", level,
                 (int)mg->lv.size() - 2);
   const MgLevel &L = mg->lv[(size_t)level];
   const uintptr_t x0 = (uintptr_t)d_x, y0 = (uintptr_t)d_y, nb = (uintptr_t)L.n * sizeof(double);
   if (x0 < y0 + nb && y0 < x0 + nb) return fail(PCGB_ERR_ARG, "pcgb_mg_level_apply: x and y overlap");
-  const cudaStream_t st = (cudaStream_t)stream;
-  if (L.rap) return rap1_apply(L, d_x, d_y, st, nullptr, nullptr);
-  return L.index_free ? hexop_apply(L.H, d_x, d_y, st) : spmv_launch(L.P, d_x, d_y, false, st);
+  return level_apply(mg, level, d_x, d_y, (cudaStream_t)stream, nullptr, nullptr);
 }
 
 int pcgb_mg_level_dinv(pcgb_mg_t mg, int level, double *d_out, void *stream) {
   PCGB_TRY(require_device());
   if (!mg || !d_out) return fail(PCGB_ERR_ARG, "pcgb_mg_level_dinv: null argument");
-  if (level < 0 || level + 1 >= (int)mg->lv.size() || level == mg->la)
+  if (!mg_smoothed(mg, level))
     return fail(PCGB_ERR_ARG, "pcgb_mg_level_dinv: level %d is not smoothed (levels 0 .. %d, not the gathered one)", level,
                 (int)mg->lv.size() - 2);
   const MgLevel &L = mg->lv[(size_t)level];
@@ -2256,24 +2278,21 @@ int pcgb_mg_setup_info(pcgb_mg_t mg, double *galerkin_ms, int64_t *element_matri
 }
 
 namespace {
-// pcgb_mg_create_ranks, (index_free) pcgb_mg_create_ranks_index_free and (d_ck_fine, kel_gather) pcgb_mg_create_ranks_field
+// pcgb_mg_create_ranks, (coarse Hex) pcgb_mg_create_ranks_index_free and (field: d_ck_fine and kel_gather, which must be
+// given) pcgb_mg_create_ranks_field
 int mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos, pcgb_halo_t gather,
                     const double *const *d_own, const double *ke_host, double E, double h, const double *d_minv_fine, int degree,
-                    double lo, pcgb_mg_t *out, bool index_free, const char *who, const double *d_ck_fine = nullptr,
+                    double lo, pcgb_mg_t *out, MgOp coarse, const char *who, bool field = false, const double *d_ck_fine = nullptr,
                     pcgb_halo_t kel_gather = nullptr) {
   PCGB_TRY(require_device());
-  if (!s || !box || !level_halos || !gather || !d_own || !ke_host || !d_minv_fine || !out)
+  if (!s || !box || !level_halos || !gather || !d_own || !ke_host || !d_minv_fine || !out || (field && (!d_ck_fine || !kel_gather)))
     return fail(PCGB_ERR_ARG, "%s: null argument", who);
-  if ((d_ck_fine == nullptr) != (kel_gather == nullptr)) return fail(PCGB_ERR_ARG, "%s: null argument", who);
   if (!s->comm || s->comm->nranks < 2) return fail(PCGB_ERR_ARG, "%s: the solver has no communicator of 2 or more ranks", who);
-  if (degree < 1 || !(lo > 0.0 && lo < 1.1) || !(E > 0.0) || !(h > 0.0))
-    return fail(PCGB_ERR_ARG, "%s: degree >= 1, 0 < lo < 1.1, E > 0 and h > 0 required", who);
+  PCGB_TRY(mg_check_ranges(degree, lo, E, h, who));
   for (int a = 0; a < 3; ++a)
     if (box->ne[a] <= 0 || box->e0[a] < 0 || box->e0[a] + box->ne[a] > box->ng[a])
       return fail(PCGB_ERR_ARG, "%s: the box does not lie in the mesh", who);
-  if (3 * hex_geom(box).nfree_nodes != s->n)
-    return fail(PCGB_ERR_ARG, "%s: the solver's operator has %lld rows, the box %lld", who, (long long)s->n,
-                (long long)(3 * hex_geom(box).nfree_nodes));
+  PCGB_TRY(mg_check_rows(s, box, who));
   if (n_ranked < 1) return fail(PCGB_ERR_ARG, "%s: the fine level does not coarsen (n_ranked >= 1 required)", who);
   // ranked levels 0 .. la: the rank's box halved la times, and the global box around it
   const int la = n_ranked;
@@ -2306,10 +2325,8 @@ int mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, cons
   for (int l = 0; l <= la; ++l)
     if (!d_own[l]) return fail(PCGB_ERR_ARG, "%s: null ownership weights of level %d", who, l);
   mg_whole_box_levels(geo);
-  if (3 * geo.back().nfree_nodes > kMgMaxCoarse)
-    return fail(PCGB_ERR_ARG, "%s: the coarsest level has %lld dofs (at most %d)", who, (long long)(3 * geo.back().nfree_nodes), kMgMaxCoarse);
-  if ((size_t)la + 1 + geo.size() > PCGB_MG_MAX_LEVELS) return fail(PCGB_ERR_ARG, "%s: more than %d levels", who, PCGB_MG_MAX_LEVELS);
-  if (d_ck_fine) {
+  PCGB_TRY(mg_check_levels(geo, (size_t)la + 1 + geo.size(), who));
+  if (field) {
     const int64_t nge = (int64_t)geo[0].nx * geo[0].ny * geo[0].nz;
     if (nge > kMgMaxGatheredElements)
       return fail(PCGB_ERR_ARG, "%s: the gathered level has %lld elements (at most %lld)", who, (long long)nge,
@@ -2318,15 +2335,10 @@ int mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, cons
         kel_gather->m != (int64_t)(s->comm->nranks - 1) * 576 * nge)
       return fail(PCGB_ERR_ARG, "%s: the element plan must list all %lld entries of the gathered level's element matrices for "
                   "every other rank", who, (long long)(576 * nge));
-    // the check runs on the legacy stream, which does not wait for non-blocking streams: finish whatever work of the caller
-    // may still be writing d_ck_fine first
-    PCGB_CUDA(cudaDeviceSynchronize());
-    int bad = 0;
-    PCGB_TRY(field_bad((int64_t)box->ne[0] * box->ne[1] * box->ne[2], d_ck_fine, 0, who, &bad));
-    if (bad) return fail(PCGB_ERR_ARG, "%s: every Ck of the field must be finite and positive", who);
+    PCGB_TRY(mg_check_field((int64_t)box->ne[0] * box->ne[1] * box->ne[2], d_ck_fine, who));
   }
   pcgb_mg_t mg = new pcgb_mg_s();
-  mg->s = s; mg->degree = degree; mg->lo = lo; mg->la = la; mg->gather = gather; mg->index_free = index_free;
+  mg->s = s; mg->degree = degree; mg->lo = lo; mg->la = la; mg->gather = gather;
   mg->ck_fine = d_ck_fine; mg->kel_gather = kel_gather;
   mg->lv.resize((size_t)la + 1 + geo.size());
   for (int l = 0; l <= la; ++l) {
@@ -2341,39 +2353,29 @@ int mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, cons
     MgLevel &L = mg->lv[(size_t)la + 1 + k];
     L.g = geo[k]; L.glev = la + (int)k; L.place = MgPlace{geo[k], 0, 0, 0};
   }
-  const int rc = mg_build(mg, ke_host, E, h, d_minv_fine, d_own);
-  mg->ck_fine = nullptr;      // the caller's array and plan: not used after create
-  mg->kel_gather = nullptr;
-  if (rc != PCGB_OK) { pcgb_mg_destroy(mg); return rc; }
-  s->mgs.push_back(mg);
-  *out = mg;
-  return PCGB_OK;
+  return mg_finish(mg, coarse, ke_host, E, h, d_minv_fine, d_own, out);
 }
 }  // namespace
 
 int pcgb_mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos, pcgb_halo_t gather,
                          const double *const *d_own, const double *ke_host, double E, double h, const double *d_minv_fine,
                          int degree, double lo, pcgb_mg_t *out) {
-  return mg_create_ranks(s, box, n_ranked, level_halos, gather, d_own, ke_host, E, h, d_minv_fine, degree, lo, out, false,
+  return mg_create_ranks(s, box, n_ranked, level_halos, gather, d_own, ke_host, E, h, d_minv_fine, degree, lo, out, MgOp::Csr,
                          "pcgb_mg_create_ranks");
 }
 
 int pcgb_mg_create_ranks_index_free(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos,
                                     pcgb_halo_t gather, const double *const *d_own, const double *ke_host, double E, double h,
                                     const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
-  return mg_create_ranks(s, box, n_ranked, level_halos, gather, d_own, ke_host, E, h, d_minv_fine, degree, lo, out, true,
+  return mg_create_ranks(s, box, n_ranked, level_halos, gather, d_own, ke_host, E, h, d_minv_fine, degree, lo, out, MgOp::Hex,
                          "pcgb_mg_create_ranks_index_free");
 }
 
 int pcgb_mg_create_ranks_field(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos,
                                pcgb_halo_t gather, pcgb_halo_t kel_gather, const double *const *d_own, const double *ke_host,
                                const double *d_ck_fine, const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
-  if (!d_ck_fine || !kel_gather) {
-    PCGB_TRY(require_device());
-    return fail(PCGB_ERR_ARG, "pcgb_mg_create_ranks_field: null argument");
-  }
-  return mg_create_ranks(s, box, n_ranked, level_halos, gather, d_own, ke_host, 1.0, 1.0, d_minv_fine, degree, lo, out, false,
-                         "pcgb_mg_create_ranks_field", d_ck_fine, kel_gather);
+  return mg_create_ranks(s, box, n_ranked, level_halos, gather, d_own, ke_host, 1.0, 1.0, d_minv_fine, degree, lo, out, MgOp::Csr,
+                         "pcgb_mg_create_ranks_field", true, d_ck_fine, kel_gather);
 }
 
 int pcgb_mg_apply(pcgb_mg_t mg, const double *d_r, double *d_z, void *stream) {
@@ -2400,7 +2402,7 @@ int pcgb_mg_info(pcgb_mg_t mg, int32_t *nlevels, int64_t *n_level, double *lambd
 
 int pcgb_mg_restrict(pcgb_mg_t mg, int level, const double *d_fine, double *d_coarse, void *stream) {
   PCGB_TRY(require_device());
-  if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || level == mg->la || !d_fine || !d_coarse)
+  if (!mg || !mg_smoothed(mg, level) || !d_fine || !d_coarse)
     return fail(PCGB_ERR_ARG, "pcgb_mg_restrict: bad argument");
   int nl = 0;
   return mg_restrict(mg, level, d_fine, d_coarse, (cudaStream_t)stream, &nl, nullptr);
@@ -2408,7 +2410,7 @@ int pcgb_mg_restrict(pcgb_mg_t mg, int level, const double *d_fine, double *d_co
 
 int pcgb_mg_prolong_add(pcgb_mg_t mg, int level, const double *d_coarse, double *d_fine, void *stream) {
   PCGB_TRY(require_device());
-  if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || level == mg->la || !d_fine || !d_coarse)
+  if (!mg || !mg_smoothed(mg, level) || !d_fine || !d_coarse)
     return fail(PCGB_ERR_ARG, "pcgb_mg_prolong_add: bad argument");
   int nl = 0;
   return mg_prolong_add(mg, level, d_coarse, d_fine, (cudaStream_t)stream, &nl, nullptr);
@@ -2416,7 +2418,7 @@ int pcgb_mg_prolong_add(pcgb_mg_t mg, int level, const double *d_coarse, double 
 
 int pcgb_mg_smooth(pcgb_mg_t mg, int level, const double *d_b, double *d_x, void *stream) {
   PCGB_TRY(require_device());
-  if (!mg || level < 0 || level + 1 >= (int)mg->lv.size() || level == mg->la || !d_b || !d_x)
+  if (!mg || !mg_smoothed(mg, level) || !d_b || !d_x)
     return fail(PCGB_ERR_ARG, "pcgb_mg_smooth: bad argument");
   int nl = 0;
   return mg_smooth(mg, level, d_b, d_x, false, false, (cudaStream_t)stream, &nl, nullptr);

@@ -74,28 +74,30 @@ def any_levels(ne, max_levels: int = _lib.MG_MAX_LEVELS) -> list:
     return out
 
 
+def _whole_box_levels(ne):
+    """The default coarsening's levels of the whole box ne and their free dofs, refused (ValueError) as pcgb_mg_create
+    refuses the box."""
+    lv = _whole_levels(ne)
+    if len(lv) < 2:
+        raise ValueError(f"HexMultigrid: the box {tuple(ne)} does not coarsen (every ne must be even and >= 4)")
+    n = [3 * v[0] * (v[1] + 1) * (v[2] + 1) for v in lv]
+    if n[-1] > MAX_COARSE:
+        raise ValueError(f"HexMultigrid: the coarsest level has {n[-1]} dofs (at most {MAX_COARSE})")
+    return lv, n
+
+
 def index_free_bytes(ne) -> int:
     """Device bytes pcgb_mg_info reports for the one-rank index-free hierarchy of the whole box `ne` (default coarsening):
     8 (5 n_0 + 6 sum n_l over the smoothed coarse levels + 2 n_c + n_c^2) - the fine level's z, D^-1 and three smoother
     vectors, each coarse level's b, x, D^-1 and three smoother vectors, the coarsest b, x and dense factor.  The few
     fixed-size reduction buffers are not counted.  Raises ValueError where pcgb_mg_create_index_free refuses the box."""
-    lv = _whole_levels(ne)
-    if len(lv) < 2:
-        raise ValueError(f"HexMultigrid: the box {tuple(ne)} does not coarsen (every ne must be even and >= 4)")
-    n = [3 * v[0] * (v[1] + 1) * (v[2] + 1) for v in lv]
-    if n[-1] > MAX_COARSE:
-        raise ValueError(f"HexMultigrid: the coarsest level has {n[-1]} dofs (at most {MAX_COARSE})")
+    _, n = _whole_box_levels(ne)
     return 8 * (5 * n[0] + 6 * sum(n[1:-1]) + 2 * n[-1] + n[-1] ** 2)
 
 
 def _rap_levels(ne):
     """The default coarsening's levels and free dofs, refused (ValueError) as pcgb_mg_create_field_rap refuses the box."""
-    lv = _whole_levels(ne)
-    if len(lv) < 2:
-        raise ValueError(f"HexMultigrid: the box {tuple(ne)} does not coarsen (every ne must be even and >= 4)")
-    n = [3 * v[0] * (v[1] + 1) * (v[2] + 1) for v in lv]
-    if n[-1] > MAX_COARSE:
-        raise ValueError(f"HexMultigrid: the coarsest level has {n[-1]} dofs (at most {MAX_COARSE})")
+    lv, n = _whole_box_levels(ne)
     if len(lv) < 3:
         raise ValueError(f"HexMultigrid: coarse='rap' needs at least 3 levels, the box {tuple(ne)} has {len(lv)} "
                          "(level 1 would be the coarsest)")
@@ -113,12 +115,11 @@ def rap_bytes(ne) -> int:
     plus levels 2 .. L-2 as CSR, 12 nnz + 4 (n + 1) bytes each (8 (n + 1) from 2^31 - 1 non-zeros on, int64 row offsets).
     Raises ValueError where pcgb_mg_create_field_rap refuses the box."""
     lv, n = _rap_levels(ne)
-    vectors = 8 * (5 * n[0] + 6 * sum(n[1:-1]) + 2 * n[-1] + n[-1] ** 2)
     csr = 0
     for l in range(2, len(lv) - 1):
         nnz = hex_csr_nnz(lv[l])
         csr += 12 * nnz + (4 if nnz < 2**31 - 1 else 8) * (n[l] + 1)
-    return vectors + csr
+    return index_free_bytes(ne) + csr
 
 
 def rap_setup_peak_bytes(ne) -> int:
@@ -249,33 +250,8 @@ class HexMultigrid:
                 raise ValueError("HexMultigrid: coarse='rap' is supported on one rank only")
             rap_bytes(block.ne)
         self.coarse = coarse
-        index_free = coarse == "index_free"
-        if coarsening == "any":
-            if ranked:
-                raise ValueError("HexMultigrid: coarsening='any' is supported on one rank only")
-            ck = None if E_field is None else field_ck(E_field, block, self.device)
-            minv = op.jacobi() if minv is None else minv.to(self.device, torch.float64).contiguous()
-            ke = np.ascontiguousarray(hex_element_stiffness(1.0, block.nu))
-            box = block.cbox()
-            with torch.cuda.device(self.device):
-                torch.cuda.synchronize(self.device)
-                _lib.check(_lib.load().pcgb_mg_create_any(op._solver, ctypes.byref(box), ke.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
-                                                          _lib.ptr(ck), float(block.E), float(block.h), _lib.ptr(minv), self.degree,
-                                                          self.lo, ctypes.byref(self._h)), "pcgb_mg_create_any")
-            return
-        if E_field is not None and not ranked:
-            ck = field_ck(E_field, block, self.device)
-            minv = op.jacobi() if minv is None else minv.to(self.device, torch.float64).contiguous()
-            ke = np.ascontiguousarray(hex_element_stiffness(1.0, block.nu))
-            box = block.cbox()
-            name = "pcgb_mg_create_field_rap" if coarse == "rap" else "pcgb_mg_create_field"
-            with torch.cuda.device(self.device):
-                torch.cuda.synchronize(self.device)
-                _lib.check(getattr(_lib.load(), name)(op._solver, ctypes.byref(box), ke.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
-                                                      _lib.ptr(ck), _lib.ptr(minv), self.degree, self.lo, ctypes.byref(self._h)), name)
-            if coarse == "rap":
-                self._ck = ck          # read by every V-cycle: it lives as long as the handle
-            return
+        if coarsening == "any" and ranked:
+            raise ValueError("HexMultigrid: coarsening='any' is supported on one rank only")
         if ranked:
             if blocks is None or len(blocks) != comm.nranks:
                 raise ValueError("HexMultigrid: a multi-rank operator needs `blocks`, one box per rank")
@@ -287,16 +263,27 @@ class HexMultigrid:
             if E_field is not None:
                 check_global_field(E_field, block.ng, self.device)
                 nge = gathered_elements(self.levels)
+        # across ranks the rank's slice of the global field
+        ck = None if E_field is None else field_ck(block_field(E_field, block) if ranked else E_field, block, self.device)
         minv = op.jacobi() if minv is None else minv.to(self.device, torch.float64).contiguous()
         ke = np.ascontiguousarray(hex_element_stiffness(1.0, block.nu))
         kep = ke.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
-        box = block.cbox()
+        box = ctypes.byref(block.cbox())
+        uniform = (float(block.E), float(block.h))
+        tail = (_lib.ptr(minv), self.degree, self.lo, ctypes.byref(self._h))
+        # The library synchronises the device before it reads minv, ck or the ownership weights, whatever stream wrote them.
         lib = _lib.load()
         with torch.cuda.device(self.device):
             if not ranked:
-                name = "pcgb_mg_create_index_free" if index_free else "pcgb_mg_create"
-                _lib.check(getattr(lib, name)(op._solver, ctypes.byref(box), kep, float(block.E), float(block.h), _lib.ptr(minv),
-                                              self.degree, self.lo, ctypes.byref(self._h)), name)
+                if coarsening == "any":
+                    name, args = "pcgb_mg_create_any", (_lib.ptr(ck), *uniform)
+                elif ck is not None:
+                    name, args = ("pcgb_mg_create_field_rap" if coarse == "rap" else "pcgb_mg_create_field"), (_lib.ptr(ck),)
+                else:
+                    name, args = ("pcgb_mg_create_index_free" if coarse == "index_free" else "pcgb_mg_create"), uniform
+                _lib.check(getattr(lib, name)(op._solver, box, kep, *args, *tail), name)
+                if coarse == "rap":
+                    self._ck = ck          # read by every V-cycle: it lives as long as the handle
                 return
             from .solver import make_halo
             la = len(self.levels) - 1
@@ -314,23 +301,19 @@ class HexMultigrid:
             self._halos.append(self._gather)
             halos = (ctypes.c_void_p * la)(*[h.value for h in self._halos[:la]])
             owns = (ctypes.c_void_p * (la + 1))(*[t.data_ptr() for t in own])
-            if E_field is not None:
-                # the rank's slice of the global field, and a plan over the gathered level's element matrices used by the
-                # set-up only
-                ck = field_ck(block_field(E_field, block), block, self.device)
+            kg = None
+            if ck is not None:
+                # a plan over the gathered level's element matrices, used by the set-up only
                 kg = make_halo(comm, others, [np.arange(576 * nge, dtype=np.int64)] * len(others), 576 * nge)
-                try:
-                    torch.cuda.synchronize(self.device)
-                    _lib.check(lib.pcgb_mg_create_ranks_field(op._solver, ctypes.byref(box), la, halos, self._gather, kg, owns, kep,
-                                                              _lib.ptr(ck), _lib.ptr(minv), self.degree, self.lo, ctypes.byref(self._h)),
-                               "pcgb_mg_create_ranks_field")
-                finally:
+                name, args = "pcgb_mg_create_ranks_field", (kg, owns, kep, _lib.ptr(ck))
+            else:
+                name = "pcgb_mg_create_ranks_index_free" if coarse == "index_free" else "pcgb_mg_create_ranks"
+                args = (owns, kep, *uniform)
+            try:
+                _lib.check(getattr(lib, name)(op._solver, box, la, halos, self._gather, *args, *tail), name)
+            finally:
+                if kg is not None:
                     lib.pcgb_halo_destroy(kg)
-                return
-            torch.cuda.synchronize(self.device)
-            name = "pcgb_mg_create_ranks_index_free" if index_free else "pcgb_mg_create_ranks"
-            _lib.check(getattr(lib, name)(op._solver, ctypes.byref(box), la, halos, self._gather, owns, kep, float(block.E),
-                                          float(block.h), _lib.ptr(minv), self.degree, self.lo, ctypes.byref(self._h)), name)
 
     @property
     def handle(self):
@@ -339,11 +322,15 @@ class HexMultigrid:
     def _vec(self, n):
         return torch.empty(n, dtype=torch.float64, device=self.device)
 
+    def _call(self, name: str, *args):
+        """The library's `name`(handle, *args, stream) on the current stream of the handle's device."""
+        with torch.cuda.device(self.device):
+            _lib.check(getattr(_lib.load(), name)(self._h, *args, _lib.stream_ptr()), name)
+
     def apply(self, r: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
         """z = M r (one V-cycle; collective across ranks)."""
         z = out if out is not None else self._vec(self.n)
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().pcgb_mg_apply(self._h, _lib.ptr(r), _lib.ptr(z), _lib.stream_ptr()), "pcgb_mg_apply")
+        self._call("pcgb_mg_apply", _lib.ptr(r), _lib.ptr(z))
         return z
 
     def info(self) -> dict:
@@ -387,69 +374,58 @@ class HexMultigrid:
     # ---- the V-cycle's parts (tests; collective across ranks)
     def level_matrix(self, level: int):
         """The CSR of smoothed coarse level `level` (1 .. levels - 2) as (rowptr int64, col int32, val float64) device tensors."""
-        lib = _lib.load()
         nnz = ctypes.c_int64()
-        _lib.check(lib.pcgb_mg_level_csr(self._h, level, None, None, None, ctypes.byref(nnz), None), "pcgb_mg_level_csr")
+        self._call("pcgb_mg_level_csr", level, None, None, None, ctypes.byref(nnz))
         n = self.info()["n"][level]
         rowptr = torch.empty(n + 1, dtype=torch.int64, device=self.device)
         col = torch.empty(nnz.value, dtype=torch.int32, device=self.device)
         val = torch.empty(nnz.value, dtype=torch.float64, device=self.device)
-        with torch.cuda.device(self.device):
-            _lib.check(lib.pcgb_mg_level_csr(self._h, level, _lib.ptr(rowptr), _lib.ptr(col), _lib.ptr(val), ctypes.byref(nnz),
-                                             _lib.stream_ptr()), "pcgb_mg_level_csr")
+        self._call("pcgb_mg_level_csr", level, _lib.ptr(rowptr), _lib.ptr(col), _lib.ptr(val), ctypes.byref(nnz))
         return rowptr, col, val
 
     def level_dinv(self, level: int) -> torch.Tensor:
         """D^-1 of smoothed level `level` (0 .. levels - 2, not the gathered level) as a device tensor, any hierarchy kind."""
         d = self._vec(self.info()["n"][level])
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().pcgb_mg_level_dinv(self._h, level, _lib.ptr(d), _lib.stream_ptr()), "pcgb_mg_level_dinv")
+        self._call("pcgb_mg_level_dinv", level, _lib.ptr(d))
         return d
 
     def level_apply(self, level: int, x: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
         """y = A_l x on smoothed coarse level `level` (1 .. levels - 2, not the gathered level), either coarse kind: the
         local product, without the level's exchange-add across ranks (x and out must not overlap)."""
         y = out if out is not None else self._vec(self.info()["n"][level])
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().pcgb_mg_level_apply(self._h, level, _lib.ptr(x), _lib.ptr(y), _lib.stream_ptr()), "pcgb_mg_level_apply")
+        self._call("pcgb_mg_level_apply", level, _lib.ptr(x), _lib.ptr(y))
         return y
 
     def restrict(self, level: int, rf: torch.Tensor) -> torch.Tensor:
         rc = self._vec(self.info()["n"][level + 1])
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().pcgb_mg_restrict(self._h, level, _lib.ptr(rf), _lib.ptr(rc), _lib.stream_ptr()), "pcgb_mg_restrict")
+        self._call("pcgb_mg_restrict", level, _lib.ptr(rf), _lib.ptr(rc))
         return rc
 
     def prolong_add(self, level: int, ec: torch.Tensor, xf: torch.Tensor) -> torch.Tensor:
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().pcgb_mg_prolong_add(self._h, level, _lib.ptr(ec), _lib.ptr(xf), _lib.stream_ptr()), "pcgb_mg_prolong_add")
+        self._call("pcgb_mg_prolong_add", level, _lib.ptr(ec), _lib.ptr(xf))
         return xf
 
     def smooth(self, level: int, b: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
         """x += S (b - A x) on `level`, in place."""
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().pcgb_mg_smooth(self._h, level, _lib.ptr(b), _lib.ptr(x), _lib.stream_ptr()), "pcgb_mg_smooth")
+        self._call("pcgb_mg_smooth", level, _lib.ptr(b), _lib.ptr(x))
         return x
 
     def coarse_solve(self, r: torch.Tensor) -> torch.Tensor:
         z = self._vec(r.numel())
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().pcgb_mg_coarse_solve(self._h, _lib.ptr(r), _lib.ptr(z), _lib.stream_ptr()), "pcgb_mg_coarse_solve")
+        self._call("pcgb_mg_coarse_solve", _lib.ptr(r), _lib.ptr(z))
         return z
 
     def gather(self, v: torch.Tensor) -> torch.Tensor:
         """The gathered level's ranked vector -> its global box, the same on every rank."""
         out = self._vec(self.info()["n_gathered"])
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().pcgb_mg_gather(self._h, _lib.ptr(v), _lib.ptr(out), _lib.stream_ptr()), "pcgb_mg_gather")
+        self._call("pcgb_mg_gather", _lib.ptr(v), _lib.ptr(out))
         return out
 
     def scatter(self, g: torch.Tensor) -> torch.Tensor:
         """This rank's entries of a global vector of the gathered level."""
         info = self.info()
         out = self._vec(info["n"][info["gather_level"]])
-        with torch.cuda.device(self.device):
-            _lib.check(_lib.load().pcgb_mg_scatter(self._h, _lib.ptr(g), _lib.ptr(out), _lib.stream_ptr()), "pcgb_mg_scatter")
+        self._call("pcgb_mg_scatter", _lib.ptr(g), _lib.ptr(out))
         return out
 
     def __del__(self):
