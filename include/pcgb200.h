@@ -497,6 +497,20 @@ int pcgb_mg_create_ranks_index_free(pcgb_solver_t s, const pcgb_hex_box *box, in
  * level-2 and level-3 matrices) and the device time of the Galerkin kernels. */
 int pcgb_mg_create_field_rap(pcgb_solver_t s, const pcgb_hex_box *box, const double *ke_host, const double *d_ck_fine,
                              const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out);
+/* pcgb_mg_create_ranks_field with the matrix-free level 1 of pcgb_mg_create_field_rap, for partitioned voxel models whose
+ * rank boxes are too large for the level-1 Galerkin matrices.  Arguments, collective contract and refusals are those of
+ * pcgb_mg_create_ranks_field, plus PCGB_ERR_ARG before anything is allocated for n_ranked < 2 (level 1 would be the
+ * gathered level, which is not smoothed).  Ranked level 1 applies y_1 = P^T A_0 P x_1 by k_mg_rap1 on the rank's level-1
+ * box from the rank's d_ck_fine, restricting without ownership weights: fine elements outside the box contribute 0.0,
+ * and every fine node of a box with even e0 interpolates from coarse nodes of the box only, so the level's exchange-add
+ * completes the assembled product.  Level 1's diagonal is summed from slabs of the rank's level-1 element matrices as in
+ * pcgb_mg_create_field_rap, then exchange-added, so its D^-1 is pcgb_mg_create_ranks_field's bit for bit; so are every
+ * level >= 2 (ranked CSR, gathered element matrices, replicated levels) and every lambda from level 2 on.  d_ck_fine is
+ * read by every V-cycle: it must outlive the handle.  pcgb_mg_level_csr refuses level 1; pcgb_mg_setup_info reports the
+ * rank's peak of element matrices, the gathered level's included. */
+int pcgb_mg_create_ranks_field_rap(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos,
+                                   pcgb_halo_t gather, pcgb_halo_t kel_gather, const double *const *d_own, const double *ke_host,
+                                   const double *d_ck_fine, const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out);
 /* For tests: the inverse diagonal of smoothed level `level` (0 .. nlevels - 2, not the gathered level of a multi-rank
  * handle; level 0: the copy of d_minv_fine) of any handle into d_out (n_l doubles), ordered on `stream`.  PCGB_ERR_ARG
  * for any other level. */

@@ -129,6 +129,9 @@ SIGNATURES = {
                                            POINTER(c_double), c_void_p, c_void_p, c_int, c_double, POINTER(c_void_p)]),
     "pcgb_mg_create_field_rap": (c_int, [c_void_p, POINTER(HexBox), POINTER(c_double), c_void_p, c_void_p, c_int, c_double,
                                          POINTER(c_void_p)]),
+    "pcgb_mg_create_ranks_field_rap": (c_int, [c_void_p, POINTER(HexBox), c_int, POINTER(c_void_p), c_void_p, c_void_p,
+                                               POINTER(c_void_p), POINTER(c_double), c_void_p, c_void_p, c_int, c_double,
+                                               POINTER(c_void_p)]),
     "pcgb_mg_level_dinv": (c_int, [c_void_p, c_int, c_void_p, c_void_p]),
     "pcgb_mg_level_apply": (c_int, [c_void_p, c_int, c_void_p, c_void_p, c_void_p]),
     "pcgb_mg_setup_info": (c_int, [c_void_p, POINTER(c_double), POINTER(c_int64)]),

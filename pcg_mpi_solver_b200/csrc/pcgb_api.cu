@@ -1791,7 +1791,8 @@ constexpr int64_t kMgRapSlabBytes = int64_t(1) << 30;
 // level 1's.  In ascending z, a slab of level-1 element layers (an even number, at most kMgRapSlabBytes, at least 2) is built
 // from the fine field with k_mg_galerkin, its diagonal entries are added into level 1's diagonal (L1.r, zeroed), and each
 // finished pair of layers gives one layer of level-2 matrices, k_mg_galerkin from the slab.  Every level-1 matrix is the
-// field hierarchy's bit for bit, so are the level-2 matrices and the diagonal.
+// field hierarchy's bit for bit, so are the level-2 matrices and the diagonal.  Across ranks the boxes are the rank's and the
+// field its slice: L1.r is the rank's part of the diagonal, which mg_build exchange-adds like every ranked level's.
 int mg_rap_level1(pcgb_mg_t mg, const double *ke_host) {
   MgLevel &L1 = mg->lv[1];
   const HexGeom &G0 = mg->lv[0].g, &G1 = L1.g, &G2 = mg->lv[2].g;
@@ -2000,7 +2001,8 @@ int mg_build(pcgb_mg_t mg, MgOp coarse, const double *ke_host, double E, double 
       PCGB_CUDA(cudaMemcpy(L.own, own[l], (size_t)L.n * sizeof(double), cudaMemcpyDeviceToDevice));
       if (l == mg->la) {   // gathered: no operator, no smoother
         if (mg->ck_fine) {   // field: the rank's Galerkin element matrices, gathered into level la + 1's global box
-          PCGB_TRY(mg_galerkin_level(mg, l, ke_host));
+          // (rap with la = 2: level 2's matrices are already in mg->kel, from mg_rap_level1)
+          if (!(coarse == MgOp::Rap && l <= 2)) PCGB_TRY(mg_galerkin_level(mg, l, ke_host));
           PCGB_TRY(mg_gather_elements(mg));
         }
         continue;
@@ -2279,7 +2281,8 @@ int pcgb_mg_setup_info(pcgb_mg_t mg, double *galerkin_ms, int64_t *element_matri
 
 namespace {
 // pcgb_mg_create_ranks, (coarse Hex) pcgb_mg_create_ranks_index_free and (field: d_ck_fine and kel_gather, which must be
-// given) pcgb_mg_create_ranks_field
+// given) pcgb_mg_create_ranks_field (coarse Rap: pcgb_mg_create_ranks_field_rap, level 1 applied by k_mg_rap1 on the rank's
+// level-1 box from the rank's Ck slice, its local product completed by the level's exchange-add like every ranked level's)
 int mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos, pcgb_halo_t gather,
                     const double *const *d_own, const double *ke_host, double E, double h, const double *d_minv_fine, int degree,
                     double lo, pcgb_mg_t *out, MgOp coarse, const char *who, bool field = false, const double *d_ck_fine = nullptr,
@@ -2294,6 +2297,8 @@ int mg_create_ranks(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, cons
       return fail(PCGB_ERR_ARG, "%s: the box does not lie in the mesh", who);
   PCGB_TRY(mg_check_rows(s, box, who));
   if (n_ranked < 1) return fail(PCGB_ERR_ARG, "%s: the fine level does not coarsen (n_ranked >= 1 required)", who);
+  if (coarse == MgOp::Rap && n_ranked < 2)
+    return fail(PCGB_ERR_ARG, "%s: n_ranked is %d (at least 2, so that level 1 is smoothed, not gathered)", who, n_ranked);
   // ranked levels 0 .. la: the rank's box halved la times, and the global box around it
   const int la = n_ranked;
   std::vector<pcgb_hex_box> rb{*box};
@@ -2376,6 +2381,13 @@ int pcgb_mg_create_ranks_field(pcgb_solver_t s, const pcgb_hex_box *box, int n_r
                                const double *d_ck_fine, const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
   return mg_create_ranks(s, box, n_ranked, level_halos, gather, d_own, ke_host, 1.0, 1.0, d_minv_fine, degree, lo, out, MgOp::Csr,
                          "pcgb_mg_create_ranks_field", true, d_ck_fine, kel_gather);
+}
+
+int pcgb_mg_create_ranks_field_rap(pcgb_solver_t s, const pcgb_hex_box *box, int n_ranked, const pcgb_halo_t *level_halos,
+                                   pcgb_halo_t gather, pcgb_halo_t kel_gather, const double *const *d_own, const double *ke_host,
+                                   const double *d_ck_fine, const double *d_minv_fine, int degree, double lo, pcgb_mg_t *out) {
+  return mg_create_ranks(s, box, n_ranked, level_halos, gather, d_own, ke_host, 1.0, 1.0, d_minv_fine, degree, lo, out, MgOp::Rap,
+                         "pcgb_mg_create_ranks_field_rap", true, d_ck_fine, kel_gather);
 }
 
 int pcgb_mg_apply(pcgb_mg_t mg, const double *d_r, double *d_z, void *stream) {

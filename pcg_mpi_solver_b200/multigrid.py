@@ -30,7 +30,9 @@ factor (`index_free_bytes`), which is what lets MG-PCG run a 512^3 box on one 80
 (pcgb_mg_create_field_rap): level 1 applies P^T A_0 P from the fine Ck field in one kernel (csrc/gmg_rap.cuh) and levels >= 2
 are the field hierarchy's CSR levels bit for bit, built from slabs of level-1 element matrices that are never held whole
 (`rap_bytes`, `rap_setup_peak_bytes`).  It preconditions a 512^3 voxel model on one 80 GB GPU, where the CSR field
-hierarchy's level 1 alone would take about 49 GB.
+hierarchy's level 1 alone would take about 49 GB.  Across ranks (`blocks` and the global E_field,
+pcgb_mg_create_ranks_field_rap) it is the multi-rank field hierarchy with the same matrix-free level 1 on every rank's
+level-1 box, from the rank's slice of the field (`rap_rank_bytes`); the rank boxes must halve at least twice.
 """
 from __future__ import annotations
 
@@ -104,10 +106,17 @@ def _rap_levels(ne):
     return lv, n
 
 
-def hex_csr_nnz(ne) -> int:
+def hex_csr_nnz(ne, x_lo: int = 1) -> int:
     """Non-zeros of the clamped stiffness matrix of the whole box ne (x = 0 nodes dropped): 9 times the free neighbour pairs,
-    which factor per axis into 3 m - 2 for an axis of m free nodes (nx on x, ny + 1 and nz + 1 on y and z)."""
-    return 9 * (3 * ne[0] - 2) * (3 * (ne[1] + 1) - 2) * (3 * (ne[2] + 1) - 2)
+    which factor per axis into 3 m - 2 for an axis of m free nodes (nx on x, ny + 1 and nz + 1 on y and z).  x_lo = 0: the
+    sub-assembled matrix of a rank's box away from x = 0 (HexBlock.x_lo), nx + 1 free nodes on x."""
+    return 9 * (3 * (ne[0] + 1 - x_lo) - 2) * (3 * (ne[1] + 1) - 2) * (3 * (ne[2] + 1) - 2)
+
+
+def _csr_bytes(ne, n, x_lo: int = 1) -> int:
+    """Device bytes of a coarse level's CSR: 12 nnz + 4 (n + 1) (8 (n + 1) from 2^31 - 1 non-zeros on, int64 row offsets)."""
+    nnz = hex_csr_nnz(ne, x_lo)
+    return 12 * nnz + (4 if nnz < 2**31 - 1 else 8) * (n + 1)
 
 
 def rap_bytes(ne) -> int:
@@ -115,11 +124,7 @@ def rap_bytes(ne) -> int:
     plus levels 2 .. L-2 as CSR, 12 nnz + 4 (n + 1) bytes each (8 (n + 1) from 2^31 - 1 non-zeros on, int64 row offsets).
     Raises ValueError where pcgb_mg_create_field_rap refuses the box."""
     lv, n = _rap_levels(ne)
-    csr = 0
-    for l in range(2, len(lv) - 1):
-        nnz = hex_csr_nnz(lv[l])
-        csr += 12 * nnz + (4 if nnz < 2**31 - 1 else 8) * (n[l] + 1)
-    return index_free_bytes(ne) + csr
+    return index_free_bytes(ne) + sum(_csr_bytes(lv[l], n[l]) for l in range(2, len(lv) - 1))
 
 
 def rap_setup_peak_bytes(ne) -> int:
@@ -157,6 +162,27 @@ def check_global_field(E_field, ng, device=None):
     if not ok:
         raise ValueError("E_field: every value must be finite and positive")
     return E_field
+
+
+def rap_rank_bytes(levels, rank: int) -> int:
+    """Device bytes pcgb_mg_info reports on rank `rank` of the multi-rank rap hierarchy of `rank_levels`' list `levels` (la =
+    len(levels) - 1 >= 2), in 8-byte entries unless stated: the vectors (the fine level's z, D^-1 and three smoother vectors;
+    each ranked smoothed level's b, x, D^-1 and three smoother vectors, level 1 included; the same six per smoothed level of
+    the replicated hierarchy of the gathered global box; the coarsest b, x and dense factor), the ownership weights of every
+    ranked level 0 .. la, b and x of the gathered level la, and the CSR of ranked levels 2 .. la-1 (the rank's sub-assembled
+    box) and of the replicated smoothed levels, as in `rap_bytes`.  Level 1 holds no matrix.  Raises ValueError for la < 2,
+    as HexMultigrid refuses it."""
+    la = len(levels) - 1
+    if la < 2:
+        raise ValueError("HexMultigrid: coarse='rap' across ranks needs the rank boxes to halve at least twice "
+                         f"(la = {la}: level 1 would be the gathered level, which is not smoothed)")
+    mine = [lv[rank] for lv in levels]
+    rep = _whole_levels(levels[-1][0].ng)
+    nr = [3 * v[0] * (v[1] + 1) * (v[2] + 1) for v in rep]
+    vectors = 5 * mine[0].n + 6 * sum(b.n for b in mine[1:la]) + 6 * sum(nr[:-1]) + 2 * nr[-1] + nr[-1] ** 2
+    own = sum(b.n for b in mine)
+    csr = sum(_csr_bytes(b.ne, b.n, b.x_lo) for b in mine[2:la]) + sum(_csr_bytes(rep[k], nr[k]) for k in range(len(rep) - 1))
+    return 8 * (vectors + own + 2 * mine[la].n) + csr
 
 
 def rank_levels(blocks) -> list:
@@ -215,12 +241,15 @@ class HexMultigrid:
 
     coarse: "csr" (the default: every smoothed coarse level a device-generated CSR matrix), "index_free" (those levels
     applied by the index-free hex-box operator, Ck = block.E 2^l block.h; `index_free_bytes` gives the one-rank hierarchy's
-    device bytes) or "rap" (one rank, default coarsening, E_field required: level 1 applied as P^T A_0 P from the fine Ck
-    field without a matrix, levels >= 2 the CSR field hierarchy's bit for bit; `rap_bytes` and `rap_setup_peak_bytes`).
-    "index_free" with E_field or coarsening="any" raises ValueError, as does any other string: Galerkin coarse matrices and
-    odd or kept axes are not one Ke on one box.  "rap" raises ValueError before any library call without E_field, with
-    coarsening="any", with a multi-rank `op` and for a box `rap_bytes` refuses (fewer than 3 levels among them).  A rap
-    handle keeps the fine Ck field on the device (8 bytes per element) and reads it in every V-cycle."""
+    device bytes) or "rap" (default coarsening, E_field required: level 1 applied as P^T A_0 P from the fine Ck field
+    without a matrix, levels >= 2 the CSR field hierarchy's bit for bit; `rap_bytes` and `rap_setup_peak_bytes` on one
+    rank, `rap_rank_bytes` across ranks, where each rank applies level 1 on its own level-1 box from its slice of the field
+    and the level's exchange-add completes the product).  "index_free" with E_field or coarsening="any" raises ValueError,
+    as does any other string: Galerkin coarse matrices and odd or kept axes are not one Ke on one box.  "rap" raises
+    ValueError before any library call without E_field, with coarsening="any", on one rank for a box `rap_bytes` refuses
+    (fewer than 3 levels among them), and across ranks without `blocks`, for what the multi-rank field hierarchy refuses,
+    and when the rank boxes do not halve at least twice (la < 2: level 1 would be the gathered level).  A rap handle keeps
+    the fine Ck field (across ranks the rank's slice) on the device (8 bytes per element) and reads it in every V-cycle."""
 
     def __init__(self, op, block: HexBlock, degree: int = 2, lo: float = 0.25, minv: torch.Tensor | None = None, blocks=None,
                  E_field=None, coarsening: str = "even", coarse: str = "csr"):
@@ -246,9 +275,10 @@ class HexMultigrid:
                 raise ValueError("HexMultigrid: coarse='rap' needs E_field (its level 1 is P^T A P of the fine field)")
             if coarsening != "even":
                 raise ValueError("HexMultigrid: coarse='rap' needs the default coarsening")
-            if ranked:
-                raise ValueError("HexMultigrid: coarse='rap' is supported on one rank only")
-            rap_bytes(block.ne)
+            if ranked and blocks is None:
+                raise ValueError("HexMultigrid: coarse='rap' across ranks needs `blocks`, one box per rank (on one rank it needs none)")
+            if not ranked:
+                rap_bytes(block.ne)
         self.coarse = coarse
         if coarsening == "any" and ranked:
             raise ValueError("HexMultigrid: coarsening='any' is supported on one rank only")
@@ -263,6 +293,8 @@ class HexMultigrid:
             if E_field is not None:
                 check_global_field(E_field, block.ng, self.device)
                 nge = gathered_elements(self.levels)
+            if coarse == "rap":
+                rap_rank_bytes(self.levels, comm.rank)
         # across ranks the rank's slice of the global field
         ck = None if E_field is None else field_ck(block_field(E_field, block) if ranked else E_field, block, self.device)
         minv = op.jacobi() if minv is None else minv.to(self.device, torch.float64).contiguous()
@@ -271,6 +303,8 @@ class HexMultigrid:
         box = ctypes.byref(block.cbox())
         uniform = (float(block.E), float(block.h))
         tail = (_lib.ptr(minv), self.degree, self.lo, ctypes.byref(self._h))
+        if coarse == "rap":
+            self._ck = ck              # read by every V-cycle: it lives as long as the handle
         # The library synchronises the device before it reads minv, ck or the ownership weights, whatever stream wrote them.
         lib = _lib.load()
         with torch.cuda.device(self.device):
@@ -282,8 +316,6 @@ class HexMultigrid:
                 else:
                     name, args = ("pcgb_mg_create_index_free" if coarse == "index_free" else "pcgb_mg_create"), uniform
                 _lib.check(getattr(lib, name)(op._solver, box, kep, *args, *tail), name)
-                if coarse == "rap":
-                    self._ck = ck          # read by every V-cycle: it lives as long as the handle
                 return
             from .solver import make_halo
             la = len(self.levels) - 1
@@ -305,7 +337,8 @@ class HexMultigrid:
             if ck is not None:
                 # a plan over the gathered level's element matrices, used by the set-up only
                 kg = make_halo(comm, others, [np.arange(576 * nge, dtype=np.int64)] * len(others), 576 * nge)
-                name, args = "pcgb_mg_create_ranks_field", (kg, owns, kep, _lib.ptr(ck))
+                name = "pcgb_mg_create_ranks_field_rap" if coarse == "rap" else "pcgb_mg_create_ranks_field"
+                args = (kg, owns, kep, _lib.ptr(ck))
             else:
                 name = "pcgb_mg_create_ranks_index_free" if coarse == "index_free" else "pcgb_mg_create_ranks"
                 args = (owns, kep, *uniform)

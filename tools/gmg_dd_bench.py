@@ -1,7 +1,7 @@
 """Jacobi-PCG against multigrid-preconditioned PCG across ranks on the bench's weak-scaled hex stacks (one box of
 --block^3 elements per rank, hexmesh.block_grid / partition_blocks), one GPU per rank.
 
-    torchrun --nproc-per-node 8 tools/gmg_dd_bench.py --block 128 --tol 1e-8 [--operator csr|ebe_ordered|ebe] [--coarse csr|index_free]
+    torchrun --nproc-per-node 8 tools/gmg_dd_bench.py --block 128 --tol 1e-8 [--operator csr|ebe_ordered|ebe] [--coarse csr|index_free|rap]
 
 For each arm, per rank: iterations, flag, the device time of the loop (CUDA events inside the solve), the host wall time
 of the whole solve (ending in a device synchronise and a barrier), and for the multigrid arm its set-up time and the
@@ -15,6 +15,8 @@ Young's modulus C in a matrix of 1), every rank generates its operator from its 
 that voxel model: the multigrid arm builds HexMultigrid(..., E_field=field) with Galerkin coarse levels
 (pcgb_mg_create_ranks_field).  The multigrid line then also reports each rank's Galerkin time and peak element-matrix
 bytes (setup_info) and the drop in free device memory across the set-up.  Without --contrast the output is unchanged.
+--coarse rap (needs --contrast) builds HexMultigrid(coarse="rap", E_field=field): every rank's level 1 applied as
+P^T A_0 P from its slice of the field, with no level-1 matrix (pcgb_mg_create_ranks_field_rap).
 """
 import argparse
 import datetime
@@ -36,11 +38,13 @@ def main():
     ap.add_argument("--degree", type=int, default=2)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--vcycles", type=int, default=20)
-    ap.add_argument("--coarse", choices=["csr", "index_free"], default="csr")
+    ap.add_argument("--coarse", choices=["csr", "index_free", "rap"], default="csr")
     ap.add_argument("--contrast", type=float, default=None)
     ap.add_argument("--fraction", type=float, default=0.4)
     ap.add_argument("--seed", type=int, default=0)
     a = ap.parse_args()
+    if a.coarse == "rap" and a.contrast is None:
+        ap.error("--coarse rap needs --contrast (its level 1 is P^T A P of a voxel field)")
     import torch
     import torch.distributed as dist
     if not torch.cuda.is_available():
