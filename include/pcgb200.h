@@ -353,6 +353,24 @@ int pcgb_hexop_diag(pcgb_hexop_t H, double *d_diag, void *stream);
 int64_t pcgb_hexop_bytes(pcgb_hexop_t H);
 int pcgb_solver_create_hexop(pcgb_hexop_t H, pcgb_halo_t halo /* may be NULL */, pcgb_comm_t comm /* may be NULL */,
                              pcgb_solver_t *out);
+/* The same operator on a periodic cell (homogenisation, DESIGN §2.13): box is the whole mesh (e0 = 0, ne = ng) of nx x ny x
+ * nz elements and as many nodes, node (lx, ly, lz) identified with (lx mod nx, ly mod ny, lz mod nz); no dof is clamped;
+ * dof = 3 node + dir, node = (lz ny + ly) nx + lx, n = 3 nx ny nz.  Each row is the box's per-node order with all 8
+ * elements around the node present (coordinates wrapped); the diagonal sums those 8 in ascending la.  The result is an
+ * ordinary pcgb_hexop_t: pcgb_hexop_apply, _diag, _bytes (16 n, plus 8 per element with a field) and
+ * pcgb_solver_create_hexop take it.  K is singular: its null space is the three rigid translations.  Refusals
+ * (PCGB_ERR_ARG, holding no device memory): e0 != 0, ne != ng or ne < 2 on some axis (ne = 1 would make an element's
+ * nodes coincide), and those of pcgb_hexop_create for ck and d_ck.
+ * pcgb_hexop_periodic_load writes b = -K u_bar, u_bar = eps_bar x, for the macroscopic strain `strain` (Voigt 11, 22,
+ * 33, 23, 13, 12, engineering shears: eps_23 = gamma_23 / 2) and element edge h.  u_bar is taken relative to the node
+ * computed, u_bar(node + d) - u_bar(node) = eps_bar h d (d in {-1, 0, 1}^3), so b depends on no absolute coordinate;
+ * each row is summed in the operator's order (csrc/hexop.cuh).  Mathematically sum_nodes b_dir = 0 (b lies in K's
+ * range).  PCGB_ERR_ARG: a handle that is not periodic, h not finite and positive, a strain that is not finite.
+ * Periodic cells run on one rank without multigrid: pcgb_solver_create_hexop refuses a periodic handle with a halo plan
+ * or a communicator, and every pcgb_mg_create* refuses a solver built on one (PCGB_ERR_ARG, before anything is allocated). */
+int pcgb_hexop_create_periodic(const pcgb_hex_box *box /* e0 = 0, ne = ng */, const double *ke_host, double ck,
+                               const double *d_ck /* NULL = uniform */, pcgb_hexop_t *out);
+int pcgb_hexop_periodic_load(pcgb_hexop_t H, const double strain[6], double h, double *d_b, void *stream);
 
 /* ---------------------------------------------------------------- opt-in: geometric multigrid preconditioner (hex boxes)
  * z = M r is one symmetric V-cycle over nested hex boxes (across ranks: pcgb_mg_create_ranks below), for a one-rank solver whose operator (CSR, EBE or ordered EBE) is
@@ -564,6 +582,24 @@ int pcgb_fields_element(pcgb_fields_t F, const double *d_x, double *d_strain, do
                         void *stream);
 int pcgb_fields_nodal(pcgb_fields_t F, const double *d_x, int kind /* 0 stress, 1 strain */, pcgb_halo_t halo /* NULL on one rank */,
                       double *d_work /* 4 per node */, double *d_out /* 3 per node */, void *stream);
+/* Periodic cells (the numbering of pcgb_hexop_create_periodic; d_x the fluctuation u~, 3 nx ny nz doubles).
+ * pcgb_fields_create_periodic: the refusals of pcgb_fields_create, with the box rule of pcgb_hexop_create_periodic.
+ * pcgb_fields_element and pcgb_fields_nodal refuse its handle (PCGB_ERR_ARG; nodal averages are not defined for it).
+ * pcgb_fields_element_periodic: pcgb_fields_element's outputs with node coordinates wrapped and the macroscopic strain
+ * `strain` (Voigt, engineering shears) added to each centroid strain as tensor strain (eps_k = grad-strain_k + eps_bar_k),
+ * before the unchanged stress law and principal values.
+ * pcgb_fields_average: the volume averages of that strain and stress over the cell, out_strain and out_stress (host, 6
+ * each), from one element pass with no per-element output and a fixed two-stage reduction (per-brick halving trees,
+ * then one CTA summing the brick partials in ascending order; the exact order is in csrc/fields.cuh), so the result is
+ * bit-reproducible.  The plain element mean is the exact volume average: on a brick the centroid strain is the element's
+ * volume average and E is constant per element.  Scratch of 12 doubles per 256-element brick is allocated and freed on
+ * `stream`, which the call synchronises.  Both refuse a handle that is not periodic and (element) x overlapping an output. */
+int pcgb_fields_create_periodic(const pcgb_hex_box *box /* e0 = 0, ne = ng */, double h, double E, double nu,
+                                const double *d_E /* NULL = uniform E */, pcgb_fields_t *out);
+int pcgb_fields_element_periodic(pcgb_fields_t F, const double *d_x, const double strain[6], double *d_strain, double *d_stress,
+                                 double *d_ps, double *d_pe, void *stream);
+int pcgb_fields_average(pcgb_fields_t F, const double *d_x, const double strain[6], double out_strain[6], double out_stress[6],
+                        void *stream);
 
 #ifdef __cplusplus
 }

@@ -7,11 +7,13 @@ Public surface (mirrors the reference's solver/partition API for this path, SURV
     CsrMatrix, SubdomainOperator, Communicator
     HexFields(block, ...)           strains, stresses, principal values and their nodal averages of a hex box
                                     (updateElemStrain / getNodalPS, pcg_solver.py:601-618, 730-814)
+    effective_stiffness(cell, ...)  the 6x6 effective elastic tensor of a periodic voxel cell (homogenize.py)
 Everything numerical runs in csrc/libpcgb200.so (hand-written sm_90a CUDA, C ABI in include/pcgb200.h).
 """
 from .solver import Communicator, SolveInfo, SubdomainOperator, solve  # noqa: F401
 from .csr import CsrMatrix  # noqa: F401
 from .fields import HexFields  # noqa: F401
+from .homogenize import effective_stiffness  # noqa: F401
 
 
 def partition_mesh(*args, **kwargs):
@@ -19,4 +21,4 @@ def partition_mesh(*args, **kwargs):
     return _pm(*args, **kwargs)
 
 
-__all__ = ["solve", "partition_mesh", "CsrMatrix", "SubdomainOperator", "Communicator", "SolveInfo", "HexFields"]
+__all__ = ["solve", "partition_mesh", "CsrMatrix", "SubdomainOperator", "Communicator", "SolveInfo", "HexFields", "effective_stiffness"]

@@ -42,6 +42,19 @@
 // brick's nodes (one more per axis) of x in shared memory with plain coalesced loads, as k_hexop does.  kOut selects the
 // outputs at compile time, so a pass without principal values has no trigonometry.  k_fields_nodal sums a scratch copy of
 // the element principal values per node; k_fields_divide finishes the average.  Offsets are 64-bit throughout.
+//
+// Periodic cells (kPeriodic, DESIGN §2.13; the numbering of hexop.cuh's periodic cells: node = (lz ny + ly) nx + lx, node
+// coordinates wrapped modulo the cell): x is the periodic fluctuation u~; the staging wraps node nx to 0 (and so on), and
+// the macroscopic strain eps_bar (Voigt, tensor shears) is added to the centroid strain, eps_k = g-strain_k + eps_bar_k;
+// the stress law and principal values are then the code above, unchanged.  Nodal averages are not defined for them.
+//   average  k_fields_average: the same element pass, fused with a deterministic two-stage reduction of the 12 values
+//            (eps_0..5, sigma_0..5) and no per-element output.  Stage 1: thread t = tx + 32 ty + 128 tz of brick b holds its
+//            element's values (0.0 for a thread outside the cell); for w = 128, 64, ..., 1: v[t] = v[t] + v[t + w] (t < w);
+//            partial[b] = v[0].  Stage 2 (k_fields_average_final, one CTA of 256 threads): with c = ceil(nb / 256), thread t
+//            sums acc = 0.0 + partial[t c] + partial[t c + 1] + ... (ascending b, b < nb), the same halving tree over the 256
+//            sums follows, and mean = sum / (nx ny nz).  On a brick the centroid strain is the element's volume average
+//            and E is constant per element, so the plain mean of the element stresses is the exact volume average of the
+//            finite-element stress field.  The result is bit-reproducible: no atomics, a fixed order.
 #pragma once
 #include "common.cuh"
 #include "hexgen.cuh"
@@ -52,6 +65,8 @@ constexpr int kFdBX = 32, kFdBY = 4, kFdBZ = 2;          // elements per brick
 constexpr int kFdThreads = kFdBX * kFdBY * kFdBZ;
 constexpr int kFdSX = kFdBX + 1, kFdSY = kFdBY + 1, kFdSZ = kFdBZ + 1;   // staged nodes
 constexpr int kFdStrain = 1, kFdStress = 2, kFdPS = 4, kFdPE = 8;         // output bits of k_fields_elem
+
+struct FieldsMacro { double e[6]; };   // the macroscopic strain of a periodic cell (Voigt, tensor shears); unread otherwise
 
 struct FieldsShape {
   HexGeom g;
@@ -94,29 +109,30 @@ __device__ __forceinline__ void principal3(const double (&s)[6], double *p) {
   p[2] = lo;
 }
 
-template <int kOut, bool kField>
-__global__ void __launch_bounds__(kFdThreads)
-k_fields_elem(FieldsShape s, const double *__restrict__ Ef, const double *__restrict__ x, double *__restrict__ strain,
-              double *__restrict__ stress, double *__restrict__ ps, double *__restrict__ pe) {
-  __shared__ double sx[kFdSZ][kFdSY][kFdSX * 3];
-  const HexGeom &g = s.g;
-  const int b = blockIdx.x;
-  const int bx = b % s.nbx, by = (b / s.nbx) % s.nby, bz = b / (s.nbx * s.nby);
-  const int ox0 = bx * kFdBX, oy0 = by * kFdBY, oz0 = bz * kFdBZ;   // first element of the brick = its first node
+// The brick's nodes of x (one more than its elements per axis) into sx: 0.0 on the clamped line and outside the box, or, on
+// a periodic cell, node n of an axis wrapped to 0
+template <bool kPeriodic>
+__device__ __forceinline__ void fields_stage(const HexGeom &g, const double *__restrict__ x, int ox0, int oy0, int oz0,
+                                             double (&sx)[kFdSZ][kFdSY][kFdSX * 3]) {
   for (int t = threadIdx.x; t < kFdSZ * kFdSY * kFdSX * 3; t += kFdThreads) {
     const int c = t % (kFdSX * 3), r = t / (kFdSX * 3);
     const int sy = r % kFdSY, sz = r / kFdSY;
     const int lx = ox0 + c / 3, ly = oy0 + sy, lz = oz0 + sz;
     double v = 0.0;
-    if (lx >= g.x_lo && lx <= g.nx && ly <= g.ny && lz <= g.nz)
+    if (kPeriodic) {
+      if (lx <= g.nx && ly <= g.ny && lz <= g.nz)
+        v = x[3 * (((int64_t)(lz == g.nz ? 0 : lz) * g.ny + (ly == g.ny ? 0 : ly)) * g.nx + (lx == g.nx ? 0 : lx)) + c % 3];
+    } else if (lx >= g.x_lo && lx <= g.nx && ly <= g.ny && lz <= g.nz) {
       v = x[3 * (((int64_t)lz * (g.ny + 1) + ly) * g.nxf + (lx - g.x_lo)) + c % 3];
+    }
     sx[sz][sy][c] = v;
   }
-  __syncthreads();
-  const int tx = threadIdx.x % kFdBX, ty = (threadIdx.x / kFdBX) % kFdBY, tz = threadIdx.x / (kFdBX * kFdBY);
-  const int ox = ox0 + tx, oy = oy0 + ty, oz = oz0 + tz;
-  if (ox >= g.nx || oy >= g.ny || oz >= g.nz) return;
-  const int64_t e = ((int64_t)oz * g.ny + oy) * g.nx + ox;
+}
+
+// the centroid strain of element (tx, ty, tz) of the staged brick (header: strain), plus eps_bar on a periodic cell
+template <bool kPeriodic>
+__device__ __forceinline__ void fields_strain(const double (&sx)[kFdSZ][kFdSY][kFdSX * 3], int tx, int ty, int tz, double q,
+                                              const FieldsMacro &m, double (&eps)[6]) {
   double gr[3][3];   // gr[a][i] = d u_i / d x_a
 #pragma unroll
   for (int a = 0; a < 3; ++a)
@@ -128,15 +144,47 @@ k_fields_elem(FieldsShape s, const double *__restrict__ Ef, const double *__rest
         const double u = sx[tz + (l >> 2)][ty + ((l >> 1) & 1)][3 * (tx + (l & 1)) + i];
         acc = ((l >> a) & 1) ? __dadd_rn(acc, u) : __dsub_rn(acc, u);
       }
-      gr[a][i] = __dmul_rn(acc, s.q);
+      gr[a][i] = __dmul_rn(acc, q);
     }
-  double eps[6];
   eps[0] = gr[0][0];
   eps[1] = gr[1][1];
   eps[2] = gr[2][2];
   eps[3] = __dmul_rn(0.5, __dadd_rn(gr[1][2], gr[2][1]));
   eps[4] = __dmul_rn(0.5, __dadd_rn(gr[0][2], gr[2][0]));
   eps[5] = __dmul_rn(0.5, __dadd_rn(gr[0][1], gr[1][0]));
+  if (kPeriodic) {
+#pragma unroll
+    for (int k = 0; k < 6; ++k) eps[k] = __dadd_rn(eps[k], m.e[k]);
+  }
+}
+
+// sigma = E D eps (header: stress)
+__device__ __forceinline__ void fields_stress(const FieldsShape &s, double E, const double (&eps)[6], double (&sg)[6]) {
+  const double tr = __dadd_rn(__dadd_rn(eps[0], eps[1]), eps[2]);
+  const double ltr = __dmul_rn(s.lam, tr);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) sg[k] = __dmul_rn(E, __dadd_rn(ltr, __dmul_rn(s.m2, eps[k])));
+#pragma unroll
+  for (int k = 3; k < 6; ++k) sg[k] = __dmul_rn(E, __dmul_rn(s.m2, eps[k]));
+}
+
+template <int kOut, bool kField, bool kPeriodic = false>
+__global__ void __launch_bounds__(kFdThreads)
+k_fields_elem(FieldsShape s, const double *__restrict__ Ef, const double *__restrict__ x, double *__restrict__ strain,
+              double *__restrict__ stress, double *__restrict__ ps, double *__restrict__ pe, const FieldsMacro m) {
+  __shared__ double sx[kFdSZ][kFdSY][kFdSX * 3];
+  const HexGeom &g = s.g;
+  const int b = blockIdx.x;
+  const int bx = b % s.nbx, by = (b / s.nbx) % s.nby, bz = b / (s.nbx * s.nby);
+  const int ox0 = bx * kFdBX, oy0 = by * kFdBY, oz0 = bz * kFdBZ;   // first element of the brick = its first node
+  fields_stage<kPeriodic>(g, x, ox0, oy0, oz0, sx);
+  __syncthreads();
+  const int tx = threadIdx.x % kFdBX, ty = (threadIdx.x / kFdBX) % kFdBY, tz = threadIdx.x / (kFdBX * kFdBY);
+  const int ox = ox0 + tx, oy = oy0 + ty, oz = oz0 + tz;
+  if (ox >= g.nx || oy >= g.ny || oz >= g.nz) return;
+  const int64_t e = ((int64_t)oz * g.ny + oy) * g.nx + ox;
+  double eps[6];
+  fields_strain<kPeriodic>(sx, tx, ty, tz, s.q, m, eps);
   if (kOut & kFdStrain) {
 #pragma unroll
     for (int k = 0; k < 6; ++k) strain[6 * e + k] = eps[k];
@@ -148,14 +196,8 @@ k_fields_elem(FieldsShape s, const double *__restrict__ Ef, const double *__rest
     for (int k = 0; k < 3; ++k) pe[3 * e + k] = p[k];
   }
   if (kOut & (kFdStress | kFdPS)) {
-    const double E = kField ? Ef[e] : s.E;
-    const double tr = __dadd_rn(__dadd_rn(eps[0], eps[1]), eps[2]);
-    const double ltr = __dmul_rn(s.lam, tr);
     double sg[6];
-#pragma unroll
-    for (int k = 0; k < 3; ++k) sg[k] = __dmul_rn(E, __dadd_rn(ltr, __dmul_rn(s.m2, eps[k])));
-#pragma unroll
-    for (int k = 3; k < 6; ++k) sg[k] = __dmul_rn(E, __dmul_rn(s.m2, eps[k]));
+    fields_stress(s, kField ? Ef[e] : s.E, eps, sg);
     if (kOut & kFdStress) {
 #pragma unroll
       for (int k = 0; k < 6; ++k) stress[6 * e + k] = sg[k];
@@ -167,6 +209,72 @@ k_fields_elem(FieldsShape s, const double *__restrict__ Ef, const double *__rest
       for (int k = 0; k < 3; ++k) ps[3 * e + k] = p[k];
     }
   }
+}
+
+constexpr int kFdAvg = 12;   // averaged values: strain 0..5, stress 0..5
+
+// v[k][t] = v[k][t] + v[k][t + w] for w = 128, 64, ..., 1 over the CTA's 256 threads (header: average); the sums end in v[k][0]
+__device__ __forceinline__ void fields_tree(double (&v)[kFdAvg][kFdThreads]) {
+#pragma unroll
+  for (int w = kFdThreads / 2; w >= 1; w >>= 1) {
+    __syncthreads();
+    if ((int)threadIdx.x < w) {
+#pragma unroll
+      for (int k = 0; k < kFdAvg; ++k) v[k][threadIdx.x] = __dadd_rn(v[k][threadIdx.x], v[k][threadIdx.x + w]);
+    }
+  }
+  __syncthreads();
+}
+
+// stage 1 of the average on a periodic cell: the element pass of k_fields_elem<., ., true>, then brick b's 12 sums into
+// partial[12 b + k]
+template <bool kField>
+__global__ void __launch_bounds__(kFdThreads)
+k_fields_average(FieldsShape s, const double *__restrict__ Ef, const double *__restrict__ x, const FieldsMacro m,
+                 double *__restrict__ partial) {
+  __shared__ double sx[kFdSZ][kFdSY][kFdSX * 3];
+  __shared__ double v[kFdAvg][kFdThreads];
+  const HexGeom &g = s.g;
+  const int b = blockIdx.x;
+  const int bx = b % s.nbx, by = (b / s.nbx) % s.nby, bz = b / (s.nbx * s.nby);
+  const int ox0 = bx * kFdBX, oy0 = by * kFdBY, oz0 = bz * kFdBZ;
+  fields_stage<true>(g, x, ox0, oy0, oz0, sx);
+  __syncthreads();
+  const int tx = threadIdx.x % kFdBX, ty = (threadIdx.x / kFdBX) % kFdBY, tz = threadIdx.x / (kFdBX * kFdBY);
+  const int ox = ox0 + tx, oy = oy0 + ty, oz = oz0 + tz;
+  if (ox < g.nx && oy < g.ny && oz < g.nz) {
+    double eps[6], sg[6];
+    fields_strain<true>(sx, tx, ty, tz, s.q, m, eps);
+    fields_stress(s, kField ? Ef[((int64_t)oz * g.ny + oy) * g.nx + ox] : s.E, eps, sg);
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+      v[k][threadIdx.x] = eps[k];
+      v[6 + k][threadIdx.x] = sg[k];
+    }
+  } else {
+#pragma unroll
+    for (int k = 0; k < kFdAvg; ++k) v[k][threadIdx.x] = 0.0;
+  }
+  fields_tree(v);
+  if (threadIdx.x < kFdAvg) partial[(int64_t)kFdAvg * b + threadIdx.x] = v[threadIdx.x][0];
+}
+
+// stage 2: one CTA; thread t sums partials t c .. t c + c - 1 in ascending order, the tree sums the 256, out = sum / ne
+__global__ void __launch_bounds__(kFdThreads)
+k_fields_average_final(int64_t nb, double ne, const double *__restrict__ partial, double *__restrict__ out) {
+  __shared__ double v[kFdAvg][kFdThreads];
+  const int64_t c = (nb + kFdThreads - 1) / kFdThreads;
+  const int64_t b0 = c * threadIdx.x, b1 = b0 + c < nb ? b0 + c : nb;
+  double acc[kFdAvg];
+#pragma unroll
+  for (int k = 0; k < kFdAvg; ++k) acc[k] = 0.0;
+  for (int64_t b = b0; b < b1; ++b)
+#pragma unroll
+    for (int k = 0; k < kFdAvg; ++k) acc[k] = __dadd_rn(acc[k], partial[kFdAvg * b + k]);
+#pragma unroll
+  for (int k = 0; k < kFdAvg; ++k) v[k][threadIdx.x] = acc[k];
+  fields_tree(v);
+  if (threadIdx.x < kFdAvg) out[threadIdx.x] = __ddiv_rn(v[threadIdx.x][0], ne);
 }
 
 // one thread per node of the box: (sum_0, sum_1, sum_2, count) of the element values pv (ne x 3) around it, ascending la
@@ -214,25 +322,42 @@ inline FieldsShape fields_shape(const HexGeom &g) {
   return s;
 }
 
-template <int kOut>
-inline void fields_elem_launch(const FieldsShape &s, const double *Ef, const double *x, double *strain, double *stress, double *ps,
-                               double *pe, cudaStream_t st) {
+template <int kOut, bool kPeriodic>
+inline void fields_elem_launch(const FieldsShape &s, const FieldsMacro &m, const double *Ef, const double *x, double *strain,
+                               double *stress, double *ps, double *pe, cudaStream_t st) {
   const unsigned grid = (unsigned)((int64_t)s.nbx * s.nby * s.nbz);
-  if (Ef) k_fields_elem<kOut, true><<<grid, kFdThreads, 0, st>>>(s, Ef, x, strain, stress, ps, pe);
-  else k_fields_elem<kOut, false><<<grid, kFdThreads, 0, st>>>(s, nullptr, x, strain, stress, ps, pe);
+  if (Ef) k_fields_elem<kOut, true, kPeriodic><<<grid, kFdThreads, 0, st>>>(s, Ef, x, strain, stress, ps, pe, m);
+  else k_fields_elem<kOut, false, kPeriodic><<<grid, kFdThreads, 0, st>>>(s, nullptr, x, strain, stress, ps, pe, m);
 }
 
-// the element pass for the outputs that are not NULL (at least one)
+// the element pass for the outputs that are not NULL (at least one); m (the macroscopic strain) only with periodic
 inline int fields_elem(const FieldsShape &s, const double *Ef, const double *x, double *strain, double *stress, double *ps, double *pe,
-                       cudaStream_t st) {
-  using L = void (*)(const FieldsShape &, const double *, const double *, double *, double *, double *, double *, cudaStream_t);
-  static const L table[16] = {nullptr, fields_elem_launch<1>, fields_elem_launch<2>, fields_elem_launch<3>,
-                              fields_elem_launch<4>, fields_elem_launch<5>, fields_elem_launch<6>, fields_elem_launch<7>,
-                              fields_elem_launch<8>, fields_elem_launch<9>, fields_elem_launch<10>, fields_elem_launch<11>,
-                              fields_elem_launch<12>, fields_elem_launch<13>, fields_elem_launch<14>, fields_elem_launch<15>};
+                       cudaStream_t st, bool periodic = false, const FieldsMacro &m = FieldsMacro{}) {
+  using L = void (*)(const FieldsShape &, const FieldsMacro &, const double *, const double *, double *, double *, double *, double *,
+                     cudaStream_t);
+#define PCGB_FD_ROW(P)                                                                                                              \
+  {nullptr, fields_elem_launch<1, P>, fields_elem_launch<2, P>, fields_elem_launch<3, P>, fields_elem_launch<4, P>,             \
+   fields_elem_launch<5, P>, fields_elem_launch<6, P>, fields_elem_launch<7, P>, fields_elem_launch<8, P>,                      \
+   fields_elem_launch<9, P>, fields_elem_launch<10, P>, fields_elem_launch<11, P>, fields_elem_launch<12, P>,                   \
+   fields_elem_launch<13, P>, fields_elem_launch<14, P>, fields_elem_launch<15, P>}
+  static const L table[2][16] = {PCGB_FD_ROW(false), PCGB_FD_ROW(true)};
+#undef PCGB_FD_ROW
   const int out = (strain ? kFdStrain : 0) | (stress ? kFdStress : 0) | (ps ? kFdPS : 0) | (pe ? kFdPE : 0);
   if (out == 0) return PCGB_OK;
-  table[out](s, Ef, x, strain, stress, ps, pe, st);
+  table[periodic ? 1 : 0][out](s, m, Ef, x, strain, stress, ps, pe, st);
+  PCGB_CHECK_LAUNCH();
+  return PCGB_OK;
+}
+
+// The volume averages of strain and stress over a periodic cell (header: average): out[0..5] strain, out[6..11] stress,
+// device; partial holds 12 doubles per brick
+inline int fields_average(const FieldsShape &s, const FieldsMacro &m, const double *Ef, const double *x, double *partial, double *out,
+                          cudaStream_t st) {
+  const int64_t nb = (int64_t)s.nbx * s.nby * s.nbz;
+  if (Ef) k_fields_average<true><<<(unsigned)nb, kFdThreads, 0, st>>>(s, Ef, x, m, partial);
+  else k_fields_average<false><<<(unsigned)nb, kFdThreads, 0, st>>>(s, nullptr, x, m, partial);
+  PCGB_CHECK_LAUNCH();
+  k_fields_average_final<<<1, kFdThreads, 0, st>>>(nb, (double)((int64_t)s.g.nx * s.g.ny * s.g.nz), partial, out);
   PCGB_CHECK_LAUNCH();
   return PCGB_OK;
 }

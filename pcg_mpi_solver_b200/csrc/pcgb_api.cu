@@ -52,6 +52,7 @@ struct pcgb_fields_s {
   FieldsShape s;
   const double *d_E = nullptr;   // per-element E (caller-owned), or NULL
   int64_t ne = 0, nnodes = 0, n = 0;   // elements, nodes (clamped line included), free dofs
+  bool periodic = false;         // a periodic cell (pcgb_fields_create_periodic)
 };
 
 // What may differ between two solves on one handle and changes the captured iterations (the operator, the x buffers and
@@ -921,6 +922,8 @@ int pcgb_solver_create_ebe_ordered(pcgb_ebe_ordered_t O, pcgb_halo_t halo, pcgb_
 // the index-free hex-box operator (pcg_solver.py:263-300 in the ordered operator's order)
 int pcgb_solver_create_hexop(pcgb_hexop_t H, pcgb_halo_t halo, pcgb_comm_t comm, pcgb_solver_t *out) {
   if (!H || !out) return fail(PCGB_ERR_ARG, "pcgb_solver_create_hexop: null argument");
+  if (H->H.periodic && (halo || comm))
+    return fail(PCGB_ERR_ARG, "pcgb_solver_create_hexop: a periodic cell runs on one rank (no halo plan or communicator)");
   return solver_create_common(FineOp{nullptr, nullptr, nullptr, H}, halo, comm, out);
 }
 
@@ -1717,10 +1720,12 @@ int mg_hex_csr(const HexGeom &g, const double *ke_host, double ck, int64_t **rp,
   return PCGB_OK;
 }
 
-// The index-free operator of box g: Ke (row-major 24x24) and its diagonal by value, Ck uniform or (d_ck) per element
-HexOp hexop_of(const HexGeom &g, const double *ke_host, double ck, const double *d_ck) {
+// The index-free operator of box g: Ke (row-major 24x24) and its diagonal by value, Ck uniform or (d_ck) per element;
+// periodic: g is a periodic cell (periodic_geom)
+HexOp hexop_of(const HexGeom &g, const double *ke_host, double ck, const double *d_ck, bool periodic = false) {
   HexOp H;
-  H.s = hexop_shape(g);
+  H.s = hexop_shape(g, periodic);
+  H.periodic = periodic;
   std::memcpy(H.ke.k, ke_host, sizeof(H.ke.k));
   for (int a = 0; a < 24; ++a) H.kd.k[a] = ke_host[a * 24 + a];
   H.ck = d_ck ? 0.0 : ck;
@@ -2099,6 +2104,8 @@ int mg_check_ranges(int degree, double lo, double E, double h, const char *who) 
 }
 
 int mg_check_rows(pcgb_solver_t s, const pcgb_hex_box *box, const char *who) {
+  // a periodic cell's rows can equal a clamped box's (8x5x5 and 8x4x4: 600), but its hierarchy is not built
+  if (s->op.H && s->op.H->H.periodic) return fail(PCGB_ERR_ARG, "%s: the solver's operator is a periodic cell's (no multigrid)", who);
   const int64_t n = 3 * hex_geom(box).nfree_nodes;
   if (n == s->n) return PCGB_OK;
   return fail(PCGB_ERR_ARG, "%s: the solver's operator has %lld rows, the box %lld", who, (long long)s->n, (long long)n);
@@ -2532,28 +2539,60 @@ int pcgb_hex_fill_field(const pcgb_hex_box *box, const double *ke_host, const do
 // calcMatVecProd (pcg_solver.py:263-300) on a structured box, every index computed from the node's coordinates; the
 // product and the diagonal (updatePreconditioner, :282-287) are bit-identical to the ordered EBE operator's on
 // hexmesh.hex_type_group(box).
+namespace {
+// pcgb_hexop_create and pcgb_hexop_create_periodic after their box checks: the handle, or the refusals of a grid too large
+// and of a field entry that is not finite and positive
+int hexop_make(const HexGeom &g, bool periodic, const double *ke_host, double ck, const double *d_ck, const char *who, pcgb_hexop_t *out) {
+  if (!d_ck && !(std::isfinite(ck) && ck > 0.0)) return fail(PCGB_ERR_ARG, "%s: Ck must be finite and positive", who);
+  PCGB_TRY(require_device());
+  const HexOp H = hexop_of(g, ke_host, ck, d_ck, periodic);
+  if ((int64_t)H.s.nbx * H.s.nby * H.s.nbz >= (int64_t)1 << 31) return fail(PCGB_ERR_ARG, "%s: box too large", who);
+  if (d_ck) {
+    // the check runs on the legacy stream, which does not wait for non-blocking streams: finish the caller's writes first
+    PCGB_CUDA(cudaDeviceSynchronize());
+    int bad = 0;
+    PCGB_TRY(field_bad((int64_t)g.nx * g.ny * g.nz, d_ck, 0, who, &bad));
+    if (bad) return fail(PCGB_ERR_ARG, "%s: every Ck of the field must be finite and positive", who);
+  }
+  pcgb_hexop_t h = new pcgb_hexop_s();
+  h->H = H;
+  *out = h;
+  return PCGB_OK;
+}
+
+// a periodic cell is a whole mesh with at least two elements per axis
+bool periodic_box_ok(const pcgb_hex_box *box) {
+  for (int a = 0; a < 3; ++a)
+    if (box->e0[a] != 0 || box->ne[a] != box->ng[a] || box->ne[a] < 2) return false;
+  return true;
+}
+}  // namespace
+
 int pcgb_hexop_create(const pcgb_hex_box *box, const double *ke_host, double ck, const double *d_ck, pcgb_hexop_t *out) {
   if (!box || !ke_host || !out) return fail(PCGB_ERR_ARG, "pcgb_hexop_create: null argument");
   *out = nullptr;
   for (int a = 0; a < 3; ++a)
     if (box->ne[a] <= 0 || box->e0[a] < 0 || (int64_t)box->e0[a] + box->ne[a] > box->ng[a])
       return fail(PCGB_ERR_ARG, "pcgb_hexop_create: the box must have ne > 0 and lie inside its global mesh on every axis");
-  if (!d_ck && !(std::isfinite(ck) && ck > 0.0)) return fail(PCGB_ERR_ARG, "pcgb_hexop_create: Ck must be finite and positive");
-  PCGB_TRY(require_device());
-  const HexOp H = hexop_of(hex_geom(box), ke_host, ck, d_ck);
-  const HexGeom &g = H.s.g;
-  if ((int64_t)H.s.nbx * H.s.nby * H.s.nbz >= (int64_t)1 << 31) return fail(PCGB_ERR_ARG, "pcgb_hexop_create: box too large");
-  if (d_ck) {
-    // the check runs on the legacy stream, which does not wait for non-blocking streams: finish the caller's writes first
-    PCGB_CUDA(cudaDeviceSynchronize());
-    int bad = 0;
-    PCGB_TRY(field_bad((int64_t)g.nx * g.ny * g.nz, d_ck, 0, "pcgb_hexop_create", &bad));
-    if (bad) return fail(PCGB_ERR_ARG, "pcgb_hexop_create: every Ck of the field must be finite and positive");
-  }
-  pcgb_hexop_t h = new pcgb_hexop_s();
-  h->H = H;
-  *out = h;
-  return PCGB_OK;
+  return hexop_make(hex_geom(box), false, ke_host, ck, d_ck, "pcgb_hexop_create", out);
+}
+
+// the periodic cell's operator (hexop.cuh): every node free, coordinates wrapped, the box's per-node order
+int pcgb_hexop_create_periodic(const pcgb_hex_box *box, const double *ke_host, double ck, const double *d_ck, pcgb_hexop_t *out) {
+  if (!box || !ke_host || !out) return fail(PCGB_ERR_ARG, "pcgb_hexop_create_periodic: null argument");
+  *out = nullptr;
+  if (!periodic_box_ok(box))
+    return fail(PCGB_ERR_ARG, "pcgb_hexop_create_periodic: a periodic cell needs e0 = 0, ne = ng and ne >= 2 on every axis");
+  return hexop_make(periodic_geom(box), true, ke_host, ck, d_ck, "pcgb_hexop_create_periodic", out);
+}
+
+int pcgb_hexop_periodic_load(pcgb_hexop_t H, const double strain[6], double h, double *d_b, void *stream) {
+  if (!H || !strain || !d_b) return fail(PCGB_ERR_ARG, "pcgb_hexop_periodic_load: null argument");
+  if (!H->H.periodic) return fail(PCGB_ERR_ARG, "pcgb_hexop_periodic_load: the operator is not a periodic cell's");
+  if (!(std::isfinite(h) && h > 0.0)) return fail(PCGB_ERR_ARG, "pcgb_hexop_periodic_load: h must be finite and positive");
+  for (int k = 0; k < 6; ++k)
+    if (!std::isfinite(strain[k])) return fail(PCGB_ERR_ARG, "pcgb_hexop_periodic_load: the strain must be finite");
+  return hexop_load(H->H, strain, h, d_b, (cudaStream_t)stream);
 }
 
 int pcgb_hexop_destroy(pcgb_hexop_t H) {
@@ -2578,25 +2617,21 @@ int64_t pcgb_hexop_bytes(pcgb_hexop_t H) { return H ? H->H.bytes : 0; }
 // ------------------------------------------------------------------------------------ strain and stress recovery
 // updateElemStrain (pcg_solver.py:601-618), getNodalPS (:730-814) and getPrincipalStress / getPrincipalStrain
 // (file_operations.py:251-301) on a hex box; the arithmetic contract is in fields.cuh.
-int pcgb_fields_create(const pcgb_hex_box *box, double h, double E, double nu, const double *d_E, pcgb_fields_t *out) {
-  if (!box || !out) return fail(PCGB_ERR_ARG, "pcgb_fields_create: null argument");
-  *out = nullptr;
-  for (int a = 0; a < 3; ++a)
-    if (box->ne[a] <= 0 || box->e0[a] < 0 || (int64_t)box->e0[a] + box->ne[a] > box->ng[a])
-      return fail(PCGB_ERR_ARG, "pcgb_fields_create: the box must have ne > 0 and lie inside its global mesh on every axis");
+namespace {
+// pcgb_fields_create and pcgb_fields_create_periodic after their box checks
+int fields_make(const HexGeom &g, bool periodic, double h, double E, double nu, const double *d_E, const char *who, pcgb_fields_t *out) {
   if (!(std::isfinite(h) && h > 0.0) || !(std::isfinite(E) && E > 0.0) || !(nu > -1.0 && nu < 0.5))
-    return fail(PCGB_ERR_ARG, "pcgb_fields_create: h and E must be finite and positive and -1 < nu < 0.5");
+    return fail(PCGB_ERR_ARG, "%s: h and E must be finite and positive and -1 < nu < 0.5", who);
   PCGB_TRY(require_device());
-  const HexGeom g = hex_geom(box);
   FieldsShape s = fields_shape(g);
-  if ((int64_t)s.nbx * s.nby * s.nbz >= (int64_t)1 << 31) return fail(PCGB_ERR_ARG, "pcgb_fields_create: box too large");
+  if ((int64_t)s.nbx * s.nby * s.nbz >= (int64_t)1 << 31) return fail(PCGB_ERR_ARG, "%s: box too large", who);
   const int64_t ne = (int64_t)g.nx * g.ny * g.nz;
   if (d_E) {
     // the check runs on the legacy stream, which does not wait for non-blocking streams: finish the caller's writes first
     PCGB_CUDA(cudaDeviceSynchronize());
     int bad = 0;
-    PCGB_TRY(field_bad(ne, d_E, 0, "pcgb_fields_create", &bad));
-    if (bad) return fail(PCGB_ERR_ARG, "pcgb_fields_create: every E of the field must be finite and positive");
+    PCGB_TRY(field_bad(ne, d_E, 0, who, &bad));
+    if (bad) return fail(PCGB_ERR_ARG, "%s: every E of the field must be finite and positive", who);
   }
   // lambda and mu as hexmesh.hex_element_stiffness(1.0, nu) computes them
   const double one = 1.0;
@@ -2608,10 +2643,36 @@ int pcgb_fields_create(const pcgb_hex_box *box, double h, double E, double nu, c
   F->s = s;
   F->d_E = d_E;
   F->ne = ne;
-  F->nnodes = (int64_t)(g.nx + 1) * (g.ny + 1) * (g.nz + 1);
+  F->nnodes = periodic ? g.nfree_nodes : (int64_t)(g.nx + 1) * (g.ny + 1) * (g.nz + 1);
   F->n = 3 * g.nfree_nodes;
+  F->periodic = periodic;
   *out = F;
   return PCGB_OK;
+}
+
+// eps_bar with tensor shears from a Voigt strain with engineering shears
+FieldsMacro fields_macro(const double strain[6]) {
+  FieldsMacro m;
+  for (int k = 0; k < 6; ++k) m.e[k] = k < 3 ? strain[k] : 0.5 * strain[k];
+  return m;
+}
+}  // namespace
+
+int pcgb_fields_create(const pcgb_hex_box *box, double h, double E, double nu, const double *d_E, pcgb_fields_t *out) {
+  if (!box || !out) return fail(PCGB_ERR_ARG, "pcgb_fields_create: null argument");
+  *out = nullptr;
+  for (int a = 0; a < 3; ++a)
+    if (box->ne[a] <= 0 || box->e0[a] < 0 || (int64_t)box->e0[a] + box->ne[a] > box->ng[a])
+      return fail(PCGB_ERR_ARG, "pcgb_fields_create: the box must have ne > 0 and lie inside its global mesh on every axis");
+  return fields_make(hex_geom(box), false, h, E, nu, d_E, "pcgb_fields_create", out);
+}
+
+int pcgb_fields_create_periodic(const pcgb_hex_box *box, double h, double E, double nu, const double *d_E, pcgb_fields_t *out) {
+  if (!box || !out) return fail(PCGB_ERR_ARG, "pcgb_fields_create_periodic: null argument");
+  *out = nullptr;
+  if (!periodic_box_ok(box))
+    return fail(PCGB_ERR_ARG, "pcgb_fields_create_periodic: a periodic cell needs e0 = 0, ne = ng and ne >= 2 on every axis");
+  return fields_make(periodic_geom(box), true, h, E, nu, d_E, "pcgb_fields_create_periodic", out);
 }
 
 int pcgb_fields_destroy(pcgb_fields_t F) {
@@ -2627,6 +2688,7 @@ static bool overlap(const double *a, int64_t na, const double *b, int64_t nb) {
 
 int pcgb_fields_element(pcgb_fields_t F, const double *d_x, double *d_strain, double *d_stress, double *d_ps, double *d_pe, void *stream) {
   if (!F || !d_x) return fail(PCGB_ERR_ARG, "pcgb_fields_element: null argument");
+  if (F->periodic) return fail(PCGB_ERR_ARG, "pcgb_fields_element: a periodic cell's fields need its strain: pcgb_fields_element_periodic");
   const int64_t ne = F->ne;
   if (overlap(d_x, F->n, d_strain, 6 * ne) || overlap(d_x, F->n, d_stress, 6 * ne) || overlap(d_x, F->n, d_ps, 3 * ne) ||
       overlap(d_x, F->n, d_pe, 3 * ne))
@@ -2637,6 +2699,7 @@ int pcgb_fields_element(pcgb_fields_t F, const double *d_x, double *d_strain, do
 int pcgb_fields_nodal(pcgb_fields_t F, const double *d_x, int kind, pcgb_halo_t halo, double *d_work, double *d_out, void *stream) {
   if (!F || !d_x || !d_work || !d_out) return fail(PCGB_ERR_ARG, "pcgb_fields_nodal: null argument");
   if (kind != 0 && kind != 1) return fail(PCGB_ERR_ARG, "pcgb_fields_nodal: kind must be 0 (stress) or 1 (strain)");
+  if (F->periodic) return fail(PCGB_ERR_ARG, "pcgb_fields_nodal: nodal averages on a periodic cell are not implemented");
   const int64_t nn = F->nnodes;
   if (halo && halo->nlocal != 4 * nn)
     return fail(PCGB_ERR_ARG, "pcgb_fields_nodal: the halo plan exchanges %lld entries, the box needs 4 per node (%lld)",
@@ -2658,6 +2721,43 @@ int pcgb_fields_nodal(pcgb_fields_t F, const double *d_x, int kind, pcgb_halo_t 
   if (halo) PCGB_TRY(halo_exchange_add(halo, d_work, st));
   k_fields_divide<<<(unsigned)((nn + 255) / 256), 256, 0, st>>>(nn, d_work, d_out);
   PCGB_CHECK_LAUNCH();
+  return PCGB_OK;
+}
+
+int pcgb_fields_element_periodic(pcgb_fields_t F, const double *d_x, const double strain[6], double *d_strain, double *d_stress,
+                                 double *d_ps, double *d_pe, void *stream) {
+  if (!F || !d_x || !strain) return fail(PCGB_ERR_ARG, "pcgb_fields_element_periodic: null argument");
+  if (!F->periodic) return fail(PCGB_ERR_ARG, "pcgb_fields_element_periodic: the handle is not a periodic cell's");
+  const int64_t ne = F->ne;
+  if (overlap(d_x, F->n, d_strain, 6 * ne) || overlap(d_x, F->n, d_stress, 6 * ne) || overlap(d_x, F->n, d_ps, 3 * ne) ||
+      overlap(d_x, F->n, d_pe, 3 * ne))
+    return fail(PCGB_ERR_ARG, "pcgb_fields_element_periodic: x overlaps an output");
+  return fields_elem(F->s, F->d_E, d_x, d_strain, d_stress, d_ps, d_pe, (cudaStream_t)stream, true, fields_macro(strain));
+}
+
+int pcgb_fields_average(pcgb_fields_t F, const double *d_x, const double strain[6], double out_strain[6], double out_stress[6],
+                        void *stream) {
+  if (!F || !d_x || !strain || !out_strain || !out_stress) return fail(PCGB_ERR_ARG, "pcgb_fields_average: null argument");
+  if (!F->periodic) return fail(PCGB_ERR_ARG, "pcgb_fields_average: the handle is not a periodic cell's");
+  const cudaStream_t st = (cudaStream_t)stream;
+  const int64_t nb = (int64_t)F->s.nbx * F->s.nby * F->s.nbz;
+  double *work = nullptr;   // kFdAvg partials per brick, then the kFdAvg means, for this call only
+  PCGB_CUDA(cudaMallocAsync((void **)&work, (size_t)(kFdAvg * (nb + 1)) * sizeof(double), st));
+  double host[kFdAvg];
+  int rc = fields_average(F->s, fields_macro(strain), F->d_E, d_x, work, work + kFdAvg * nb, st);
+  if (rc == PCGB_OK) {
+    const cudaError_t e = cudaMemcpyAsync(host, work + kFdAvg * nb, sizeof(host), cudaMemcpyDeviceToHost, st);
+    if (e != cudaSuccess) rc = fail(PCGB_ERR_CUDA, "pcgb_fields_average: %s", cudaGetErrorString(e));
+  }
+  const cudaError_t fe = cudaFreeAsync(work, st);
+  const cudaError_t se = cudaStreamSynchronize(st);
+  if (rc != PCGB_OK) return rc;
+  if (fe != cudaSuccess || se != cudaSuccess)
+    return fail(PCGB_ERR_CUDA, "pcgb_fields_average: %s", cudaGetErrorString(fe != cudaSuccess ? fe : se));
+  for (int k = 0; k < 6; ++k) {
+    out_strain[k] = host[k];
+    out_stress[k] = host[6 + k];
+  }
   return PCGB_OK;
 }
 

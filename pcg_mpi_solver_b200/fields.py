@@ -10,6 +10,9 @@ and getNodalPS (pcg_solver.py:730-814) on the boxes `hexmesh` generates (uniform
 
 The arithmetic (centroid Q1 gradient, the stress law of hex_element_stiffness, the invariant-form principal values and
 the fixed nodal summation order) is stated in the header of csrc/fields.cuh and in DESIGN §2.10.
+
+`PeriodicFields(cell, E_field=f)` does the same for a periodic cell (hexmesh.PeriodicCell, DESIGN §2.13) from its
+fluctuation u~ and a macroscopic strain: `element(x, strain)` and the bit-reproducible volume average `average(x, strain)`.
 """
 from __future__ import annotations
 
@@ -19,7 +22,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .hexmesh import HexBlock, _same_device, check_field, interface_node_lists
+from .hexmesh import HexBlock, PeriodicCell, _same_device, check_field, interface_node_lists
 
 ELEMENT_FIELDS = {"strain": 6, "stress": 6, "ps": 3, "pe": 3}
 
@@ -99,5 +102,77 @@ class HexFields:
             if self._halo:
                 lib.pcgb_halo_destroy(self._halo)
                 self._halo = None
+        except Exception:
+            pass
+
+
+def _voigt_strain(strain) -> np.ndarray:
+    e = np.ascontiguousarray(strain, dtype=np.float64)
+    if e.shape != (6,) or not np.isfinite(e).all():
+        raise ValueError(f"PeriodicFields: strain must be 6 finite Voigt components, got {strain!r}")
+    return e
+
+
+class PeriodicFields:
+    """Field recovery of a periodic cell on `device`.  x is the periodic fluctuation u~ (3 ne[0] ne[1] ne[2] dofs, the
+    numbering of hexmesh.generate_periodic_operator) and `strain` the macroscopic strain (Voigt 11, 22, 33, 23, 13, 12 with
+    engineering shears), added to every element's centroid strain.  E_field: as HexFields, kept on the device."""
+
+    def __init__(self, cell: PeriodicCell, device="cuda", E_field=None):
+        self.block = cell
+        self.device = torch.device(device)
+        self.n_elements = cell.n_elements
+        self._E = None
+        if E_field is not None:
+            check_field(E_field, cell, self.device)
+            t = torch.from_numpy(E_field) if isinstance(E_field, np.ndarray) else E_field
+            self._E = t.reshape(-1).to(self.device, torch.float64).contiguous()
+        self._h = ctypes.c_void_p()
+        box = cell.cbox()
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().pcgb_fields_create_periodic(ctypes.byref(box), float(cell.h), float(cell.E), float(cell.nu),
+                                                               _lib.ptr(self._E), ctypes.byref(self._h)), "pcgb_fields_create_periodic")
+
+    def _check_x(self, x: torch.Tensor):
+        if not isinstance(x, torch.Tensor) or x.dtype != torch.float64 or x.dim() != 1 or x.numel() != self.block.n:
+            raise ValueError(f"PeriodicFields: x must be a float64 vector of the cell's {self.block.n} dofs")
+        if x.device.type != "cuda" or not _same_device(x.device, self.device):
+            raise ValueError(f"PeriodicFields: x is on {x.device}, expected {self.device}")
+        return x.contiguous()
+
+    def element(self, x: torch.Tensor, strain, fields=("strain", "stress", "ps", "pe")) -> dict:
+        """HexFields.element's outputs with the macroscopic strain included (strain and stress with tensor shears)."""
+        x = self._check_x(x)
+        e = _voigt_strain(strain)
+        bad = [f for f in fields if f not in ELEMENT_FIELDS]
+        if bad or not fields:
+            raise ValueError(f"PeriodicFields.element: fields must be a non-empty subset of {tuple(ELEMENT_FIELDS)}, got {tuple(fields)}")
+        out = {f: torch.empty((self.n_elements, ELEMENT_FIELDS[f]), dtype=torch.float64, device=self.device) for f in fields}
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().pcgb_fields_element_periodic(self._h, _lib.ptr(x), e.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
+                                                                *(_lib.ptr(out.get(f)) for f in ELEMENT_FIELDS), _lib.stream_ptr()),
+                       "pcgb_fields_element_periodic")
+        return out
+
+    def average(self, x: torch.Tensor, strain):
+        """(<strain>, <stress>): the volume averages over the cell, two float64 numpy arrays of 6 (Voigt, tensor shears),
+        from one element pass and a fixed-order reduction (csrc/fields.cuh), bit-reproducible from run to run."""
+        x = self._check_x(x)
+        e = _voigt_strain(strain)
+        es, ss = np.empty(6), np.empty(6)
+        dp = ctypes.POINTER(ctypes.c_double)
+        with torch.cuda.device(self.device):
+            _lib.check(_lib.load().pcgb_fields_average(self._h, _lib.ptr(x), e.ctypes.data_as(dp), es.ctypes.data_as(dp),
+                                                       ss.ctypes.data_as(dp), _lib.stream_ptr()), "pcgb_fields_average")
+        return es, ss
+
+    def nodal(self, x=None, kind: str = "stress"):
+        raise ValueError("PeriodicFields.nodal: nodal averages on periodic cells are not implemented")
+
+    def __del__(self):
+        try:
+            if self._h:
+                _lib.load().pcgb_fields_destroy(self._h)
+                self._h = ctypes.c_void_p()
         except Exception:
             pass

@@ -105,6 +105,32 @@ class HexBlock:
         return [(self.e0[a], self.e0[a] + self.ne[a]) for a in range(3)]
 
 
+@dataclass
+class PeriodicCell:
+    """A periodic cell of ne[0] x ne[1] x ne[2] hex elements of edge h (homogenisation; DESIGN §2.13): node (lx, ly, lz) is
+    identified with (lx mod ne[0], ly mod ne[1], lz mod ne[2]), so the cell has as many nodes as elements and no clamped
+    dof; dof = 3 node + dir, node = (lz ne[1] + ly) ne[0] + lx.  Every ne must be >= 2 (the library refuses less)."""
+    ne: tuple
+    h: float = 1.0
+    E: float = 1.0
+    nu: float = 0.3
+
+    @property
+    def n_elements(self) -> int:
+        return int(self.ne[0]) * int(self.ne[1]) * int(self.ne[2])
+
+    @property
+    def n(self) -> int:
+        return 3 * self.n_elements
+
+    def cbox(self) -> _lib.HexBox:
+        """The whole-mesh box (e0 = 0, ng = ne) the periodic entry points take."""
+        b = _lib.HexBox()
+        for a in range(3):
+            b.ng[a], b.e0[a], b.ne[a] = int(self.ne[a]), 0, int(self.ne[a])
+        return b
+
+
 def _same_device(a, b) -> bool:
     """torch devices a and b are one device ('cuda' stands for the current CUDA device)."""
     a, b = torch.device(a), torch.device(b)
@@ -218,6 +244,14 @@ def generate_box_operator(block: HexBlock, device="cuda", E_field=None):
     generate_matrix."""
     from .hexop import HexBoxOperator
     return HexBoxOperator(block, device=device, E_field=E_field)
+
+
+def generate_periodic_operator(cell: PeriodicCell, device="cuda", E_field=None):
+    """The index-free operator of a periodic cell (hexop.PeriodicCellOperator): the HexBoxOperator interface, accepted by
+    SubdomainOperator (Jacobi-PCG), refused by multigrid.HexMultigrid.  E_field: as in generate_matrix, shape
+    (ne[2], ne[1], ne[0])."""
+    from .hexop import PeriodicCellOperator
+    return PeriodicCellOperator(cell, device=device, E_field=E_field)
 
 
 def hex_mdf_model(ng, E: float = 1.0, nu: float = 0.3, h: float | None = None, traction: float = 1.0, E_field=None):

@@ -42,7 +42,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .hexmesh import HexBlock, block_field, check_field, field_ck, hex_element_stiffness, interface_lists
+from .hexmesh import HexBlock, PeriodicCell, block_field, check_field, field_ck, hex_element_stiffness, interface_lists
 
 MAX_GATHERED = 1 << 17    # dofs of the largest global box gathered onto every rank (kMgMaxGathered)
 MAX_COARSE = 1536         # dofs of the largest coarsest level (kMgMaxCoarse)
@@ -253,6 +253,10 @@ class HexMultigrid:
 
     def __init__(self, op, block: HexBlock, degree: int = 2, lo: float = 0.25, minv: torch.Tensor | None = None, blocks=None,
                  E_field=None, coarsening: str = "even", coarse: str = "csr"):
+        from .hexop import PeriodicCellOperator
+        if isinstance(getattr(op, "A", None), PeriodicCellOperator) or isinstance(block, PeriodicCell):
+            raise ValueError("HexMultigrid: periodic cells have no multigrid (their coarse levels and singular coarsest level "
+                             "are not built); use Jacobi-PCG")
         self.op, self.block, self.degree, self.lo = op, block, int(degree), float(lo)
         self.n = op.n
         self.device = op.device
